@@ -12,9 +12,13 @@ with fp32 master parameters / fp32 gradients, random-init weights of the referen
 
 Prints ONE JSON line (rank 0).  `value` = pairs/s with inputs resident in HBM (CUDA-event timed, max over ranks);
 `e2e` = the same through the public module API with pinned HOST buffers (prefetched H2D of every step's inputs and
-a D2H read of the loss inside the timed region); `roofline` = the tcgen05 GEMM kernel's achieved TFLOP/s over all of
-its launches in one step (CUDA events around each launch) against MEASURED_PEAKS.json; `cpu_baseline` = the oracle
-timed on this box's host cores on a bounded sample.
+a D2H read of the loss inside the timed region); `roofline` = the wgmma GEMM kernel's achieved TFLOP/s over all of
+its launches in one step (CUDA events around each launch) against MEASURED_PEAKS.json when present, else the H100 SXM
+data-sheet figure; `cpu_baseline` = the oracle timed on the host cores on a bounded sample.
+
+`--dump-outputs DIR` writes what the last timed step returned to its caller as float32 .npy files: the loss, both
+feature matrices and a fixed, seeded sample of every parameter gradient.  Inputs and weights are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -45,11 +49,11 @@ def measured_peaks():
             p = json.load(f)
         return {"tflops": float(p.get("bf16_tflops_sustained", p.get("bf16_tflops"))), "hbm_gbs": float(p["hbm_gbs"]),
                 "source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"}
-    return {"tflops": 1400.0, "hbm_gbs": 6650.0, "source": "B200_PROFILING.md fallback, sustained (of fallback)"}
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (dense bf16, HBM3), not measured"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -104,8 +108,8 @@ def run_ours(args):
     from xpretrain_b200.utils import distributed as xdist
 
     # N > 1, optional (XP_SM_RESERVE=n, default 0): cap NCCL at n CTAs and leave n SMs out of every backward GEMM grid so that the
-    # overlapped gradient all-reduce never displaces a persistent GEMM CTA.  Measured: +2.8 % at 2 GPUs, but -2.6 % at 8 GPUs, where
-    # the thinner all-reduce (1.75x the bytes per rank) exposes its tail (profiles/r02_bench_n8_*.json) — hence off by default.
+    # overlapped gradient all-reduce never displaces a persistent GEMM CTA.  Off by default: at 8 GPUs the thinner all-reduce
+    # (1.75x the bytes per rank) can expose its tail.
     reserve = int(os.environ.get("XP_SM_RESERVE", "0")) if int(os.environ.get("WORLD_SIZE", "1")) > 1 else 0
     if reserve > 0:
         os.environ.setdefault("NCCL_MAX_CTAS", str(reserve))
@@ -142,12 +146,15 @@ def run_ours(args):
         host.append((v, ids.pin_memory(), torch.ones(B, Lt, dtype=torch.long).pin_memory()))
     resident = [tuple(t.to(dev) for t in h) for h in host]
 
+    last_out = {}
+
     def step(video, ids, mask):
         for p in params:
             p.grad = None
         out = model(video=video, text_input_ids=ids, text_input_mask=mask)
         loss = gather_nce_loss(out["vis_features"], out["text_features"], model.clipmodel.logit_scale)
         loss.backward()
+        last_out.update(loss=loss, vis=out["vis_features"], txt=out["text_features"])
         return loss
 
     def barrier():
@@ -178,6 +185,8 @@ def run_ours(args):
     ms_resident = timed(lambda i: step(*resident[i % n_host]), args.steps)
     launches = ops.launch_count()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out, model)
 
     # ---- e2e: host buffers -> prefetched H2D on a side stream (the reference's PrefetchLoader pattern,
     #      dataloader.py:92-157) -> module API -> loss.item() (D2H) every step
@@ -238,7 +247,7 @@ def run_ours(args):
         host[:] = host_f32
         del host_u8
 
-    # ---- roofline of the dominant kernel (the tcgen05 GEMM): CUDA events around every launch of one step
+    # ---- roofline of the dominant kernel (the wgmma GEMM): CUDA events around every launch of one step
     roof = None
     # per-launch / per-block CUDA-event timings below are taken with the text tower and the bias column sums on the MAIN stream:
     # kernels that overlap on side streams would be charged each other's time
@@ -253,10 +262,9 @@ def run_ours(args):
         g_flops = sum(f for (f, _, _) in rec)
         peaks = measured_peaks()
         achieved = g_flops / (g_ms * 1e-3) / 1e12 if g_ms > 0 else 0.0
-        roof = {"kernel": "xp::gemm_kernel (tcgen05 bf16, all launches of one step)", "bound": "tensor",
+        roof = {"kernel": "xp::gemm_kernel (wgmma bf16, all launches of one step)", "bound": "tensor",
                 "achieved": round(achieved, 1), "peak": peaks["tflops"], "unit": "TFLOP/s",
-                "frac": round(achieved / peaks["tflops"], 4), "traffic": ncu_traffic()[0],
-                "traffic_of": ncu_traffic()[1], "peak_source": peaks["source"],
+                "frac": round(achieved / peaks["tflops"], 4), "peak_source": peaks["source"],
                 "launches_per_step": len(rec), "gemm_ms_per_step": round(g_ms, 3),
                 "gemm_share_of_step": round(g_ms / ms_resident, 4)}
 
@@ -301,7 +309,7 @@ def run_ours(args):
         torch.cuda.synchronize()
         n_par = sum(p.numel() for p in params)
         o_ms = o0.elapsed_time(o1) / 5
-        hbm = measured_peaks().get("hbm_gbs", 6576.4)
+        hbm = measured_peaks()["hbm_gbs"]
         # a complete training step: fwd (incl. the per-forward fp32 -> bf16 weight re-cast) + gather + loss + bwd + clip + AdamW
         for _ in range(2):
             step(*resident[0]); opt.step(max_grad_norm=5.0)
@@ -339,7 +347,7 @@ def run_ours(args):
                                f"{' + DP grad all-reduce' if world > 1 else ''}",
                    "global_batch": pairs, "frames": T, "tokens": Lt, "parallelism": f"dp{world}",
                    "sm_reserve_for_nccl": reserve, "grad_allreduce_dtype": os.environ.get("XP_GRAD_COMM", "fp32") if world > 1 else None,
-                   "l2": "inputs (462 MB video + 40 GB activations per step) far exceed the 126 MB L2",
+                   "l2": "inputs (462 MB video + 40 GB activations per step) far exceed the 50 MB L2",
                    "weights": "random init with the reference's init statistics, fp32 masters, bf16 compute copies"},
         "e2e": {"value": round(e2e_value, 2), "unit": UNIT, "ms_per_step": round(ms_e2e, 3),
                 "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "last_loss": last["loss"]},
@@ -365,18 +373,26 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
-def ncu_traffic():
-    """(dram__bytes_read + dram__bytes_write of one captured GEMM launch, what that launch was) from the committed ncu capture
-    profiles/r02_ncu_gemm_traffic.json (a property of that capture, not of this run); (None, None) when none is committed."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r02_ncu_gemm_traffic.json")
-    try:
-        with open(path) as f:
-            d = json.load(f)
-        return d["traffic_bytes"], {"algorithmic_bytes": d["algorithmic_bytes"]["total"],
-                                    "launch": f"{d['kernel']} M={d['shape']['M']} N={d['shape']['N']} K={d['shape']['K']}",
-                                    "source": "profiles/r02_ncu_gemm_traffic.json (one ncu --set full capture of this kernel, not of this run)"}
-    except (OSError, KeyError, ValueError):
-        return None, None
+GRAD_SAMPLE = 4096      # gradient elements dumped per parameter tensor (all of them for smaller tensors)
+
+
+def dump_outputs(out_dir, last_out, model):
+    """The last timed step's results as float32 .npy files under out_dir (a few MB in all)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": last_out["loss"].detach().reshape(1), "vis_features": last_out["vis"].detach(),
+              "text_features": last_out["txt"].detach()}
+    g = torch.Generator().manual_seed(0)
+    parts = []
+    for _, p in model.named_parameters():
+        flat = p.grad.detach().reshape(-1) if p.grad is not None else torch.zeros(p.numel(), device=p.device)
+        if flat.numel() > GRAD_SAMPLE:
+            flat = flat[torch.randint(flat.numel(), (GRAD_SAMPLE,), generator=g).to(flat.device)]
+        parts.append(flat)
+    arrays["grad_sample"] = torch.cat(parts)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.float().cpu().numpy())
 
 
 # -------------------------------------------------------------------------------- reference / CPU arm
@@ -453,7 +469,7 @@ def run_reference(args):
 
 def gpu_eager_baseline(dev, batch):
     """north_star's 1-GPU bar, measured by the same run: the reference algorithm (oracle port: the same torch ops in the same
-    order as CLIP_ViP.py / loss.py) in PyTorch eager on THIS B200 under bf16 autocast (`.to(bf16)` crashes in the reference,
+    order as CLIP_ViP.py / loss.py) in PyTorch eager on THIS GPU under bf16 autocast (`.to(bf16)` crashes in the reference,
     SURVEY.md §8c), fwd + InfoNCE + bwd, 2 warm-up + 3 timed steps; falls back to a smaller batch when eager runs out of memory."""
     import torch
     from oracle import clipvip_oracle as O
@@ -686,7 +702,7 @@ def run_encoder(args):
                     "h2d_bytes_per_step": x_host.numel() * x_host.element_size(), "d2h_bytes_per_step": 4,
                     "last_loss": last.get("loss")},
             "gpu_launches": int(launches * world), "clocks": clocks,
-            "roofline": {"kernel": "xp::gemm_kernel (tcgen05 bf16, all launches of one step)", "bound": "tensor",
+            "roofline": {"kernel": "xp::gemm_kernel (wgmma bf16, all launches of one step)", "bound": "tensor",
                          "achieved": round(ach, 1), "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": round(ach / peaks["tflops"], 4),
                          "traffic": None, "peak_source": peaks["source"], "launches_per_step": len(rec),
                          "gemm_ms_per_step": round(g_ms, 3), "gemm_share_of_step": round(g_ms / ms_res, 4)},
@@ -710,7 +726,11 @@ def main():
                     help="clipvip = BASELINE.json configs[1]/[2] (default, the headline); timesformer = configs[3] (HD-VILA "
                          "spatio-temporal encoder); swin3d = configs[4] (LF-VILA Swin-3D video encoder)")
     ap.add_argument("--no-eager", action="store_true", help="skip the gpu_eager_baseline leg (N = 1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (loss, features, sampled gradients) as float32 .npy files")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "clipvip"):
+        ap.error("--dump-outputs applies to the CLIP-ViP workload of this implementation (--impl ours --workload clipvip)")
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "clipvip":

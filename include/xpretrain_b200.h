@@ -1,5 +1,5 @@
 /*
- * xpretrain_b200 — C ABI of the B200-native CLIP-ViP / HD-VILA hot path.
+ * xpretrain_b200 — C ABI of the H100-native CLIP-ViP / HD-VILA hot path.
  *
  * The reference (microsoft/XPretrain) is 100 % Python: it has no FFI or
  * plugin boundary for this path, so the seam a maintainer binds is the set of
@@ -10,7 +10,7 @@
  *   - `stream` is a cudaStream_t passed as void*;
  *   - bf16 = __nv_bfloat16 bits, f32 = IEEE float, i64 = int64_t;
  *   - return 0 on success, negative on error; xp_last_error() gives the text.
- *     There is no CPU fallback: without a B200 every call fails loudly.
+ *     There is no CPU fallback: without an H100 (sm_90a) every call fails loudly.
  */
 #ifndef XPRETRAIN_B200_H
 #define XPRETRAIN_B200_H
@@ -31,7 +31,7 @@ int64_t xp_launch_count(void);
 void xp_launch_count_reset(void);
 
 /* ------------------------------------------------------------------ GEMM --
- * C[M,N] = epilogue( alpha * sum_k A[m,k] * B[n,k] )      (tcgen05 / TMEM / TMA)
+ * C[M,N] = epilogue( alpha * sum_k A[m,k] * B[n,k] )      (wgmma / TMA)
  * Replaces every nn.Linear on the path and its autograd:
  *   forward  y = x W^T + b         CLIP_ViP.py:341-343,379 (q/k/v/out_proj), :393-395 (fc1/fc2),
  *                                   :1141-1145 (visual/text projection), :178 (patch conv as im2col GEMM)
@@ -67,7 +67,7 @@ typedef struct XpGemm {
   int64_t c_group, c_group_stride, r_group, r_group_stride;
   int32_t block_n;    /* 0 = auto, else 128 or 256 */
   int32_t max_ctas;   /* 0 = one persistent CTA per SM */
-  int32_t cta_pair;   /* 0 = auto (2-CTA cta_group::2 pairs on 256x256 tiles when M, N >= 256), 1 = never, 2 = force */
+  int32_t cta_pair;   /* 0 or 1: single-CTA tiles (sm_90 has no CTA pairs; other values are rejected) */
   int32_t reserved;
 } XpGemm;
 
@@ -159,26 +159,11 @@ int xp_eos_offsets(const int64_t* ids, int64_t* offsets, int32_t* index, int32_t
 int64_t xp_vip_attention_workspace_bytes(int32_t B, int32_t H, int32_t T, int32_t M);
 int xp_vip_attention_fwd(const void* qkv, void* out, float* lse, float* workspace, int32_t B, int32_t H, int32_t T,
                          int32_t L, int32_t M, int32_t C, void* stream);
-/* Same contract, tcgen05/TMEM kernel (S and P·V on the 5th-gen tensor cores, softmax thread-per-TMEM-lane). */
-int xp_vip_attention_fwd_tc(const void* qkv, void* out, float* lse, float* workspace, int32_t B, int32_t H, int32_t T,
-                            int32_t L, int32_t M, int32_t C, void* stream);
-/* First half of the above (frame rows + per-frame partials of the global rows, before the combine step). */
-int xp_vip_attention_fwd_tc_partial(const void* qkv, void* out, float* lse, float* workspace, int32_t B, int32_t H,
-                                    int32_t T, int32_t L, int32_t M, int32_t C, void* stream);
 /* dqkv bf16 [B*S, 3C] = gradient w.r.t. the (un-scaled-q) projection outputs, i.e. the dq part already carries
  * q_scale (CLIP_ViP.py:341), so the QKV dgrad/wgrad GEMMs treat the three thirds uniformly. */
 int xp_vip_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                          float* workspace, int32_t B, int32_t H, int32_t T, int32_t L, int32_t M, int32_t C,
                          float q_scale, void* stream);
-
-/* tcgen05/TMEM backward: S, dP, dV, dK, dQ on the 5th-gen tensor cores.  delta f32 [B, H, S] is scratch that
- * receives rowsum(dout * out). */
-int xp_vip_attention_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
-                            float* workspace, float* delta, int32_t B, int32_t H, int32_t T, int32_t L, int32_t M,
-                            int32_t C, float q_scale, void* stream);
-int xp_vip_attention_bwd_tc_partial(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
-                                    float* workspace, float* delta, int32_t B, int32_t H, int32_t T, int32_t L,
-                                    int32_t M, int32_t C, float q_scale, void* stream);
 
 /* ------------------------------------------------------- text-tower attention --
  * CLIPAttention.forward (CLIP_ViP.py:266-330) between the QKV projection and out_proj, with the causal mask
@@ -203,7 +188,7 @@ int xp_nce_softmax_grad(const float* z, const float* logit_scale, float* lse_row
 /* Fused exchange + loss: replaces `hvd.allgather(vis)`, `hvd.allgather(txt)` (CLIP-ViP/src/pretrain/run_pretrain.py:344-345;
  * rank-major concat, semantics pinned by LF-VILA/src/utils/dist.py:21-41) AND NCELearnableTempLoss.forward (loss.py:134-141)
  * with ONE cooperative kernel (csrc/nce_fused.cu): device-side flag barrier over peer-mapped exchange buffers, logits tiles
- * on tcgen05 whose operand rows are loaded straight from the owning peer's memory over NVLink (hi/lo split in the producer),
+ * on wgmma whose operand rows are loaded straight from the owning peer's memory over NVLink (hi/lo split in the producer),
  * row/column log-sum-exps, loss (overwritten), d logit_scale (overwritten), g_scaled bf16 [N, ld_g] = exp(logit_scale)*dL/dZ,
  * and the bf16 copies vis_hi / txt_hi [N, d] that the local gradient GEMMs use.  N = world * b <= 1536.
  *   mode 0: peer_bufs = device array of `world` exchange-buffer base pointers (own buffer at [rank]); every buffer is

@@ -3,7 +3,7 @@ gradient clipping + warm-up/decay learning-rate schedule + parameter grouping).
 
 TEST INFRASTRUCTURE ONLY — never imported by the product package.
 
-Restates (file:line under /root/reference/CLIP-ViP/src):
+Restates (file:line under the reference's CLIP-ViP/src):
   optimization/adamw.py:40-103    AdamW.step: m, v EMAs; denom = sqrt(v) + eps (eps OUTSIDE the bias correction);
                                   step_size = lr * sqrt(1 - b2^t) / (1 - b1^t); p -= step_size * m / denom; THEN the
                                   decoupled decay p -= lr * wd * p (on the already updated p, with the uncorrected lr)

@@ -7,8 +7,8 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline /
 `--impl reference` legs may import this module; the product path under
 `xpretrain_b200/` never does.
 
-Parity pinned: `tests/golden/make_golden.py` (run in the authoring container,
-where /root/reference exists) checks every function here against the
+Parity pinned: `tests/golden/make_golden.py` (run against a checkout of the
+reference named by XP_REFERENCE_ROOT) checks every function here against the
 reference's own modules (CLIP-ViP/src/modeling/CLIP_ViP.py,
 CLIP-ViP/src/optimization/loss.py) to fp32 round-off and writes the golden
 vectors that `tests/test_oracle_golden.py` replays on any machine.

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY — imported by tests/, tests/golden/make_golden_swin3d.py and tools/; never by the product package.
 
-A functional fp32 PyTorch restatement of /root/reference/LF-VILA/src/models/video_encoder.py (eval mode, or training mode with
+A functional fp32 PyTorch restatement of the reference's LF-VILA/src/models/video_encoder.py (eval mode, or training mode with
 explicit DropPath factors).  Parity pinned by tests/golden/make_golden_swin3d.py against the reference's own `SwinTransformer3D`
 (imported with stub `timm` / `mmcv` modules): forward and every parameter gradient to fp32 round-off.
 

@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE ONLY — imported by tests/, tests/golden/make_golden_timesformer.py and tools/ (baseline timing);
 the product package never imports it.
 
-A functional fp32 PyTorch restatement of `/root/reference/hd-vila/src/modeling/timesformer.py` (eval mode / DropPath
+A functional fp32 PyTorch restatement of the reference's `hd-vila/src/modeling/timesformer.py` (eval mode / DropPath
 inactive: SURVEY.md §8c).  Parity pinned: tests/golden/make_golden_timesformer.py loads these seeded weights into the
 reference's own `TimeSformer`, asserts agreement to fp32 round-off (forward and every parameter gradient) and writes
 tests/golden/timesformer_*.pt.

@@ -1,14 +1,14 @@
 """Generate the golden vectors under tests/golden/ from the REAL reference.
 
-Runs only in the authoring container, where /root/reference (microsoft/XPretrain) is mounted:
+Needs a checkout of the reference (microsoft/XPretrain), named by XP_REFERENCE_ROOT:
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    XP_REFERENCE_ROOT=<path to XPretrain> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
 It imports the reference's own modules (CLIP-ViP/src/modeling/CLIP_ViP.py, src/optimization/loss.py)
 unmodified, loads the oracle's deterministic synthetic weights into them, runs forward / loss /
 backward in fp32 on CPU, (1) asserts that oracle/clipvip_oracle.py reproduces the reference to fp32
 round-off — this is what pins the oracle — and (2) writes small .pt fixtures that
-tests/test_oracle_golden.py (CPU) and tests/test_gpu_parity.py (B200) replay without the reference.
+tests/test_oracle_golden.py (CPU) and tests/test_gpu_parity.py (GPU) replay without the reference.
 No reference source is copied; only numeric outputs are stored.
 """
 import os
@@ -20,7 +20,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("XP_REFERENCE_ROOT", "/root/reference")
+REF = os.environ["XP_REFERENCE_ROOT"]
 sys.path.insert(0, os.path.join(REF, "CLIP-ViP"))
 sys.dont_write_bytecode = True
 
@@ -65,6 +65,23 @@ ROW_GRAD_KEYS = {"vision_model.encoder.layers.0.mlp.fc1.weight": 512, "vision_mo
 def _pack_f16(g):
     s = float(g.abs().max().clamp_min(1e-30))
     return {"scale": s, "data": (g / s).to(torch.float16)}
+
+
+GRAD_SAMPLE_ELEMS = 12288     # per whole-gradient entry: a seeded sample of whole rows keeps the fixture under 1 MB
+
+
+def sample_rows(candidates, row_numel):
+    """A fixed, seeded subset (sorted) of the row indices `candidates`, about GRAD_SAMPLE_ELEMS elements in all."""
+    k = max(1, min(len(candidates), GRAD_SAMPLE_ELEMS // row_numel))
+    pick = torch.randperm(len(candidates), generator=torch.Generator().manual_seed(0))[:k]
+    return candidates[pick.sort().values]
+
+
+def pack_rows(g, candidates):
+    """A row sample of g[candidates], normalised by the max over ALL candidate rows (the scale of the whole entry)."""
+    rows = sample_rows(candidates, g[0].numel())
+    s = float(g[candidates].abs().max().clamp_min(1e-30))
+    return {"rows": rows, "scale": s, "data": (g[rows] / s).to(torch.float16)}
 
 
 def run_case(name, cfg, B, T, Lt, ragged, weight_seed, data_seed, with_hidden, full_grads=False):
@@ -115,17 +132,17 @@ def run_case(name, cfg, B, T, Lt, ragged, weight_seed, data_seed, with_hidden, f
                                                  "vision_model.embeddings.position_embedding"))},
     }
     if full_grads:
-        full = {k: _pack_f16(grads[k]) for k in FULL_GRAD_KEYS}
+        full = {k + "[rows]": pack_rows(grads[k], torch.arange(grads[k].shape[0])) for k in FULL_GRAD_KEYS}
         for k, n in ROW_GRAD_KEYS.items():
-            full[k + f"[:{n}]"] = _pack_f16(grads[k][:n])
+            full[k + "[rows]"] = pack_rows(grads[k], torch.arange(n))
         tk = "text_model.embeddings.token_embedding.weight"
         rows = torch.unique(ids)
-        full[tk + "[rows]"] = {"rows": rows, **_pack_f16(grads[tk][rows])}
+        full[tk + "[rows]"] = pack_rows(grads[tk], rows)
         rest = grads[tk].clone()
         rest[rows] = 0
         assert float(rest.abs().max()) == 0.0                                        # untouched rows: exactly zero
         gold["grad_full"] = full
-        gold["grad_vectors"] = {k: g.clone() for k, g in grads.items() if g.dim() <= 1 or g.numel() <= 4096}
+        gold["grad_vectors"] = {k: _pack_f16(g) for k, g in grads.items() if g.dim() <= 1 or g.numel() <= 4096}
     if with_hidden:
         vh = out["vision_model_output"].hidden_states
         th = out["text_model_output"].hidden_states

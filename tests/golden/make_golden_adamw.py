@@ -1,13 +1,13 @@
 """Golden vectors for the optimizer step (SURVEY.md §8(f).1) from the REAL reference.
 
-Runs only in the authoring container (needs /root/reference):
+Needs a checkout of the reference, named by XP_REFERENCE_ROOT:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_adamw.py
 
 Drives the reference's own `AdamW` (optimization/adamw.py), `build_e2e_optimizer_w_lr_mul` (optimization/utils.py),
 `get_lr_sched` (optimization/sched.py) and torch's `clip_grad_norm_` exactly as run_pretrain.py:388-423 does, for a few
 steps on a small named parameter set, asserts oracle/adamw_oracle.py reproduces every tensor bit-for-bit, and stores the
-trajectory (no reference source) for tests/test_oracle_golden.py (CPU) and tests/test_gpu_optim.py (B200).
+trajectory (no reference source) for tests/test_oracle_golden.py (CPU) and tests/test_gpu_optim.py (GPU).
 """
 import os
 import sys
@@ -18,7 +18,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("XP_REFERENCE_ROOT", "/root/reference")
+REF = os.environ["XP_REFERENCE_ROOT"]     # a checkout of microsoft/XPretrain
 sys.path.insert(0, os.path.join(REF, "CLIP-ViP"))
 sys.dont_write_bytecode = True
 

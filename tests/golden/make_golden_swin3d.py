@@ -1,6 +1,6 @@
 """Golden vectors for BASELINE.json config #5 (LF-VILA Swin-3D video encoder) from the REAL reference.
 
-Runs only in the authoring container (needs /root/reference):
+Needs a checkout of the reference, named by XP_REFERENCE_ROOT:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_swin3d.py
 
@@ -19,7 +19,7 @@ import torch.nn as nn
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("XP_REFERENCE_ROOT", "/root/reference")
+REF = os.environ["XP_REFERENCE_ROOT"]     # a checkout of microsoft/XPretrain
 sys.dont_write_bytecode = True
 
 from oracle import swin3d_oracle as O  # noqa: E402

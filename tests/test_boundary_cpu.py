@@ -66,8 +66,8 @@ def test_wgrad_plan_fills_waves():
     from xpretrain_b200.ops import wgrad_plan
     for n_out, n_in in [(3072, 768), (768, 3072), (2304, 768), (768, 768)]:
         bn, s = wgrad_plan(n_out, n_in, 150784)
-        tiles = ((n_out + 255) // 256) * ((n_in + 255) // 256) * s        # CTA pairs: 256 x 256 tiles on 74 clusters
-        assert tiles / (-(-tiles // 74) * 74) > 0.9
+        tiles = ((n_out + 127) // 128) * ((n_in + bn - 1) // bn) * s       # 128 x block_n tiles on the 132 SMs of an H100
+        assert tiles / (-(-tiles // 132) * 132) > 0.9
 
 
 def test_timesformer_module_has_the_reference_state_dict():

@@ -1,4 +1,4 @@
-"""B200: the rest of the drop-in boundary (SURVEY.md §8b / VERDICT r1 items a12, a13, b):
+"""H100: the rest of the drop-in boundary (SURVEY.md §8b / VERDICT r1 items a12, a13, b):
 `forward_video` / `forward_text` / `get_*_features(if_norm)` (VidCLIP.py:83-90, CLIP_ViP.py:992-1085),
 `freeze_text_encoder` (VidCLIP.py:92-103), and the contract that a weight written IN PLACE through `p.data` — the idiom
 of the reference's own AdamW (CLIP-ViP/src/optimization/adamw.py:89,101), which autograd's version counter does not see —
@@ -14,7 +14,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def dev():
     if not torch.cuda.is_available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     return torch.device("cuda", 0)
 
 

@@ -1,4 +1,4 @@
-"""B200: retrieval evaluation kernels (SURVEY.md §8f.3) vs the reference golden and the numpy oracle."""
+"""H100: retrieval evaluation kernels (SURVEY.md §8f.3) vs the reference golden and the numpy oracle."""
 import os
 
 import numpy as np
@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "these tests need the B200"
+    assert torch.cuda.is_available(), "these tests need the H100"
     return torch.device("cuda", 0)
 
 

@@ -1,4 +1,4 @@
-"""B200: the fused optimizer step (SURVEY.md §8(f).1) against the reference trajectory golden and the oracle."""
+"""H100: the fused optimizer step (SURVEY.md §8(f).1) against the reference trajectory golden and the oracle."""
 import os
 
 import pytest
@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "these tests need the B200"
+    assert torch.cuda.is_available(), "these tests need the H100"
     return torch.device("cuda", 0)
 
 

@@ -1,4 +1,4 @@
-"""B200: the CUDA path (VidCLIP module -> C ABI kernels) against the CPU oracle and the golden vectors that were
+"""H100: the CUDA path (VidCLIP module -> C ABI kernels) against the CPU oracle and the golden vectors that were
 generated from the real reference (tests/golden/make_golden.py).
 
 Tolerances (bf16 compute, fp32 oracle).  BASELINE.md §3 calibrates what bf16 costs the REFERENCE ITSELF
@@ -14,9 +14,9 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-# Small-golden bars.  Calibrated on this pool's B200 (profiles/r02_pytest_gpu_parity_v2_fp32_residual.log): the reference's own
-# bf16-autocast run deviates from its fp32 output by 3.8e-3 (video) / 7.7e-3 (text) at full depth; ours by 3.6e-3 / 7.3e-3.
-EMB_REL_L2 = 1.2e-2      # 1.5 x the reference's bf16 deviation of the text tower (the larger one)
+# Small-golden bars, set from the deviation of the reference's own bf16-autocast run from its fp32 output at full depth
+# (the full-depth tests below measure that deviation on the GPU they run on and calibrate against it).
+EMB_REL_L2 = 1.2e-2      # about 1.5 x the reference's bf16 deviation of the text tower (the larger one)
 ROW_COSINE = 1.0 - 1e-3
 LOSS_REL = 1e-2          # a 2..4-pair loss at logit scale ~100 is one sample of the logits error (see _assert_calibrated)
 GRAD_COSINE = 0.97
@@ -25,7 +25,7 @@ GRAD_COSINE = 0.97
 @pytest.fixture(scope="module")
 def dev():
     if not torch.cuda.is_available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     return torch.device("cuda", 0)
 
 
@@ -125,7 +125,8 @@ def _errors_vs_full_golden(gold, vis, txt, loss, grads):
         else:
             got = grads[k]
         e["d " + k] = _rel(got, want)
-    vec = [(k, g) for k, g in gold["grad_vectors"].items() if float(g.norm()) > 1e-3 * gold["grad_norms"]["logit_scale"] and "k_proj.bias" not in k]
+    vec = [(k, _unpack(e)) for k, e in gold["grad_vectors"].items()]
+    vec = [(k, g) for k, g in vec if float(g.norm()) > 1e-3 * gold["grad_norms"]["logit_scale"] and "k_proj.bias" not in k]
     e["d vectors (worst)"] = max(_rel(grads[k], g) for k, g in vec)
     e["d vectors (median)"] = sorted(_rel(grads[k], g) for k, g in vec)[len(vec) // 2]
     return e
@@ -136,8 +137,9 @@ CALIBRATION = 1.5      # ours may deviate from the fp32 reference by at most 1.5
 
 def _full12_case(dev, golden_dir, pad_to):
     """T = 12, 12 + 12 layers, ragged text — the BENCH model — against the golden made from the real reference
-    (tests/golden/make_golden.py full12): full-tensor relative L2 of the features, the logits matrix and twelve whole
-    weight-gradient tensors (+ all bias / LayerNorm gradient vectors), each CALIBRATED against the deviation the reference
+    (tests/golden/make_golden.py full12): relative L2 of the features, the logits matrix, a fixed seeded sample of whole rows
+    (~12 k elements each) of fifteen weight-gradient tensors and all bias / LayerNorm gradient vectors, each CALIBRATED
+    against the deviation the reference
     algorithm itself shows in bf16 on the same inputs on this GPU (autocast and all-bf16), not against a hand-set number.
     With pad_to = 64 the golden batch occupies rows 0..3 of a 64-pair batch (BASELINE.json configs[1]'s per-GPU batch):
     the loss is taken on those rows only, so every gradient must still equal the reference's."""
@@ -177,9 +179,8 @@ def _full12_case(dev, golden_dir, pad_to):
 def _assert_calibrated(ours, ref):
     """Full tensors (features, logits matrix, whole gradient tensors): our deviation from the fp32 reference golden may be at
     most CALIBRATION = 1.5 x the deviation of the REFERENCE's own bf16 path (autocast: fp32 residual stream, bf16 matmul inputs)
-    on the same inputs on this GPU — tighter than SURVEY.md §8c's 2x.  Measured (profiles/r02_pytest_gpu_parity_v2_fp32_residual.log):
-    features 0.95x, logits 1.24x, gradients 0.93x - 1.29x.  With `residual_fp32=False` (round-1 bf16 stream) the features sit at
-    2.4x and only the all-bf16 bar holds, which is why the fp32 stream is the default."""
+    on the same inputs on this GPU — tighter than SURVEY.md §8c's 2x.  With `residual_fp32=False` (bf16 residual stream) only
+    the all-bf16 bar holds, which is why the fp32 stream is the default."""
     import os
     against = "pure" if os.environ.get("XP_RESIDUAL_BF16") == "1" else "autocast"
     for k in ours:

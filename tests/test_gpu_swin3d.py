@@ -1,4 +1,4 @@
-"""B200: BASELINE.json config #5 (LF-VILA Swin-3D video encoder) — kernels and module against the oracle and the reference goldens."""
+"""H100: BASELINE.json config #5 (LF-VILA Swin-3D video encoder) — kernels and module against the oracle and the reference goldens."""
 import os
 
 import pytest
@@ -21,7 +21,7 @@ def _cos(a, b):
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "these tests need the B200"
+    assert torch.cuda.is_available(), "these tests need the H100"
     return torch.device("cuda", 0)
 
 

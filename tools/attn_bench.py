@@ -1,5 +1,5 @@
 """Time the proxy-token attention kernels alone at the BENCH shape (B = 64, 12 heads, 12 frames, 196 + 4 tokens):
-tcgen05 forward, mma.sync backward (round 1's hot path) and the pipelined tcgen05 backward.  CUDA events on the
+TMA + wgmma forward and backward.  CUDA events on the
 launching stream, L2 flushed between iterations.  FLOPs: 1.474 GFLOP forward per (sample, layer) (SURVEY.md §8d), x2.5 backward."""
 import json
 import sys
@@ -19,9 +19,7 @@ qkv[:, :C] *= 0.35
 out = torch.empty(B * S, C, dtype=bf16, device=dev)
 dout = torch.randn(B * S, C, generator=g).to(dev).to(bf16)
 lse = torch.empty(B, H, S, device=dev)
-delta = torch.empty(B, H, S, device=dev)
 dqkv = torch.empty(B * S, 3 * C, dtype=bf16, device=dev)
-dqkv2 = torch.empty_like(dqkv)
 ws = ops.vip_attention_workspace(B, H, T, M, dev)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
@@ -42,12 +40,9 @@ def timeit(fn, iters=10):
 
 f_fwd = 1.474e9 * B
 res = {}
-res["fwd_tc_ms"] = timeit(lambda: ops.vip_attention_fwd_tc(qkv, out, lse, ws, B, H, T, L, M, C))
-res["bwd_mma_ms"] = timeit(lambda: ops.vip_attention_bwd(qkv, out, dout, lse, dqkv, ws, B, H, T, L, M, C, 0.125))
-res["bwd_tc_ms"] = timeit(lambda: ops.vip_attention_bwd_tc(qkv, out, dout, lse, dqkv2, ws, delta, B, H, T, L, M, C, 0.125))
-res["fwd_tc_tflops"] = f_fwd / res["fwd_tc_ms"] / 1e9
-res["bwd_mma_tflops"] = 2.5 * f_fwd / res["bwd_mma_ms"] / 1e9
-res["bwd_tc_tflops"] = 2.5 * f_fwd / res["bwd_tc_ms"] / 1e9
-res["bwd_tc_vs_mma_rel_l2"] = float((dqkv2.float() - dqkv.float()).norm() / dqkv.float().norm())
+res["fwd_ms"] = timeit(lambda: ops.vip_attention_fwd(qkv, out, lse, ws, B, H, T, L, M, C))
+res["bwd_ms"] = timeit(lambda: ops.vip_attention_bwd(qkv, out, dout, lse, dqkv, ws, B, H, T, L, M, C, 0.125))
+res["fwd_tflops"] = f_fwd / res["fwd_ms"] / 1e9
+res["bwd_tflops"] = 2.5 * f_fwd / res["bwd_ms"] / 1e9
 res["shape"] = dict(B=B, H=H, T=T, L=L, M=M)
 print(json.dumps(res))

@@ -1,7 +1,7 @@
 """PyTorch-eager GPU baseline for the bench workload (BASELINE.md §3 "same-box GPU eager baseline").
 
-The reference itself (/root/reference) does not exist on the GPU box, so this times its pinned restatement
-(oracle/clipvip_oracle.py: the same torch ops in the same order as CLIP_ViP.py / loss.py) on the B200 under
+The reference itself is not needed on the GPU machine: this times its pinned restatement
+(oracle/clipvip_oracle.py: the same torch ops in the same order as CLIP_ViP.py / loss.py) on the H100 under
 torch.autocast(bfloat16) — the reference cannot run `.to(bfloat16)` (SURVEY.md §8c), autocast is its working
 bf16 mode.  fwd + InfoNCE + bwd, CUDA-event timed, B = 64 (falls back to 32 / 16 if eager runs out of memory).
 This is a measurement tool (it executes oracle/ on purpose); nothing in the product imports it.

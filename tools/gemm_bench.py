@@ -1,4 +1,4 @@
-"""Time the tcgen05 GEMM on the ViP layer shapes at B = 64 (M = 150784): QKV, out-proj, fc1 + QuickGELU (two outputs), fc2,
+"""Time the wgmma GEMM on the ViP layer shapes at B = 64 (M = 150784): QKV, out-proj, fc1 + QuickGELU (two outputs), fc2,
 dgrad(fc2) + dQuickGELU, dgrad(fc1), wgrad(fc1).  CUDA events, L2 flushed between iterations.  XP_GEMM_DEBUG=1 turns the
 epilogue stores off (profiling: how much of a launch is the store traffic)."""
 import json

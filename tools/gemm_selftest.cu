@@ -72,8 +72,6 @@ __global__ void ref_gemm(const __nv_bfloat16* A, const __nv_bfloat16* B, float* 
   C[(long)m * N + n] = v;
 }
 
-static int g_cta_pair = 0;  // 0 auto, 1 single-CTA kernel only, 2 force CTA pairs
-
 struct Case {
   const char* name;
   int M, N, K, a_layout, b_layout, act, out, splits, bn;
@@ -125,7 +123,7 @@ static int run_case(const Case& c, bool timing) {
   g.scale_cols = c.qscale ? (c.N / 3 / 8 * 8) : 0;
   g.alpha = alpha; g.col_scale = 0.125f;
   g.block_n = c.bn;
-  g.cta_pair = g_cta_pair;
+  g.cta_pair = 0;
   int rc = xp_gemm(&g, nullptr);
   if (rc) {
     printf("[%s] xp_gemm error: %s\n", c.name, xp_last_error());
@@ -226,8 +224,6 @@ static int run_case(const Case& c, bool timing) {
 
 int main(int argc, char** argv) {
   int fails = 0;
-  if (getenv("XP_CTA_PAIR")) g_cta_pair = atoi(getenv("XP_CTA_PAIR"));
-  printf("cta_pair mode %d\n", g_cta_pair);
   const Case basic[] = {
       {"kk_small_bn128", 128, 128, 64, 0, 0, 0, XP_OUT_F32, 1, 128, false, false, false},
       {"kk_k256_bn128", 128, 128, 256, 0, 0, 0, XP_OUT_F32, 1, 128, false, false, false},

@@ -1,4 +1,4 @@
-"""Timing of BASELINE.json config #5 (LF-VILA Swin-3D video encoder, released VideoEncoder config) on one B200.
+"""Timing of BASELINE.json config #5 (LF-VILA Swin-3D video encoder, released VideoEncoder config) on one H100.
 
 fwd + bwd of the module (synthetic video, a weighted-sum loss, DropPath off), CUDA-event timed, at BASELINE.json's
 [8,3,32,224,224] and the reference-native 192x320; beside it the reference algorithm in PyTorch eager (the pinned oracle, bf16
@@ -37,7 +37,7 @@ def main():
     model.load_state_dict(sd)
     model = model.to(dev).train()
     sdo = {k: (v.to(dev).requires_grad_(True) if v.is_floating_point() else v.to(dev)) for k, v in sd.items()}
-    peak = 1376.3
+    peak = 989.0          # NVIDIA H100 SXM data sheet, dense bf16 (a 700 W card); MEASURED_PEAKS.json overrides it
     try:
         with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) as f:
             peak = float(json.load(f).get("bf16_tflops_sustained", peak))

@@ -1,4 +1,4 @@
-"""Timing of BASELINE.json config #4 (HD-VILA TimeSformer, depth 4, dim 1024, 16 heads) on one B200.
+"""Timing of BASELINE.json config #4 (HD-VILA TimeSformer, depth 4, dim 1024, 16 heads) on one H100.
 
 fwd + bwd of the module (synthetic feature maps, a weighted-sum loss), CUDA-event timed, for the three shapes BASELINE.md §2
 lists; beside it the reference algorithm in PyTorch eager (the pinned oracle, bf16 autocast) on the same GPU.
@@ -38,7 +38,7 @@ def main():
     model.load_state_dict(sd)
     model = model.to(dev).train()
     sdo = {k: v.to(dev).requires_grad_(True) for k, v in sd.items()}
-    peak = 1376.3
+    peak = 989.0          # NVIDIA H100 SXM data sheet, dense bf16 (a 700 W card); MEASURED_PEAKS.json overrides it
     try:
         with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) as f:
             mp = json.load(f)

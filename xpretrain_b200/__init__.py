@@ -1,4 +1,4 @@
-"""xpretrain_b200 — B200-native (sm_100a) implementation of the XPretrain video-text dual-encoder hot path.
+"""xpretrain_b200 — H100-native (sm_90a) implementation of the XPretrain video-text dual-encoder hot path.
 
 Public surface mirrors the reference's CLIP-ViP entry points (SURVEY.md §8b):
   xpretrain_b200.modeling.VidCLIP            <- CLIP-ViP/src/modeling/VidCLIP.py

@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/xpretrain_b200.h).
 
-There is deliberately no fallback: if `libxpretrain_b200.so` is missing, or a call is made without a
-B200, the error is raised to the caller.  Build with `python -c "import __graft_entry__ as g; g.build()"`
+There is deliberately no fallback: if `libxpretrain_b200.so` is missing, or a call is made without an
+H100 (sm_90a), the error is raised to the caller.  Build with `python -c "import __graft_entry__ as g; g.build()"`
 (or `make`) — the library is kept in-tree under xpretrain_b200/lib/.
 """
 from __future__ import annotations
@@ -81,16 +81,8 @@ SIGNATURES = {
     "xp_vip_attention_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
     "xp_vip_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                      c_void_p]),
-    "xp_vip_attention_fwd_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                                        c_void_p]),
-    "xp_vip_attention_fwd_tc_partial": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                                c_int, c_void_p]),
     "xp_vip_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                      c_int, c_int, c_int, c_float, c_void_p]),
-    "xp_vip_attention_bwd_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                        c_int, c_int, c_int, c_int, c_float, c_void_p]),
-    "xp_vip_attention_bwd_tc_partial": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "xp_text_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "xp_text_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
                                       c_void_p]),

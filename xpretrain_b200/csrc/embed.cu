@@ -1,5 +1,5 @@
 // Embedding-side kernels of the CLIP-ViP path (all HBM-/latency-bound, index arithmetic bit-exact):
-//   * im2col of the stride-16 patch conv (CLIP_ViP.py:157-159,178-179) so the conv runs on the tcgen05 GEMM,
+//   * im2col of the stride-16 patch conv (CLIP_ViP.py:157-159,178-179) so the conv runs on the wgmma GEMM,
 //   * the position/temporal add table and the cls / video-proxy rows (CLIP_ViP.py:170-176,183-195),
 //   * their backward (scatter into class_embedding, added_cls, position_embedding, temporal_embedding),
 //   * CLIP text embeddings forward/backward (CLIP_ViP.py:222-225) and EOS pooling index (CLIP_ViP.py:776).

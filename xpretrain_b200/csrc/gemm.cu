@@ -1,9 +1,10 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:
-//   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared memory ring
-//   -> tcgen05.mma (single issuing thread, fp32 accumulators in TMEM, double buffered)
-//   -> tcgen05.ld epilogue (bias / q-scale / QuickGELU / dQuickGELU / residual) -> global.
-// One CTA per SM, 12 warps: warp0 = TMA producer, warp1 = MMA issuer, warp2 = TMEM allocator,
-// warps 4..11 = epilogue (two warps per TMEM lane quarter, each taking half of the columns).
+// Persistent warp-specialised bf16 GEMM for sm_90a:
+//   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (full / empty mbarriers)
+//   -> wgmma (two consumer warpgroups, 64 rows each, fp32 accumulators in registers)
+//   -> register epilogue (bias / q-scale / QuickGELU / dQuickGELU / GELU / residual) -> global.
+// One CTA per SM, 3 warpgroups: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = MMA + epilogue for rows
+// [0, 64) and [64, 128) of the 128 x BN tile.  While the consumers run a tile's epilogue the producer is already
+// filling the ring with the next tile's k-blocks.
 //
 // Replaces (see include/xpretrain_b200.h) every nn.Linear forward/backward on
 // the CLIP-ViP hot path: CLIP_ViP.py:341-343,379,393-395,1141-1145 and the
@@ -17,9 +18,8 @@ namespace xp {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
-constexpr int GEMM_THREADS = 384;  // 4 control warps + 8 epilogue warps
-constexpr int EPI_THREADS = 256;
+constexpr int MMA_K = 16;
+constexpr int GEMM_THREADS = 384;  // producer warpgroup + 2 consumer warpgroups
 
 struct GemmDev {
   void* c;
@@ -33,11 +33,7 @@ struct GemmDev {
   int splits;
   int scale_cols;
   float alpha, col_scale;
-  int wide;                 // C / aux / residual rows are 32-byte aligned (ld % 16 == 0)
   uint32_t mn_lbo, mn_sbo;  // MN-major descriptor strides (bytes): 64-element atom stride, 8-k-row group stride
-  int dbg;                  // profiling only (XP_GEMM_DEBUG): 1 no stores at all, 2 no wait for the staging boxes (racy), 4 stage but
-                            // do not issue the TMA stores, 8 activation = identity, 16 no epilogue input loads, 32 no aux store
-  int tma_c, tma_aux;       // pair kernel: C / the aux output leave through shared-memory staging + TMA stores
 };
 
 template <int BN>
@@ -46,9 +42,8 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : 6;
-  static constexpr int TMEM_COLS = 2 * BN;
   // ring + 1 KiB alignment slack + barriers
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + 2 * BN * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
 __device__ __forceinline__ float act_gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -58,53 +53,19 @@ __device__ __forceinline__ float act_gelu_erf_grad(float x) {
   return cdf + x * pdf;
 }
 
-// 16 consecutive bf16 (32 bytes) of one row: one 256-bit access when the row segment is 32-byte aligned,
-// else two 128-bit accesses (the second only if those 8 columns exist).
-__device__ __forceinline__ void ld_bf16x16(const __nv_bfloat16* ptr, bool wide, bool second, uint32_t (&w)[8]) {
-  if (wide) {
-    asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
-                 : "l"(ptr));
-  } else {
-    const uint4 a = *reinterpret_cast<const uint4*>(ptr);
-    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
-    w[4] = w[5] = w[6] = w[7] = 0u;
-    if (second) {
-      const uint4 b = *reinterpret_cast<const uint4*>(ptr + 8);
-      w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-    }
-  }
-}
-__device__ __forceinline__ void st_bf16x16(__nv_bfloat16* ptr, bool wide, bool second, const float (&v)[16]) {
-  uint32_t w[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) w[i] = pack_bf16(v[2 * i], v[2 * i + 1]);
-  if (wide) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-                 "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-                 : "memory");
-  } else {
-    *reinterpret_cast<uint4*>(ptr) = make_uint4(w[0], w[1], w[2], w[3]);
-    if (second) *reinterpret_cast<uint4*>(ptr + 8) = make_uint4(w[4], w[5], w[6], w[7]);
-  }
-}
-
 template <int BN, int A_MN, int B_MN, int OUT, int ACT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int NH = BN / 128;  // n128 accumulator blocks per consumer thread
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* bias_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);  // [2][BN]
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
   const int num_m = (p.M + BM - 1) / BM;
@@ -114,33 +75,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int kb_total = (p.K + BK - 1) / BK;
   const int kb_per = (kb_total + p.splits - 1) / p.splits;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], EPI_THREADS);
+      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
@@ -151,7 +99,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int k0 = split * kb_per;
         const int k1 = min(kb_total, k0 + kb_per);
         for (int kb = k0; kb < k1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
           uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
           uint8_t* sB = sA + Cfg::A_BYTES;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
@@ -176,68 +124,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 1) {
-    // -------------------------------------------------------- MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN, A_MN, B_MN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-        const int split = tile / num_mn;
-        const int k0 = split * kb_per;
-        const int k1 = min(kb_total, k0 + kb_per);
-        if (k0 >= k1) continue;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = k0; kb < k1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sB = sA + Cfg::A_BYTES;
-#pragma unroll
-          for (int j = 0; j < BK / UMMA_K; ++j) {
-            // K-major: 16 elements = 32 B further along the swizzled row; 8-row groups 1024 B apart.
-            // MN-major: 16 k-rows = 2048 B further; 64-element MN atoms BK*128 B apart.
-            const uint64_t adesc = A_MN ? make_smem_desc_sw128(sA + j * (UMMA_K * 128), p.mn_lbo, p.mn_sbo)
-                                        : make_smem_desc_sw128(sA + j * (UMMA_K * 2), 16, 1024);
-            const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sB + j * (UMMA_K * 128), p.mn_lbo, p.mn_sbo)
-                                        : make_smem_desc_sw128(sB + j * (UMMA_K * 2), 16, 1024);
-            umma_bf16(d_tmem, adesc, bdesc, idesc, (kb > k0 || j > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs retire
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ---------------------------------------------------------- epilogue
-    // 8 warps: warp (4+e) owns TMEM lane quarter e&3 and column half e>>2 of every accumulator.
-    const int ew = warp - 4;
-    const int quarter = ew & 3;  // == warp % 4, the lane quarter this warp may read
-    const int half = ew >> 2;
-    const int etid = threadIdx.x - 128;  // 0..255
-    constexpr int CHUNKS = BN / 64;      // 32-column chunks per warp per tile
-    // kernel parameters used per element live in registers (the asm "memory" clobbers would otherwise force
-    // ptxas to re-read them from the constant bank inside the loops)
-    const bool wide = p.wide != 0;       // every bf16 row segment is 32-byte aligned -> 256-bit accesses
-    constexpr int act = ACT;             // compile-time: the unused activation branches are not even generated
+  } else {
+    // ---------------------------------------------- MMA + epilogue (64 rows per warpgroup)
+    const int cw = wg - 1;                    // rows [64 cw, 64 cw + 64) of the tile
+    const int wq = (threadIdx.x >> 5) & 3;    // warp within the warpgroup: 16 of those rows
+    // kernel parameters used per element live in registers
+    constexpr int act = ACT;
     const int N = p.N, scale_cols = p.scale_cols;
     const float alpha = p.alpha, col_scale = p.col_scale;
     __nv_bfloat16* const aux_p = p.aux;
-    const bool need_aux_in = (act == XP_ACT_DQUICK_GELU || act == XP_ACT_DGELU_ERF);
-    // the one extra bf16 INPUT the epilogue streams: the saved pre-activation (dGELU) or the residual
+    constexpr bool need_aux_in = (ACT == XP_ACT_DQUICK_GELU || ACT == XP_ACT_DGELU_ERF);
+    // the one extra bf16 INPUT the epilogue reads: the saved pre-activation (dGELU) or the residual
     const __nv_bfloat16* const xin_p = need_aux_in ? p.aux : p.residual;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // this warpgroup's A rows: one 64-row slab = one 64-element MN atom (MN-major) or 64 swizzled 128-byte rows (K-major)
+    constexpr uint32_t A_OFF = 64 * 128;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const int split = tile / num_mn;
       const int mn = tile - split * num_mn;
@@ -246,48 +148,115 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const int k0 = split * kb_per;
       const int k1 = min(kb_total, k0 + kb_per);
       if (k0 >= k1) continue;
-      // stage this tile's bias slice in shared memory (double buffered by accumulator stage)
-      float* sbias = bias_smem + acc * BN;
-      for (int i = etid; i < BN; i += EPI_THREADS) {
-        const int n = n_blk * BN + i;
-        sbias[i] = (p.bias != nullptr && n < N && split == 0) ? p.bias[n] : 0.f;
+      float acc[NH][64];
+#pragma unroll
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = k0; kb < k1; ++kb) {
+        mbar_wait_nocall(&full_bar[stage], phase);
+        const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * A_OFF;
+        const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < BK / MMA_K; ++j) {
+          // K-major: 16 elements = 32 B further along the swizzled row; 8-row groups 1024 B apart.
+          // MN-major: 16 k-rows = 2048 B further; 64-element MN atoms BK*128 B apart.
+          const uint64_t adesc = A_MN ? make_smem_desc_sw128(sA + j * (MMA_K * 128), p.mn_lbo, p.mn_sbo)
+                                      : make_smem_desc_sw128(sA + j * (MMA_K * 2), 16, 1024);
+#pragma unroll
+          for (int h = 0; h < NH; ++h) {
+            // columns [128 h, 128 h + 128) of B: two MN atoms (MN-major) or 128 rows (K-major) further, 16 KiB either way
+            const uint32_t bh = sB + h * (128 * 128);
+            const uint64_t bdesc = B_MN ? make_smem_desc_sw128(bh + j * (MMA_K * 128), p.mn_lbo, p.mn_sbo)
+                                        : make_smem_desc_sw128(bh + j * (MMA_K * 2), 16, 1024);
+            wgmma_m64n128k16_bf16<A_MN, B_MN>(acc[h], adesc, bdesc);
+          }
+        }
+        wgmma_commit();
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+        // the previous k-block's MMAs have retired once at most this block's group is in flight: free its slot
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
       }
-      const int row = m_blk * BM + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      constexpr bool kTmaEpi = false;                    // TMA-store epilogue: 2-CTA kernel only (names below are unused here)
-      const uint32_t stg = 0;
-      const CUtensorMap& tmC = tmA;
-      const CUtensorMap& tmX = tmA;
-      const int m_tile0 = 0;
-      uint32_t st_pairs = 0;
-      constexpr bool kBiasDirect = false;
-      const float* const bias_t = nullptr;
-      (void)bias_t;
-      constexpr bool xin_tma = false, xin_live = false;  // TMA-loaded epilogue input: 2-CTA dGELU kernels only
-      uint64_t* const xbar = nullptr;
-      uint32_t xph = 0;
-      const int num_clusters = 0;
-      auto xin_issue = [](int, int) {};
-      (void)stg; (void)tmC; (void)tmX; (void)m_tile0; (void)st_pairs; (void)xbar; (void)xph; (void)num_clusters; (void)xin_issue;
-#include "gemm_epilogue.inc"
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+      // ---- epilogue straight from the accumulator registers: this thread holds rows r and r + 8, column pairs
+      const int row_base = m_blk * BM + cw * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int row = row_base + rr * 8;
+        if (row >= p.M) continue;
+        const long long c_off = p.c_group > 0 ? (row / p.c_group) * p.c_group_stride + (row % p.c_group) * p.ldc
+                                              : static_cast<long long>(row) * p.ldc;
+        const long long x_off = need_aux_in ? static_cast<long long>(row) * p.ld_aux
+                                            : (p.r_group > 0 ? (row / p.r_group) * p.r_group_stride + (row % p.r_group) * p.ldr
+                                                             : static_cast<long long>(row) * p.ldr);
+        const long long a_off = static_cast<long long>(row) * p.ld_aux;
+#pragma unroll
+        for (int h = 0; h < NH; ++h) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int n = n_blk * BN + h * 128 + i * 8 + (lane & 3) * 2;
+            if (n >= N) continue;   // N % 8 == 0: a column pair is either wholly inside or wholly outside
+            float2 b = make_float2(0.f, 0.f);
+            if (p.bias != nullptr && split == 0) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+            float v0 = fmaf(acc[h][4 * i + 2 * rr], alpha, b.x);
+            float v1 = fmaf(acc[h][4 * i + 2 * rr + 1], alpha, b.y);
+            if (n < scale_cols) {
+              v0 *= col_scale;
+              v1 *= col_scale;
+            }
+            uint32_t xg = 0;
+            if (xin_p != nullptr) xg = *reinterpret_cast<const uint32_t*>(xin_p + x_off + n);
+            if (act == XP_ACT_QUICK_GELU) {
+              if (aux_p != nullptr) *reinterpret_cast<uint32_t*>(aux_p + a_off + n) = pack_bf16(v0, v1);
+              v0 = quick_gelu(v0);
+              v1 = quick_gelu(v1);
+            } else if (act == XP_ACT_DQUICK_GELU) {
+              v0 *= quick_gelu_grad(bf16_lo(xg));
+              v1 *= quick_gelu_grad(bf16_hi(xg));
+            } else if (act == XP_ACT_GELU_ERF) {
+              if (aux_p != nullptr) *reinterpret_cast<uint32_t*>(aux_p + a_off + n) = pack_bf16(v0, v1);
+              v0 = act_gelu_erf(v0);
+              v1 = act_gelu_erf(v1);
+            } else if (act == XP_ACT_DGELU_ERF) {
+              v0 *= act_gelu_erf_grad(bf16_lo(xg));
+              v1 *= act_gelu_erf_grad(bf16_hi(xg));
+            } else if (xin_p != nullptr) {   // residual add (never combined with a dGELU epilogue)
+              v0 += bf16_lo(xg);
+              v1 += bf16_hi(xg);
+            }
+            if (OUT == XP_OUT_BF16) {
+              *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.c) + c_off + n) = pack_bf16(v0, v1);
+            } else if (OUT == XP_OUT_F32) {
+              *reinterpret_cast<float2*>(static_cast<float*>(p.c) + c_off + n) = make_float2(v0, v1);
+            } else {
+              asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(static_cast<float*>(p.c) + c_off + n), "f"(v0),
+                           "f"(v1)
+                           : "memory");
+            }
+          }
+        }
+      }
+    }
   }
 }
 
 template <int BN, int A_MN, int B_MN, int OUT, int ACT>
-static int launch_gemm(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int grid,
-                       cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int grid, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   auto kern = gemm_kernel<BN, A_MN, B_MN, OUT, ACT>;
   static bool attr_set = false;  // per instantiation
@@ -303,10 +272,10 @@ static int launch_gemm(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMa
 template <int BN, int OUT, int ACT>
 static int dispatch_layout(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev,
                            int grid, cudaStream_t stream) {
-  if (g->a_layout == 0 && g->b_layout == 0) return launch_gemm<BN, 0, 0, OUT, ACT>(g, tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 0 && g->b_layout == 1) return launch_gemm<BN, 0, 1, OUT, ACT>(g, tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 1 && g->b_layout == 1) return launch_gemm<BN, 1, 1, OUT, ACT>(g, tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 1 && g->b_layout == 0) return launch_gemm<BN, 1, 0, OUT, ACT>(g, tmA, tmB, dev, grid, stream);
+  if (g->a_layout == 0 && g->b_layout == 0) return launch_gemm<BN, 0, 0, OUT, ACT>(tmA, tmB, dev, grid, stream);
+  if (g->a_layout == 0 && g->b_layout == 1) return launch_gemm<BN, 0, 1, OUT, ACT>(tmA, tmB, dev, grid, stream);
+  if (g->a_layout == 1 && g->b_layout == 1) return launch_gemm<BN, 1, 1, OUT, ACT>(tmA, tmB, dev, grid, stream);
+  if (g->a_layout == 1 && g->b_layout == 0) return launch_gemm<BN, 1, 0, OUT, ACT>(tmA, tmB, dev, grid, stream);
   return fail("xp_gemm: a_layout/b_layout must be 0 or 1");
 }
 
@@ -331,65 +300,6 @@ static int dispatch_out(const XpGemm* g, const CUtensorMap& tmA, const CUtensorM
     case XP_OUT_BF16: return dispatch_act_bf16<BN>(g, tmA, tmB, dev, grid, stream);
     case XP_OUT_F32: return dispatch_layout<BN, XP_OUT_F32, XP_ACT_NONE>(g, tmA, tmB, dev, grid, stream);
     case XP_OUT_F32_ATOMIC: return dispatch_layout<BN, XP_OUT_F32_ATOMIC, XP_ACT_NONE>(g, tmA, tmB, dev, grid, stream);
-  }
-  return fail("xp_gemm: bad out mode");
-}
-
-#include "gemm_pair.inc"
-
-// tensor maps of the TMA-store epilogue (set by xp_gemm before dispatch_pair; copies of tmA when unused)
-static thread_local CUtensorMap t_tmC, t_tmX;
-
-template <int A_MN, int B_MN, int OUT, int ACT>
-static int launch_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int clusters,
-                       cudaStream_t stream) {
-  auto kern = gemm_pair_kernel<A_MN, B_MN, OUT, ACT>;
-  static bool attr_set = false;  // per instantiation
-  if (!attr_set) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR_SMEM_BYTES));
-    attr_set = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = PAIR_SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  XP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, t_tmC, t_tmX, dev));
-  XP_CHECK_LAUNCH("gemm_pair_kernel");
-  return 0;
-}
-
-template <int OUT, int ACT>
-static int dispatch_pair_layout(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev,
-                                int clusters, cudaStream_t stream) {
-  if (g->a_layout == 0 && g->b_layout == 0) return launch_pair<0, 0, OUT, ACT>(tmA, tmB, dev, clusters, stream);
-  if (g->a_layout == 0 && g->b_layout == 1) return launch_pair<0, 1, OUT, ACT>(tmA, tmB, dev, clusters, stream);
-  if (g->a_layout == 1 && g->b_layout == 1) return launch_pair<1, 1, OUT, ACT>(tmA, tmB, dev, clusters, stream);
-  if (g->a_layout == 1 && g->b_layout == 0) return launch_pair<1, 0, OUT, ACT>(tmA, tmB, dev, clusters, stream);
-  return fail("xp_gemm: a_layout/b_layout must be 0 or 1");
-}
-
-static int dispatch_pair(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev,
-                         int clusters, cudaStream_t stream) {
-  switch (g->out) {
-    case XP_OUT_BF16:
-      switch (g->act) {
-        case XP_ACT_NONE: return dispatch_pair_layout<XP_OUT_BF16, XP_ACT_NONE>(g, tmA, tmB, dev, clusters, stream);
-        case XP_ACT_QUICK_GELU: return dispatch_pair_layout<XP_OUT_BF16, XP_ACT_QUICK_GELU>(g, tmA, tmB, dev, clusters, stream);
-        case XP_ACT_DQUICK_GELU: return dispatch_pair_layout<XP_OUT_BF16, XP_ACT_DQUICK_GELU>(g, tmA, tmB, dev, clusters, stream);
-        case XP_ACT_GELU_ERF: return dispatch_pair_layout<XP_OUT_BF16, XP_ACT_GELU_ERF>(g, tmA, tmB, dev, clusters, stream);
-        case XP_ACT_DGELU_ERF: return dispatch_pair_layout<XP_OUT_BF16, XP_ACT_DGELU_ERF>(g, tmA, tmB, dev, clusters, stream);
-      }
-      return fail("xp_gemm: bad act");
-    case XP_OUT_F32: return dispatch_pair_layout<XP_OUT_F32, XP_ACT_NONE>(g, tmA, tmB, dev, clusters, stream);
-    case XP_OUT_F32_ATOMIC: return dispatch_pair_layout<XP_OUT_F32_ATOMIC, XP_ACT_NONE>(g, tmA, tmB, dev, clusters, stream);
   }
   return fail("xp_gemm: bad out mode");
 }
@@ -435,14 +345,10 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
     bn = (g->N >= 256 && tiles256 >= nsm) ? 256 : 128;
   }
   if (bn != 128 && bn != 256) return fail("xp_gemm: block_n must be 0, 128 or 256");
-  // 2-CTA pairs (256 x 256 tiles, UMMA M = 256) whenever the problem is big enough; cta_pair: 0 auto, 1 never, 2 force
-  bool pair = g->cta_pair == 2 || (g->cta_pair == 0 && g->block_n != 128 && g->N >= 256 && g->M >= 256);
-  if (g->cta_pair < 0 || g->cta_pair > 2) return fail("xp_gemm: cta_pair must be 0, 1 or 2");
-  if (pair) bn = 256;
-  const long long total = pair ? static_cast<long long>((g->M + 2 * BM - 1) / (2 * BM)) * ((g->N + 255) / 256) * splits
-                               : static_cast<long long>(num_m) * ((g->N + bn - 1) / bn) * splits;
+  // sm_90 has no CTA pairs: cta_pair 0 (auto) and 1 (never) both run the single-CTA kernel
+  if (g->cta_pair < 0 || g->cta_pair > 1) return fail("xp_gemm: cta_pair must be 0 or 1 (no CTA pairs on sm_90)");
+  const long long total = static_cast<long long>(num_m) * ((g->N + bn - 1) / bn) * splits;
   int grid = g->max_ctas > 0 ? g->max_ctas : nsm;
-  if (pair) grid /= 2;   // clusters
   if (grid < 1) grid = 1;
   if (grid > total) grid = static_cast<int>(total);
 
@@ -454,7 +360,7 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
     rc = make_tmap_bf16_2d(&tmA, g->a, g->M, g->K, g->lda, 64, BK);
   if (rc) return rc;
   if (g->b_layout == 0)
-    rc = make_tmap_bf16_2d(&tmB, g->b, g->K, g->N, g->ldb, BK, pair ? 128 : bn);   // a pair CTA stages half of B
+    rc = make_tmap_bf16_2d(&tmB, g->b, g->K, g->N, g->ldb, BK, bn);
   else
     rc = make_tmap_bf16_2d(&tmB, g->b, g->N, g->K, g->ldb, 64, BK);
   if (rc) return rc;
@@ -479,32 +385,9 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
   dev.scale_cols = g->scale_cols;
   dev.alpha = g->alpha;
   dev.col_scale = g->col_scale;
-  {
-    auto ok32 = [](const void* ptr, long long ld) { return ptr == nullptr || ((reinterpret_cast<uintptr_t>(ptr) & 31) == 0 && ld % 16 == 0); };
-    dev.wide = (g->out != XP_OUT_BF16 || ok32(g->c, g->ldc)) && ok32(g->aux, g->ld_aux) && ok32(g->residual, g->ldr) &&
-               (g->c_group_stride % 16 == 0) && (g->r_group_stride % 16 == 0);
-  }
-  static const int gemm_dbg = [] { const char* e = getenv("XP_GEMM_DEBUG"); return e ? atoi(e) : 0; }();
-  dev.dbg = gemm_dbg;
   dev.mn_lbo = g_dbg_mn_lbo ? g_dbg_mn_lbo : BK * 128;
   dev.mn_sbo = g_dbg_mn_sbo ? g_dbg_mn_sbo : 1024;
 
-  dev.tma_c = dev.tma_aux = 0;
-  t_tmC = tmA;
-  t_tmX = tmA;
-  static const bool tma_epi_off = getenv("XP_GEMM_NO_TMA_STORE") != nullptr;
-  if (pair && g->out == XP_OUT_BF16 && g->c_group == 0 && !tma_epi_off) {
-    // epilogue through shared memory + TMA stores: boxes of 64 columns x 32 rows (one epilogue warp's rows), 128B swizzle
-    if (make_tmap_bf16_2d(&t_tmC, g->c, g->N, g->M, g->ldc, 64, 32)) return -1;
-    dev.tma_c = 1;
-    static const bool tma_aux_off = getenv("XP_GEMM_NO_TMA_AUX") != nullptr;
-    // aux by TMA: stored by the GELU epilogues, loaded (next tile's boxes, ahead of time) by the dGELU epilogues
-    if (g->aux && g->act != XP_ACT_NONE && splits == 1 && !tma_aux_off) {
-      if (make_tmap_bf16_2d(&t_tmX, g->aux, g->N, g->M, g->ld_aux, 64, 32)) return -1;
-      dev.tma_aux = 1;
-    }
-  }
-  if (pair) return dispatch_pair(g, tmA, tmB, dev, grid, stream);
   return bn == 256 ? dispatch_out<256>(g, tmA, tmB, dev, grid, stream)
                    : dispatch_out<128>(g, tmA, tmB, dev, grid, stream);
 }

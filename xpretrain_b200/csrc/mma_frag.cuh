@@ -1,6 +1,6 @@
-// Warp-level mma.sync.m16n8k16 (bf16 -> fp32) building blocks shared by the attention kernels that run on the legacy
-// tensor-core path (vip_attention.cu, seg_attention.cu): swizzled [rows][64] bf16 shared-memory tiles, cp.async staging,
-// ldmatrix fragment loads.
+// Warp-level mma.sync.m16n8k16 (bf16 -> fp32) building blocks of the segment / window attention (seg_attention.cu):
+// swizzled [rows][64] bf16 shared-memory tiles, cp.async staging, ldmatrix fragment loads.  vip_attention.cu shares the
+// head-dim / exp2 constants and the zero-row store.
 #pragma once
 #include <cstdint>
 

@@ -6,9 +6,9 @@
 //   G = dL/dZ = (softmax_rows(Z) + softmax_cols(Z) - 2I) / N
 //   dV = s G T,  dT = s G^T V,  d logit_scale = sum_ij G_ij Z_ij         (SURVEY.md §8e closed form)
 //
-// The two GEMM-shaped steps run on the tcgen05 GEMM (gemm.cu).  To keep fp32-level logits out of bf16
+// The two GEMM-shaped steps run on the wgmma GEMM (gemm.cu).  To keep fp32-level logits out of bf16
 // tensor-core inputs, V and T are split into bf16 hi + lo parts and the three significant cross terms are
-// concatenated along K:  [Vh | Vh | Vl] . [Th | Tl | Th]^T  (K = 3d), i.e. one tcgen05 GEMM, ~2^-16 relative error.
+// concatenated along K:  [Vh | Vh | Vl] . [Th | Tl | Th]^T  (K = 3d), i.e. one GEMM, ~2^-16 relative error.
 // The kernels here are the prep / softmax / gradient pieces around those GEMMs.
 #include "../../include/xpretrain_b200.h"
 #include "common.h"

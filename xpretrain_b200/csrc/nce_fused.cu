@@ -7,27 +7,36 @@
 //      NVLink / NVSwitch) and raises a per-rank epoch flag on every peer (st.release.sys) — a device-side barrier, no NCCL;
 //   2. each CTA owns one 128 x 128 tile of Z = V T^T.  Its producer warps LOAD THE OPERAND ROWS STRAIGHT FROM THE OWNING
 //      PEER'S MEMORY (ld.relaxed.sys, 16 B per lane, coalesced per row), split every fp32 value into bf16 hi + lo and
-//      stage the four 128B-swizzled operand tiles {A_hi, A_lo, B_hi, B_lo} of a 64-column block in shared memory; one
-//      thread issues tcgen05.mma for hi*hi + hi*lo + lo*hi into a TMEM accumulator (fp32-grade logits on bf16 tensor
-//      cores).  A two-stage ring overlaps the NVLink loads of block c+1 with the MMAs of block c — the transfer rides
-//      under the math tile by tile, there is no gathered copy of the fp32 embeddings;
+//      stage the four 128B-swizzled operand tiles {A_hi, A_lo, B_hi, B_lo} of a 64-column block in shared memory; each
+//      of the two producer warpgroups then issues wgmma for hi*hi + hi*lo + lo*hi on its 64 tile rows into register
+//      accumulators (fp32-grade logits on bf16 tensor cores).  A two-stage ring overlaps the NVLink loads of block c+1
+//      with the MMAs of block c — the transfer rides under the math tile by tile, there is no gathered copy of the fp32
+//      embeddings;
 //   3. the epilogue scales by exp(logit_scale), parks the tile in shared memory and emits per-tile row / column
 //      (max, sum-exp) partials; after ONE grid barrier every CTA combines the partials it needs into the row / column
 //      log-sum-exps and writes its tile of exp(logit_scale) * dL/dZ (bf16) plus its share of the loss and of
 //      d logit_scale; the last CTA to finish adds the per-tile shares in a fixed order (deterministic, identical on all ranks).
 // Tiles on the first tile column / row also write the bf16 copies of V / T that the (local, collective-free) gradient
-// GEMMs dV = s G T, dT = s G^T V consume.  Launched cooperatively: (N/128)^2 CTAs <= SM count (N <= 1536).
+// GEMMs dV = s G T, dT = s G^T V consume.  Launched cooperatively: (N/128)^2 co-resident CTAs, one per SM (2-stage ring) or two per SM (compact variant).
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "ptx.cuh"
 
 namespace xp {
 
-constexpr int NF_THREADS = 288;                    // warps 0-3: A producers + epilogue, 4-7: B producers, 8: MMA issuer
+constexpr int NF_THREADS = 256;                    // warpgroup 0: A producers + epilogue, 1: B producers; both issue MMAs
 constexpr int NF_TILE = 128;
 constexpr int NF_STAGE_BYTES = 4 * NF_TILE * 128;  // A_hi, A_lo, B_hi, B_lo: [128 rows][64 bf16]
 constexpr int NF_ZLD = NF_TILE + 1;                // padded row pitch of the parked fp32 tile
-constexpr int NF_SMEM_MAIN = 2 * NF_STAGE_BYTES;   // 131072 (>= 128 * 129 * 4 for the parked tile)
+// Operand ring (2 stages: NVLink loads of block c+1 overlap the MMAs of block c) or, when (N/128)^2 tiles do not fit one CTA
+// per SM, a compact variant with ONE stage, half the loads in flight and <= 128 registers, so that two CTAs share an SM.
+// The parked fp32 tile (128 x 129) reuses the ring after the MMAs.
+__host__ __device__ constexpr int nf_smem_main(int stages) {
+  return stages * NF_STAGE_BYTES > NF_TILE * NF_ZLD * 4 ? stages * NF_STAGE_BYTES : NF_TILE * NF_ZLD * 4;
+}
+__host__ __device__ constexpr int nf_smem_bytes(int stages) {
+  return nf_smem_main(stages) + 2 * NF_TILE * 4 + 8 * 4 + 4 * 8 + 1024;
+}
 constexpr int NF_FLAG_BYTES = 1024;
 
 struct NfParams {
@@ -88,7 +97,10 @@ __device__ __forceinline__ const float* nf_row(const NfParams& p, int which, int
   return static_cast<const float*>(p.peers[which * p.world + rk]) + static_cast<long long>(loc) * p.d;
 }
 
-__global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const NfParams p) {
+template <int STAGES>
+__global__ void __launch_bounds__(NF_THREADS, 3 - STAGES) nce_gather_fused_kernel(const NfParams p) {
+  constexpr int NF_SMEM_MAIN = nf_smem_main(STAGES);
+  constexpr int LOADS = STAGES == 2 ? 16 : 8;        // 16-byte peer loads in flight per thread
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -97,8 +109,7 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
   float* s_lr = reinterpret_cast<float*>(gbase + NF_SMEM_MAIN);      // [128] row LSE
   float* s_lc = s_lr + NF_TILE;                                      // [128] column LSE
   float* s_red = s_lc + NF_TILE;                                     // [8]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(s_red + 8);            // full[2], empty[2], acc
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 5);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(s_red + 8);            // full[2], empty[2]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tp = blockIdx.x / p.nt, tq = blockIdx.x % p.nt;          // tile row (videos) / tile column (texts)
@@ -107,14 +118,9 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
   if (tid == 0) {
     mbar_init(&bar[0], 8);
     mbar_init(&bar[1], 8);
-    mbar_init(&bar[2], 1);
-    mbar_init(&bar[3], 1);
-    mbar_init(&bar[4], 1);
+    mbar_init(&bar[2], 2);    // one arrival per warpgroup once its MMAs on the stage retired
+    mbar_init(&bar[3], 2);
     fence_barrier_init();
-  }
-  if (warp == 8) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
   }
 
   // ---------------------------------------------------------------- 1. publish + device-side flag barrier
@@ -143,14 +149,14 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
       while (static_cast<int>(ld_acquire_sys(flag) - p.epoch) < 0) spin_guard(t0, "a peer's epoch flag", NF_PEER_TIMEOUT_CYCLES);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tD = *tmem_slot;
 
-  // ---------------------------------------------------------------- 2. logits tile on tcgen05, operands from peer memory
+  // ---------------------------------------------------------------- 2. logits tile on wgmma, operands from peer memory
   const int nblk = p.d / 64;
-  if (warp < 8) {
+  float acc[64];                                     // rows [64 which, 64 which + 64) x 128 columns of the tile
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  {
     const int which = warp >> 2;                     // 0: A = V rows of tile row tp, 1: B = T rows of tile column tq
     const int pw = warp & 3;
     const int tile0 = (which == 0 ? tp : tq) * NF_TILE;
@@ -158,18 +164,21 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
     __nv_bfloat16* hi_out = which == 0 ? p.vis_hi : p.txt_hi;
     const int sub = lane >> 4, t16 = lane & 15;      // 2 rows per warp instruction, 16 lanes x 16 B per 256-B row segment
     for (int c = 0; c < nblk; ++c) {
-      const int s = c & 1;
-      mbar_wait(&bar[2 + s], ((c >> 1) & 1) ^ 1);
+      const int s = c % STAGES;
+      const uint32_t ph = (c / STAGES) & 1;
+      mbar_wait_nocall(&bar[2 + s], ph ^ 1);
       const uint32_t st_hi = base + s * NF_STAGE_BYTES + which * 2 * NF_TILE * 128, st_lo = st_hi + NF_TILE * 128;
-      float4 x[16];
 #pragma unroll
-      for (int it = 0; it < 16; ++it) {              // all 16 NVLink loads in flight before the first use
-        const int r = tile0 + it * 8 + pw * 2 + sub;
+      for (int it0 = 0; it0 < 16; it0 += LOADS) {
+      float4 x[LOADS];
+#pragma unroll
+      for (int it = 0; it < LOADS; ++it) {           // LOADS NVLink loads in flight before the first use
+        const int r = tile0 + (it0 + it) * 8 + pw * 2 + sub;
         x[it] = r < p.N ? ld_peer_f4(nf_row(p, which, r) + c * 64 + t16 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
 #pragma unroll
-      for (int it = 0; it < 16; ++it) {
-        const int row = it * 8 + pw * 2 + sub;
+      for (int it = 0; it < LOADS; ++it) {
+        const int row = (it0 + it) * 8 + pw * 2 + sub;
         const float v[4] = {x[it].x, x[it].y, x[it].z, x[it].w};
         float h[4], l[4];
 #pragma unroll
@@ -186,58 +195,69 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
         if (write_hi && r < p.N)
           *reinterpret_cast<uint2*>(hi_out + static_cast<long long>(r) * p.d + c * 64 + t16 * 4) = make_uint2(h0, h1);
       }
+      }
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&bar[s]);
-    }
-  } else if (lane == 0) {
-    constexpr uint32_t idesc = make_idesc_bf16(NF_TILE, NF_TILE, 0, 0);
-    for (int c = 0; c < nblk; ++c) {
-      const int s = c & 1;
-      mbar_wait(&bar[s], (c >> 1) & 1);
-      fence_proxy_async_smem();
-      tc_fence_after();
-      const uint32_t a_hi = base + s * NF_STAGE_BYTES, a_lo = a_hi + NF_TILE * 128, b_hi = a_lo + NF_TILE * 128,
-                     b_lo = b_hi + NF_TILE * 128;
+      // both operand tiles of block c staged (8 warps): this warpgroup's 64 rows of A against all 128 rows of B
+      mbar_wait_nocall(&bar[s], ph);
+      const uint32_t a_hi = base + s * NF_STAGE_BYTES + which * 64 * 128, a_lo = a_hi + NF_TILE * 128,
+                     b_hi = base + s * NF_STAGE_BYTES + 2 * NF_TILE * 128, b_lo = b_hi + NF_TILE * 128;
       const uint32_t aa[3] = {a_hi, a_hi, a_lo}, bb[3] = {b_hi, b_lo, b_hi};
+      wgmma_fence_regs(acc);
+      wgmma_fence();
 #pragma unroll
       for (int g = 0; g < 3; ++g)
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks)
-          umma_bf16(tD, make_smem_desc_sw128(aa[g] + ks * 32, 16, 1024), make_smem_desc_sw128(bb[g] + ks * 32, 16, 1024), idesc,
-                    (c > 0 || g > 0 || ks > 0) ? 1u : 0u);
-      umma_commit(&bar[2 + s]);
+          wgmma_m64n128k16_bf16<0, 0>(acc, make_smem_desc_sw128(aa[g] + ks * 32, 16, 1024),
+                                      make_smem_desc_sw128(bb[g] + ks * 32, 16, 1024));
+      wgmma_commit();
+      wgmma_fence_regs(acc);
+      if (STAGES == 2) {
+        wgmma_wait<1>();                             // block c-1's MMAs retired: its stage may be refilled
+        if (c > 0 && (tid & 127) == 0) mbar_arrive(&bar[2 + (s ^ 1)]);
+      } else {
+        wgmma_wait<0>();                             // the single stage is free once this block's MMAs retired
+        if ((tid & 127) == 0) mbar_arrive(&bar[2]);
+      }
     }
-    umma_commit(&bar[4]);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
   }
 
   // ---------------------------------------------------------------- 3a. epilogue: scaled tile -> smem, per-tile partials
   const float s_exp = expf(*p.logit_scale);
   const int rows_valid = min(NF_TILE, p.N - tp * NF_TILE), cols_valid = min(NF_TILE, p.N - tq * NF_TILE);
+  __syncthreads();                                   // every MMA has read the ring: the parked tile may overwrite it
+  {
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int col = i * 8 + (lane & 3) * 2;
+      zs[r0 * NF_ZLD + col] = s_exp * acc[4 * i];
+      zs[r0 * NF_ZLD + col + 1] = s_exp * acc[4 * i + 1];
+      zs[(r0 + 8) * NF_ZLD + col] = s_exp * acc[4 * i + 2];
+      zs[(r0 + 8) * NF_ZLD + col + 1] = s_exp * acc[4 * i + 3];
+    }
+  }
+  __syncthreads();
   if (warp < 4) {
-    mbar_wait(&bar[4], 0);
-    tc_fence_after();
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
     float m = -INFINITY, sum = 0.f;
 #pragma unroll
     for (int ch = 0; ch < 4; ++ch) {
-      uint32_t o[32];
-      tmem_ld32(tD + lane_off + ch * 32, o);
-      tmem_ld_wait(o);
+      const float* o = zs + tid * NF_ZLD + ch * 32;
       float cm = -INFINITY;
 #pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        const float z = s_exp * __uint_as_float(o[e]);
-        zs[tid * NF_ZLD + ch * 32 + e] = z;
-        if (ch * 32 + e < cols_valid) cm = fmaxf(cm, z);
-      }
+      for (int e = 0; e < 32; ++e)
+        if (ch * 32 + e < cols_valid) cm = fmaxf(cm, o[e]);
       if (cm > m) {
         sum *= expf(m - cm);
         m = cm;
       }
 #pragma unroll
       for (int e = 0; e < 32; ++e)
-        if (ch * 32 + e < cols_valid) sum += expf(s_exp * __uint_as_float(o[e]) - m);
+        if (ch * 32 + e < cols_valid) sum += expf(o[e] - m);
     }
     if (tid < rows_valid) {
       float* rp = p.rowpart + (static_cast<long long>(tq) * p.Npad + tp * NF_TILE + tid) * 2;
@@ -338,12 +358,6 @@ __global__ void __launch_bounds__(NF_THREADS, 1) nce_gather_fused_kernel(const N
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tD, 128);
-  }
 }
 
 }  // namespace xp
@@ -368,8 +382,20 @@ extern "C" int xp_nce_gather_fused(const XpNceGather* a, void* stream) {
   if (a->b < 1) return fail("xp_nce_gather_fused: empty batch");
   const long long N = static_cast<long long>(a->world) * a->b;
   const int nt = static_cast<int>((N + NF_TILE - 1) / NF_TILE);
-  if (nt * nt > sm_count())
-    return fail("xp_nce_gather_fused: global batch too large for one co-resident wave of 128x128 tiles (N <= 1536 on B200)");
+  // every tile's CTA must be co-resident (one grid barrier): one CTA per SM with the 2-stage ring, else two per SM with the
+  // compact variant (N <= 1408 / 2048 on the 132 SMs of an H100)
+  static int blocks_per_sm[2] = {0, 0};   // [0]: compact (1 stage), [1]: 2 stages
+  if (blocks_per_sm[1] == 0) {
+    const void* k1 = reinterpret_cast<const void*>(nce_gather_fused_kernel<1>);
+    const void* k2 = reinterpret_cast<const void*>(nce_gather_fused_kernel<2>);
+    XP_CHECK_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, nf_smem_bytes(1)));
+    XP_CHECK_CUDA(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, nf_smem_bytes(2)));
+    XP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm[0], k1, NF_THREADS, nf_smem_bytes(1)));
+    XP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm[1], k2, NF_THREADS, nf_smem_bytes(2)));
+  }
+  const bool two_stage = nt * nt <= blocks_per_sm[1] * sm_count();
+  if (!two_stage && nt * nt > blocks_per_sm[0] * sm_count())
+    return fail("xp_nce_gather_fused: global batch too large for one co-resident wave of 128x128 tiles");
   if (a->ld_g < N) return fail("xp_nce_gather_fused: ld_g < N");
   if (a->mode == 0 && (a->b * a->d) % 4 != 0) return fail("xp_nce_gather_fused: b*d must be a multiple of 4");
   NfParams p;
@@ -386,15 +412,11 @@ extern "C" int xp_nce_gather_fused(const XpNceGather* a, void* stream) {
   p.colpart = ws + 2LL * nt * p.Npad;
   p.part = ws + 4LL * nt * p.Npad;
   p.counters = reinterpret_cast<unsigned int*>(ws + 4LL * nt * p.Npad + 2LL * nt * nt);
-  const int smem = NF_SMEM_MAIN + 2 * NF_TILE * 4 + 8 * 4 + 5 * 8 + 16 + 1024;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(nce_gather_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr = true;
-  }
   void* args[] = {&p};
-  XP_CHECK_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(nce_gather_fused_kernel), dim3(nt * nt), dim3(NF_THREADS),
-                                            args, smem, static_cast<cudaStream_t>(stream)));
+  const void* kern = two_stage ? reinterpret_cast<const void*>(nce_gather_fused_kernel<2>)
+                               : reinterpret_cast<const void*>(nce_gather_fused_kernel<1>);
+  XP_CHECK_CUDA(cudaLaunchCooperativeKernel(kern, dim3(nt * nt), dim3(NF_THREADS), args, nf_smem_bytes(two_stage ? 2 : 1),
+                                            static_cast<cudaStream_t>(stream)));
   XP_CHECK_LAUNCH("nce_gather_fused_kernel");
   return 0;
 }

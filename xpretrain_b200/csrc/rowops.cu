@@ -48,7 +48,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // ------------------------------------------------------------------ LayerNorm forward
 // Optionally fused with the residual add in fp32 (the reference keeps the residual stream in fp32 under autocast; a bf16
-// stream costs ~2.4x its feature error, profiles/r02_parity_calibration.md):  s = x (+ add);  sum_out = s (fp32);
+// stream multiplies its feature error):  s = x (+ add);  sum_out = s (fp32);
 // y = LN(s).  x is bf16 or fp32 (XF32), y bf16 or fp32 (YF32), add is the bf16 branch output (ADD).
 __device__ __forceinline__ void unpack8_h(const uint4& u, float (&f)[8]) {
   const __half2* h = reinterpret_cast<const __half2*>(&u);

@@ -15,7 +15,7 @@
 //   seg_attn_delta_kernel  delta = rowsum(dO * O)
 //   seg_attn_dkv_kernel    key-stationary:   dK, dV
 //   seg_attn_dq_kernel     query-stationary: dQ (scaled back through the q pre-scale)
-// The attentions are 0.5-2 % of a TimeSformer block's FLOPs (the tcgen05 GEMMs around them carry the rest).
+// The attentions are 0.5-2 % of a TimeSformer block's FLOPs (the wgmma GEMMs around them carry the rest).
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "mma_frag.cuh"

@@ -3,14 +3,19 @@
 // Reference: CLIPAttention.forward2, CLIP_ViP.py:332-381.  Patch queries of frame t attend to
 // [M global keys ; L keys of frame t] (:352-363); the M global queries (cls + video proxies) attend to
 // all M + T*L keys (:366-375).  The reference materialises the per-frame K/V with repeat+cat; here a CTA
-// stages rows {0..M-1} U {M+t*L .. M+(t+1)*L-1} of the fused qkv buffer once in shared memory and treats
+// stages the L frame rows and the M global rows of the fused qkv buffer once in shared memory and treats
 // the global queries as extra query rows: their softmax over all frames is assembled from per-frame
 // partials (max, sum, unnormalised output) by a small combine kernel.  q arrives pre-scaled by
 // head_dim**-0.5 from the QKV GEMM epilogue (CLIP_ViP.py:341).
 //
-// Tensor-core path: warp-level mma.sync.m16n8k16 (bf16 -> fp32) with ldmatrix-fed fragments; 200 keys fit
-// one CTA so the softmax is a two-block online pass.  (A tcgen05/TMEM version is the planned upgrade; the
-// attention is 4 % of the block's FLOPs, the GEMMs around it are tcgen05.)
+// Hopper path: one thread stages the operands by TMA (two boxes per matrix: the L frame rows into shared-memory rows
+// [0, L), the M global rows into rows [248, 248 + M), both 1024-byte aligned for the 128B swizzle; the rows between
+// are zero), completion on an mbarrier.  Two warpgroups each own 64-row tiles and run every product on wgmma:
+//   forward   S = Q·Kᵀ (both operands from shared memory), online softmax over 64-key blocks in registers, and
+//             O += P·V with P taken from registers as the A operand (split into bf16 hi + lo, see below);
+//   backward  pass A (key-stationary): Sᵀ = K·Qᵀ and dPᵀ = V·dOᵀ, then dV += Pᵀ·dO and dK += dSᵀ·Q with Pᵀ / dSᵀ in
+//             registers; pass B (query-stationary): S = Q·Kᵀ, dP = dO·Vᵀ, dQ += dS·K.  No operand is transposed in
+//             memory: V, dO, Q and K serve as MN-major B operands where the product contracts over their rows.
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "ptx.cuh"
@@ -18,10 +23,11 @@
 
 namespace xp {
 
-constexpr int ROWS = 208;       // padded query/key rows per CTA (13 m16 tiles); M + L <= ROWS
-constexpr int NTILE = ROWS / 16;
-constexpr int ATT_WARPS = 7;
-constexpr int ATT_THREADS = ATT_WARPS * 32;
+constexpr int SROWS = 256;                 // shared-memory rows per staged matrix (4 tiles of 64)
+constexpr int GROW = 248;                  // first shared-memory row of the global tokens (1024-byte aligned)
+constexpr int MAT_BYTES = SROWS * 128;     // one [256][64] bf16 matrix, 128B-swizzled
+constexpr int TILE_BYTES = 64 * 128;       // 64 rows
+constexpr int ATT_THREADS = 256;           // two warpgroups
 
 struct AttnDims {
   int B, H, T, L, M;
@@ -31,181 +37,182 @@ struct AttnDims {
   int C;
 };
 
-
 __device__ __forceinline__ long long token_row(const AttnDims& d, int b, int t, int i) {
   return static_cast<long long>(b) * d.S + (i < d.M ? i : d.M + static_cast<long long>(t) * d.L + (i - d.M));
 }
+// shared-memory row r: a frame token (r < L), a global token (GROW <= r < GROW + M) or zero padding
+__device__ __forceinline__ bool row_valid(int r, const AttnDims& d) { return r < d.L || (r >= GROW && r < GROW + d.M); }
+__device__ __forceinline__ bool row_global(int r) { return r >= GROW; }
+__device__ __forceinline__ int row_seq(int r, const AttnDims& d) { return r >= GROW ? r - GROW : d.M + r; }
+// a 64-row tile holds at least one token (tile 3 always holds the global rows)
+__device__ __forceinline__ bool tile_live(int k, const AttnDims& d) { return k == 3 || 64 * k < d.L; }
 
-// Stage the q/k/v rows of (b, h, t) with cp.async; rows >= M+L are zero.
-__device__ __forceinline__ void stage_qkv(const __nv_bfloat16* __restrict__ qkv, const AttnDims& d, int b, int h, int t,
-                                          uint32_t sQ, uint32_t sK, uint32_t sV) {
-  const int nq = d.M + d.L;
-  for (int idx = threadIdx.x; idx < 3 * ROWS * 8; idx += ATT_THREADS) {
-    const int mat = idx / (ROWS * 8);
-    const int rem = idx - mat * (ROWS * 8);
-    const int row = rem >> 3, chunk = rem & 7;
-    const uint32_t dst = tile_addr(mat == 0 ? sQ : (mat == 1 ? sK : sV), row, chunk);
-    if (row < nq) {
-      cp_async16(dst, qkv + token_row(d, b, t, row) * d.ld_qkv + static_cast<long long>(mat) * d.C + h * HD + chunk * 8);
-    } else {
-      st_shared_zero16(dst);
+__device__ __forceinline__ uint64_t kdesc(uint32_t addr) { return make_smem_desc_sw128(addr, 16, 1024); }     // K-major
+__device__ __forceinline__ uint64_t mndesc(uint32_t addr) { return make_smem_desc_sw128(addr, 8192, 1024); }  // MN-major
+
+// Zero the padding rows of NMAT matrices, then TMA the frame rows and global rows of each; every thread waits.
+template <int NMAT>
+__device__ __forceinline__ void stage_rows(uint8_t* sm, uint64_t* bar, const CUtensorMap* const (&mapL)[NMAT],
+                                           const CUtensorMap* const (&mapM)[NMAT], const int (&col)[NMAT], const AttnDims& d,
+                                           int b, int t) {
+  if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    fence_barrier_init();
+  }
+  const uint32_t base = smem_u32(sm);
+  for (int idx = threadIdx.x; idx < NMAT * SROWS * 8; idx += ATT_THREADS) {
+    const int m = idx / (SROWS * 8), row = (idx >> 3) % SROWS;
+    if (!row_valid(row, d)) st_shared_zero16(base + m * MAT_BYTES + row * 128 + (idx & 7) * 16);
+  }
+  fence_proxy_async_smem();     // the zero rows are read by wgmma (async proxy)
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(bar, NMAT * (d.L + d.M) * 128);
+#pragma unroll
+    for (int m = 0; m < NMAT; ++m) {
+      tma_load_2d(sm + m * MAT_BYTES, mapL[m], bar, col[m], static_cast<int>(b * d.S + d.M + static_cast<long long>(t) * d.L));
+      tma_load_2d(sm + m * MAT_BYTES + GROW * 128, mapM[m], bar, col[m], static_cast<int>(b * d.S));
     }
+  }
+  mbar_wait_nocall(bar, 0);
+}
+
+// P (or dS) of a 64 x 64 accumulator as the A fragments of the four k16 steps: k-step ks covers columns [16 ks, 16 ks + 16)
+__device__ __forceinline__ void acc_to_afrag(const float (&x)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    a[ks][0] = pack_bf16(x[8 * ks + 0], x[8 * ks + 1]);
+    a[ks][1] = pack_bf16(x[8 * ks + 2], x[8 * ks + 3]);
+    a[ks][2] = pack_bf16(x[8 * ks + 4], x[8 * ks + 5]);
+    a[ks][3] = pack_bf16(x[8 * ks + 6], x[8 * ks + 7]);
   }
 }
 
 // ======================================================================== forward
 // grid (T, H, B).  out: [B*S, C] bf16 (frame rows); lse: [B, H, S] fp32 (frame rows);
 // part: [B, H, T, M, 66] fp32 = {max, sum, unnormalised out[64]} of the global queries over this frame's keys.
-template <int NT>  // n8 tiles in this key block
-__device__ __forceinline__ void fwd_key_block(uint32_t sK, uint32_t sV, int key0, int lane, const uint32_t (&qa)[4][4],
-                                              float (&o)[8][4], float (&m_run)[2], float (&l_run)[2], int nq, int M,
-                                              bool mask_global_keys, int row_lo) {
-  float s[NT][4];
-#pragma unroll
-  for (int i = 0; i < NT; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-  for (int np = 0; np < NT / 2; ++np) {
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      uint32_t b[4];
-      load_b_nk(sK, key0 + np * 16, ks, lane, b);
-      mma_bf16(s[2 * np], qa[ks], b[0], b[1]);
-      mma_bf16(s[2 * np + 1], qa[ks], b[2], b[3]);
-    }
-  }
-  // masks: padded keys; for global QUERY rows, the global keys count only once (frame 0)
-  float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-  for (int i = 0; i < NT; ++i) {
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int key = key0 + i * 8 + (lane & 3) * 2 + (e & 1);
-      const int row = row_lo + (e >> 1) * 8;
-      const bool dead = key >= nq || (mask_global_keys && row < M && key < M);
-      if (dead) s[i][e] = -INFINITY;
-      mx[e >> 1] = fmaxf(mx[e >> 1], s[i][e]);
-    }
-  }
-  float corr[2], m_new[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-    m_new[r] = fmaxf(m_run[r], mx[r]);
-    corr[r] = (m_new[r] == -INFINITY) ? 1.f : fast_exp2((m_run[r] - m_new[r]) * LOG2E);
-    l_run[r] *= corr[r];
-    m_run[r] = m_new[r];
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    o[i][0] *= corr[0]; o[i][1] *= corr[0];
-    o[i][2] *= corr[1]; o[i][3] *= corr[1];
-  }
-  const float mb[2] = {m_new[0] == -INFINITY ? 0.f : m_new[0] * LOG2E, m_new[1] == -INFINITY ? 0.f : m_new[1] * LOG2E};
-#pragma unroll
-  for (int i = 0; i < NT; ++i) {
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float pv = fast_exp2(fmaf(s[i][e], LOG2E, -mb[e >> 1]));  // exp2(-inf) = 0 for masked entries
-      s[i][e] = pv;
-      l_run[e >> 1] += pv;
-    }
-  }
-#pragma unroll
-  for (int kk = 0; kk < NT / 2; ++kk) {
-    uint32_t pa[4];
-    pa[0] = pack_bf16(s[2 * kk][0], s[2 * kk][1]);
-    pa[1] = pack_bf16(s[2 * kk][2], s[2 * kk][3]);
-    pa[2] = pack_bf16(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-    pa[3] = pack_bf16(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-    for (int dp = 0; dp < 4; ++dp) {
-      uint32_t b[4];
-      load_b_kn(sV, key0 + kk * 16, dp, lane, b);
-      mma_bf16(o[2 * dp], pa, b[0], b[1]);
-      mma_bf16(o[2 * dp + 1], pa, b[2], b[3]);
-    }
-  }
-}
-
 __global__ void __launch_bounds__(ATT_THREADS, 2)
-vip_attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, float* __restrict__ lse,
-                    float* __restrict__ part, const AttnDims d) {
+vip_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_constant__ CUtensorMap tmM,
+                    __nv_bfloat16* __restrict__ out, float* __restrict__ lse, float* __restrict__ part, const AttnDims d) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sQ = (raw + 127u) & ~127u;
-  const uint32_t sK = sQ + ROWS * 128, sV = sK + ROWS * 128;
-  uint8_t* sQ_ptr = smem_raw + (sQ - raw);
+  uint8_t* sm = smem_raw + (((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw));
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + 3 * MAT_BYTES);
   const int t = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nq = d.M + d.L;
+  {
+    const CUtensorMap* const mL[3] = {&tmL, &tmL, &tmL};
+    const CUtensorMap* const mM[3] = {&tmM, &tmM, &tmM};
+    const int col[3] = {h * HD, d.C + h * HD, 2 * d.C + h * HD};
+    stage_rows<3>(sm, bar, mL, mM, col, d, b, t);
+  }
+  const uint32_t sQ = smem_u32(sm), sK = sQ + MAT_BYTES, sV = sK + MAT_BYTES;
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool mask_gg = (t != 0);   // (global query, global key) pairs belong to frame 0 only
 
-  stage_qkv(qkv, d, b, h, t, sQ, sK, sV);
-  cp_async_wait_all();
-  __syncthreads();
-
-  for (int mt = warp; mt < NTILE; mt += ATT_WARPS) {
-    if (mt * 16 >= nq) break;
-    uint32_t qa[4][4];
-    load_a_frags(sQ, mt * 16, lane, qa);
-    float o[8][4];
+  for (int qt = wg; qt < 4; qt += 2) {
+    if (!tile_live(qt, d)) continue;
+    const int r_lo = qt * 64 + wq * 16 + (lane >> 2);
+    const bool qg[2] = {row_global(r_lo), row_global(r_lo + 8)};
+    float o[32];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-    const int row_lo = mt * 16 + (lane >> 2);
-    fwd_key_block<14>(sK, sV, 0, lane, qa, o, m_run, l_run, nq, d.M, t != 0, row_lo);
-    fwd_key_block<12>(sK, sV, 112, lane, qa, o, m_run, l_run, nq, d.M, t != 0, row_lo);
+#pragma unroll 1
+    for (int kb = 0; kb < 4; ++kb) {
+      if (!tile_live(kb, d)) continue;
+      float s[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = 0.f;
+      wgmma_fence_regs(s);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+        wgmma_m64n64k16_ss<0, 0>(s, kdesc(sQ + qt * TILE_BYTES + ks * 32), kdesc(sK + kb * TILE_BYTES + ks * 32));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      // masks: padding keys; for global QUERY rows, the global keys count only once (frame 0)
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = kb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
+          const bool dead = !row_valid(key, d) || (mask_gg && qg[e >> 1] && row_global(key));
+          if (dead) s[4 * i + e] = -INFINITY;
+          mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * i + e]);
+        }
+      float corr[2], mb[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        const float m_new = fmaxf(m_run[r], mx[r]);
+        corr[r] = (m_new == -INFINITY) ? 1.f : fast_exp2((m_run[r] - m_new) * LOG2E);
+        l_run[r] *= corr[r];
+        m_run[r] = m_new;
+        mb[r] = m_new == -INFINITY ? 0.f : m_new * LOG2E;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        o[4 * i + 0] *= corr[0]; o[4 * i + 1] *= corr[0];
+        o[4 * i + 2] *= corr[1]; o[4 * i + 3] *= corr[1];
+      }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float pv = fast_exp2(fmaf(s[i], LOG2E, -mb[(i >> 1) & 1]));   // exp2(-inf) = 0 for masked entries
+        s[i] = pv;
+        l_run[(i >> 1) & 1] += pv;
+      }
+      // P·V with P split into bf16 hi + lo (P = hi + lo to ~2^-16): rounding P to bf16 is the largest error of the forward,
+      // and it reaches the pooled CLS features through the global-query rows
+      uint32_t ph[4][4], pl[4][4];
+      acc_to_afrag(s, ph);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          pl[ks][j] = pack_bf16(s[8 * ks + 2 * j] - bf16_lo(ph[ks][j]), s[8 * ks + 2 * j + 1] - bf16_hi(ph[ks][j]));
+      wgmma_fence_regs(o);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t vd = mndesc(sV + kb * TILE_BYTES + ks * 16 * 128);
+        wgmma_m64n64k16_rs<1>(o, ph[ks], vd);
+        wgmma_m64n64k16_rs<1>(o, pl[ks], vd);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
       l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
     }
-    // ---- global-query rows: write the per-frame partial (fp32, unnormalised)
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const int row = row_lo + r * 8;
-      if (row < d.M) {
-        float* p = part + (((static_cast<long long>(b) * d.H + h) * d.T + t) * d.M + row) * 66;
+      const int row = r_lo + r * 8;
+      if (!row_valid(row, d)) continue;
+      if (row_global(row)) {   // global-query row: this frame's partial (fp32, unnormalised)
+        float* p = part + (((static_cast<long long>(b) * d.H + h) * d.T + t) * d.M + (row - GROW)) * 66;
         if ((lane & 3) == 0) {
           p[0] = m_run[r];
           p[1] = l_run[r];
         }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          p[2 + i * 8 + (lane & 3) * 2] = o[i][2 * r];
-          p[2 + i * 8 + (lane & 3) * 2 + 1] = o[i][2 * r + 1];
+          p[2 + i * 8 + (lane & 3) * 2] = o[4 * i + 2 * r];
+          p[2 + i * 8 + (lane & 3) * 2 + 1] = o[4 * i + 2 * r + 1];
         }
-      }
-    }
-    // ---- frame rows: normalise, stage through this tile's (now dead) Q rows, store 128-byte rows
-    const float inv[2] = {l_run[0] > 0.f ? 1.f / l_run[0] : 0.f, l_run[1] > 0.f ? 1.f / l_run[1] : 0.f};
-    __syncwarp();
+      } else {                 // frame row: normalised output + LSE
+        const float inv = l_run[r] > 0.f ? 1.f / l_run[r] : 0.f;
+        const long long tr = token_row(d, b, t, row_seq(row, d));
+        __nv_bfloat16* dst = out + tr * d.ld_o + h * HD + (lane & 3) * 2;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = mt * 16 + (lane >> 2) + r * 8;
-        const uint32_t v = pack_bf16(o[i][2 * r] * inv[r], o[i][2 * r + 1] * inv[r]);
-        *reinterpret_cast<uint32_t*>(sQ_ptr + (tile_addr(sQ, row, i) - sQ) + (lane & 3) * 4) = v;
-      }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int idx = lane + it * 32;
-      const int row = mt * 16 + (idx >> 3), chunk = idx & 7;
-      if (row >= d.M && row < nq) {
-        const uint4 v = *reinterpret_cast<const uint4*>(sQ_ptr + (tile_addr(sQ, row, chunk) - sQ));
-        *reinterpret_cast<uint4*>(out + token_row(d, b, t, row) * d.ld_o + h * HD + chunk * 8) = v;
-      }
-    }
-    if ((lane & 3) == 0) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = row_lo + r * 8;
-        if (row >= d.M && row < nq)
-          lse[(static_cast<long long>(b) * d.H + h) * d.S + (token_row(d, b, t, row) - static_cast<long long>(b) * d.S)] =
-              m_run[r] + logf(l_run[r]);
+        for (int i = 0; i < 8; ++i)
+          *reinterpret_cast<uint32_t*>(dst + i * 8) = pack_bf16(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
+        if ((lane & 3) == 0)
+          lse[(static_cast<long long>(b) * d.H + h) * d.S + (tr - static_cast<long long>(b) * d.S)] = m_run[r] + logf(l_run[r]);
       }
     }
   }
@@ -232,205 +239,193 @@ vip_attn_fwd_combine_kernel(const float* __restrict__ part, __nv_bfloat16* __res
   }
 }
 
+
 // ======================================================================= backward
 // dqkv: [B*S, 3C] bf16 (frame rows written here; the M global rows by the combine kernel);
 // gpart: [B, H, T, M, 3, 64] fp32 partial dq/dk/dv of the global rows from this frame.
-struct BwdSmem {
-  uint32_t sQ, sK, sV, sdO;
-  float* lse;
-  float* delta;
-};
-
-__device__ __forceinline__ void p_and_ds(float s, float dp, float lse_l2, float delta, bool valid, float& p, float& ds) {
-  p = valid ? fast_exp2(fmaf(s, LOG2E, -lse_l2)) : 0.f;
-  ds = p * (dp - delta);
-}
-
-__global__ void __launch_bounds__(ATT_THREADS, 2)
-vip_attn_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict__ out,
-                    const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+vip_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_constant__ CUtensorMap tmM,
+                    const __grid_constant__ CUtensorMap tdL, const __grid_constant__ CUtensorMap tdM,
+                    const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
                     __nv_bfloat16* __restrict__ dqkv, float* __restrict__ gpart, const AttnDims d, float q_scale) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sQ = (raw + 127u) & ~127u;
-  const uint32_t sK = sQ + ROWS * 128, sV = sK + ROWS * 128, sdO = sV + ROWS * 128;
-  float* s_lse = reinterpret_cast<float*>(smem_raw + (sdO + ROWS * 128 - raw));  // lse * log2(e), +inf on padding
-  float* s_delta = s_lse + ROWS;
+  uint8_t* sm = smem_raw + (((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw));
+  float* s_lse = reinterpret_cast<float*>(sm + 4 * MAT_BYTES);   // lse * log2(e), +inf on padding rows
+  float* s_delta = s_lse + SROWS;                                  // rowsum(dO * O)
+  uint64_t* bar = reinterpret_cast<uint64_t*>(s_delta + SROWS);
   const int t = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nq = d.M + d.L;
-  const bool mask_gg = (t != 0);  // (global query, global key) pairs belong to frame 0 only
-
-  stage_qkv(qkv, d, b, h, t, sQ, sK, sV);
-  // dO rows + delta_i = sum_d dO[i,d] * O[i,d]  (8 lanes per row, 16 bytes each)
-  for (int base = 0; base < ROWS; base += ATT_THREADS / 8) {
+  {
+    const CUtensorMap* const mL[4] = {&tmL, &tmL, &tmL, &tdL};
+    const CUtensorMap* const mM[4] = {&tmM, &tmM, &tmM, &tdM};
+    const int col[4] = {h * HD, d.C + h * HD, 2 * d.C + h * HD, h * HD};
+    stage_rows<4>(sm, bar, mL, mM, col, d, b, t);
+  }
+  // delta_i = sum_d dO[i,d] * O[i,d] and the saved LSE per shared-memory row (8 lanes per row, 16 bytes each)
+  for (int base = 0; base < SROWS; base += ATT_THREADS / 8) {
     const int row = base + (threadIdx.x >> 3), chunk = threadIdx.x & 7;
-    if (row < ROWS) {
-      float dot = 0.f;
-      uint4 g = make_uint4(0, 0, 0, 0);
-      if (row < nq) {
-        const long long off = token_row(d, b, t, row) * d.ld_o + h * HD + chunk * 8;
-        g = *reinterpret_cast<const uint4*>(dout + off);
-        const uint4 o = *reinterpret_cast<const uint4*>(out + off);
-        const uint32_t gw[4] = {g.x, g.y, g.z, g.w}, ow[4] = {o.x, o.y, o.z, o.w};
+    float dot = 0.f;
+    const bool valid = row_valid(row, d);
+    long long tr = 0;
+    if (valid) {
+      tr = token_row(d, b, t, row_seq(row, d));
+      const long long off = tr * d.ld_o + h * HD + chunk * 8;
+      const uint4 g = *reinterpret_cast<const uint4*>(dout + off);
+      const uint4 o = *reinterpret_cast<const uint4*>(out + off);
+      const uint32_t gw[4] = {g.x, g.y, g.z, g.w}, ow[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-        for (int i = 0; i < 4; ++i) dot += bf16_lo(gw[i]) * bf16_lo(ow[i]) + bf16_hi(gw[i]) * bf16_hi(ow[i]);
-      }
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(tile_addr(sdO, row, chunk)), "r"(g.x), "r"(g.y),
-                   "r"(g.z), "r"(g.w)
-                   : "memory");
-      dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-      dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-      dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-      if (chunk == 0) {
-        s_delta[row] = dot;
-        s_lse[row] = row < nq ? lse[(static_cast<long long>(b) * d.H + h) * d.S +
-                                    (token_row(d, b, t, row) - static_cast<long long>(b) * d.S)] * LOG2E
-                              : INFINITY;
-      }
+      for (int i = 0; i < 4; ++i) dot += bf16_lo(gw[i]) * bf16_lo(ow[i]) + bf16_hi(gw[i]) * bf16_hi(ow[i]);
+    }
+    dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+    dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+    dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+    if (chunk == 0) {
+      s_delta[row] = dot;
+      s_lse[row] = valid ? lse[(static_cast<long long>(b) * d.H + h) * d.S + (tr - static_cast<long long>(b) * d.S)] * LOG2E
+                         : INFINITY;
     }
   }
-  cp_async_wait_all();
   __syncthreads();
 
+  const uint32_t sQ = smem_u32(sm), sK = sQ + MAT_BYTES, sV = sK + MAT_BYTES, sdO = sV + MAT_BYTES;
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool mask_gg = (t != 0);
   float* gp = gpart + ((static_cast<long long>(b) * d.H + h) * d.T + t) * d.M * 3 * HD;
 
   // ------------------------------------------------ pass A: key-stationary -> dK, dV
-  for (int kt = warp; kt < NTILE; kt += ATT_WARPS) {
-    if (kt * 16 >= nq) break;
-    uint32_t ka[4][4], va[4][4];
-    load_a_frags(sK, kt * 16, lane, ka);
-    load_a_frags(sV, kt * 16, lane, va);
-    float dk[8][4], dv[8][4];
+  for (int kt = wg; kt < 4; kt += 2) {
+    if (!tile_live(kt, d)) continue;
+    const int k_lo = kt * 64 + wq * 16 + (lane >> 2);
+    float dk[32], dv[32];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
-    const int key_lo = kt * 16 + (lane >> 2);
+    for (int i = 0; i < 32; ++i) dk[i] = dv[i] = 0.f;
 #pragma unroll 1
-    for (int qb = 0; qb < NTILE; ++qb) {
-      if (qb * 16 >= nq) break;
-      float st[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}}, dpt[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    for (int qb = 0; qb < 4; ++qb) {
+      if (!tile_live(qb, d)) continue;
+      float st[32], dpt[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
+      wgmma_fence_regs(st);
+      wgmma_fence_regs(dpt);
+      wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        uint32_t bq[4], bo[4];
-        load_b_nk(sQ, qb * 16, ks, lane, bq);
-        load_b_nk(sdO, qb * 16, ks, lane, bo);
-        mma_bf16(st[0], ka[ks], bq[0], bq[1]);
-        mma_bf16(st[1], ka[ks], bq[2], bq[3]);
-        mma_bf16(dpt[0], va[ks], bo[0], bo[1]);
-        mma_bf16(dpt[1], va[ks], bo[2], bo[3]);
+        wgmma_m64n64k16_ss<0, 0>(st, kdesc(sK + kt * TILE_BYTES + ks * 32), kdesc(sQ + qb * TILE_BYTES + ks * 32));
+        wgmma_m64n64k16_ss<0, 0>(dpt, kdesc(sV + kt * TILE_BYTES + ks * 32), kdesc(sdO + qb * TILE_BYTES + ks * 32));
       }
-      float pt[2][4], dst[2][4];
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(st);
+      wgmma_fence_regs(dpt);
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int i = 0; i < 8; ++i)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const int q = qb * 16 + i * 8 + (lane & 3) * 2 + (e & 1);
-          const int key = key_lo + (e >> 1) * 8;
-          const bool valid = q < nq && key < nq && !(mask_gg && q < d.M && key < d.M);
-          p_and_ds(st[i][e], dpt[i][e], s_lse[q], s_delta[q], valid, pt[i][e], dst[i][e]);
+          const int q = qb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
+          const int key = k_lo + (e >> 1) * 8;
+          const bool valid = row_valid(q, d) && row_valid(key, d) && !(mask_gg && row_global(q) && row_global(key));
+          const float p = valid ? fast_exp2(fmaf(st[4 * i + e], LOG2E, -s_lse[q])) : 0.f;
+          st[4 * i + e] = p;
+          dpt[4 * i + e] = p * (dpt[4 * i + e] - s_delta[q]);
         }
-      }
-      uint32_t pa[4], da[4];
-      pa[0] = pack_bf16(pt[0][0], pt[0][1]); pa[1] = pack_bf16(pt[0][2], pt[0][3]);
-      pa[2] = pack_bf16(pt[1][0], pt[1][1]); pa[3] = pack_bf16(pt[1][2], pt[1][3]);
-      da[0] = pack_bf16(dst[0][0], dst[0][1]); da[1] = pack_bf16(dst[0][2], dst[0][3]);
-      da[2] = pack_bf16(dst[1][0], dst[1][1]); da[3] = pack_bf16(dst[1][2], dst[1][3]);
+      uint32_t ap[4][4], ad[4][4];
+      acc_to_afrag(st, ap);
+      acc_to_afrag(dpt, ad);
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
+      wgmma_fence();
 #pragma unroll
-      for (int dp = 0; dp < 4; ++dp) {
-        uint32_t bo[4], bq[4];
-        load_b_kn(sdO, qb * 16, dp, lane, bo);
-        load_b_kn(sQ, qb * 16, dp, lane, bq);
-        mma_bf16(dv[2 * dp], pa, bo[0], bo[1]);
-        mma_bf16(dv[2 * dp + 1], pa, bo[2], bo[3]);
-        mma_bf16(dk[2 * dp], da, bq[0], bq[1]);
-        mma_bf16(dk[2 * dp + 1], da, bq[2], bq[3]);
+      for (int ks = 0; ks < 4; ++ks) {
+        wgmma_m64n64k16_rs<1>(dv, ap[ks], mndesc(sdO + qb * TILE_BYTES + ks * 16 * 128));
+        wgmma_m64n64k16_rs<1>(dk, ad[ks], mndesc(sQ + qb * TILE_BYTES + ks * 16 * 128));
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const int key = key_lo + r * 8;
-      if (key >= nq) continue;
-      if (key >= d.M) {
-        __nv_bfloat16* row = dqkv + token_row(d, b, t, key) * d.ld_qkv + h * HD + (lane & 3) * 2;
+      const int key = k_lo + r * 8;
+      if (!row_valid(key, d)) continue;
+      if (!row_global(key)) {
+        __nv_bfloat16* row = dqkv + token_row(d, b, t, row_seq(key, d)) * d.ld_qkv + h * HD + (lane & 3) * 2;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          *reinterpret_cast<uint32_t*>(row + d.C + i * 8) = pack_bf16(dk[i][2 * r], dk[i][2 * r + 1]);
-          *reinterpret_cast<uint32_t*>(row + 2 * d.C + i * 8) = pack_bf16(dv[i][2 * r], dv[i][2 * r + 1]);
+          *reinterpret_cast<uint32_t*>(row + d.C + i * 8) = pack_bf16(dk[4 * i + 2 * r], dk[4 * i + 2 * r + 1]);
+          *reinterpret_cast<uint32_t*>(row + 2 * d.C + i * 8) = pack_bf16(dv[4 * i + 2 * r], dv[4 * i + 2 * r + 1]);
         }
       } else {
-        float* g = gp + static_cast<long long>(key) * 3 * HD + (lane & 3) * 2;
+        float* g = gp + static_cast<long long>(key - GROW) * 3 * HD + (lane & 3) * 2;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          g[HD + i * 8] = dk[i][2 * r]; g[HD + i * 8 + 1] = dk[i][2 * r + 1];
-          g[2 * HD + i * 8] = dv[i][2 * r]; g[2 * HD + i * 8 + 1] = dv[i][2 * r + 1];
+          g[HD + i * 8] = dk[4 * i + 2 * r]; g[HD + i * 8 + 1] = dk[4 * i + 2 * r + 1];
+          g[2 * HD + i * 8] = dv[4 * i + 2 * r]; g[2 * HD + i * 8 + 1] = dv[4 * i + 2 * r + 1];
         }
       }
     }
   }
 
   // ---------------------------------------------------- pass B: query-stationary -> dQ
-  for (int qt = warp; qt < NTILE; qt += ATT_WARPS) {
-    if (qt * 16 >= nq) break;
-    uint32_t qa[4][4], oa[4][4];
-    load_a_frags(sQ, qt * 16, lane, qa);
-    load_a_frags(sdO, qt * 16, lane, oa);
-    float dq[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
-    const int q_lo = qt * 16 + (lane >> 2);
+  for (int qt = wg; qt < 4; qt += 2) {
+    if (!tile_live(qt, d)) continue;
+    const int q_lo = qt * 64 + wq * 16 + (lane >> 2);
     const float lse_r[2] = {s_lse[q_lo], s_lse[q_lo + 8]}, del_r[2] = {s_delta[q_lo], s_delta[q_lo + 8]};
+    float dq[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) dq[i] = 0.f;
 #pragma unroll 1
-    for (int kb = 0; kb < NTILE; ++kb) {
-      if (kb * 16 >= nq) break;
-      float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}}, dp_[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    for (int kb = 0; kb < 4; ++kb) {
+      if (!tile_live(kb, d)) continue;
+      float s[32], dp[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(dp);
+      wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        uint32_t bk[4], bv[4];
-        load_b_nk(sK, kb * 16, ks, lane, bk);
-        load_b_nk(sV, kb * 16, ks, lane, bv);
-        mma_bf16(s[0], qa[ks], bk[0], bk[1]);
-        mma_bf16(s[1], qa[ks], bk[2], bk[3]);
-        mma_bf16(dp_[0], oa[ks], bv[0], bv[1]);
-        mma_bf16(dp_[1], oa[ks], bv[2], bv[3]);
+        wgmma_m64n64k16_ss<0, 0>(s, kdesc(sQ + qt * TILE_BYTES + ks * 32), kdesc(sK + kb * TILE_BYTES + ks * 32));
+        wgmma_m64n64k16_ss<0, 0>(dp, kdesc(sdO + qt * TILE_BYTES + ks * 32), kdesc(sV + kb * TILE_BYTES + ks * 32));
       }
-      float ds[2][4];
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(dp);
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int i = 0; i < 8; ++i)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const int key = kb * 16 + i * 8 + (lane & 3) * 2 + (e & 1);
+          const int key = kb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
           const int q = q_lo + (e >> 1) * 8;
-          const bool valid = q < nq && key < nq && !(mask_gg && q < d.M && key < d.M);
-          float p;
-          p_and_ds(s[i][e], dp_[i][e], lse_r[e >> 1], del_r[e >> 1], valid, p, ds[i][e]);
+          const bool valid = row_valid(q, d) && row_valid(key, d) && !(mask_gg && row_global(q) && row_global(key));
+          const float p = valid ? fast_exp2(fmaf(s[4 * i + e], LOG2E, -lse_r[e >> 1])) : 0.f;
+          dp[4 * i + e] = p * (dp[4 * i + e] - del_r[e >> 1]);
         }
-      }
-      uint32_t da[4];
-      da[0] = pack_bf16(ds[0][0], ds[0][1]); da[1] = pack_bf16(ds[0][2], ds[0][3]);
-      da[2] = pack_bf16(ds[1][0], ds[1][1]); da[3] = pack_bf16(ds[1][2], ds[1][3]);
+      uint32_t ad[4][4];
+      acc_to_afrag(dp, ad);
+      wgmma_fence_regs(dq);
+      wgmma_fence();
 #pragma unroll
-      for (int dp = 0; dp < 4; ++dp) {
-        uint32_t bk[4];
-        load_b_kn(sK, kb * 16, dp, lane, bk);
-        mma_bf16(dq[2 * dp], da, bk[0], bk[1]);
-        mma_bf16(dq[2 * dp + 1], da, bk[2], bk[3]);
-      }
+      for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs<1>(dq, ad[ks], mndesc(sK + kb * TILE_BYTES + ks * 16 * 128));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dq);
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int q = q_lo + r * 8;
-      if (q >= nq) continue;
-      if (q >= d.M) {
-        __nv_bfloat16* row = dqkv + token_row(d, b, t, q) * d.ld_qkv + h * HD + (lane & 3) * 2;
+      if (!row_valid(q, d)) continue;
+      if (!row_global(q)) {
+        __nv_bfloat16* row = dqkv + token_row(d, b, t, row_seq(q, d)) * d.ld_qkv + h * HD + (lane & 3) * 2;
 #pragma unroll
         for (int i = 0; i < 8; ++i)
-          *reinterpret_cast<uint32_t*>(row + i * 8) = pack_bf16(dq[i][2 * r] * q_scale, dq[i][2 * r + 1] * q_scale);
+          *reinterpret_cast<uint32_t*>(row + i * 8) = pack_bf16(dq[4 * i + 2 * r] * q_scale, dq[4 * i + 2 * r + 1] * q_scale);
       } else {
-        float* g = gp + static_cast<long long>(q) * 3 * HD + (lane & 3) * 2;
+        float* g = gp + static_cast<long long>(q - GROW) * 3 * HD + (lane & 3) * 2;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          g[i * 8] = dq[i][2 * r];
-          g[i * 8 + 1] = dq[i][2 * r + 1];
+          g[i * 8] = dq[4 * i + 2 * r];
+          g[i * 8 + 1] = dq[4 * i + 2 * r + 1];
         }
       }
     }
@@ -453,9 +448,10 @@ vip_attn_bwd_combine_kernel(const float* __restrict__ gpart, __nv_bfloat16* __re
   }
 }
 
+
 static int make_dims(AttnDims& d, int B, int H, int T, int L, int M, int C) {
   if (C != H * HD) return fail("vip_attention: head_dim must be 64 (C == 64*H)");
-  if (M + L > ROWS) return fail("vip_attention: M + L must be <= 208");
+  if (M + L > 208) return fail("vip_attention: M + L must be <= 208");
   if (M < 1 || M > 8) return fail("vip_attention: 1 <= M <= 8 global tokens");
   d.B = B; d.H = H; d.T = T; d.L = L; d.M = M;
   d.S = static_cast<long long>(M) + static_cast<long long>(T) * L;
@@ -464,6 +460,16 @@ static int make_dims(AttnDims& d, int B, int H, int T, int L, int M, int C) {
   d.ld_o = C;
   return 0;
 }
+
+// TMA maps of a [B*S, width] bf16 matrix: boxes of 64 columns x L frame rows and 64 columns x M global rows
+static int make_row_maps(CUtensorMap* mL, CUtensorMap* mM, const void* base, long long width, const AttnDims& d) {
+  const uint64_t rows = static_cast<uint64_t>(d.B) * static_cast<uint64_t>(d.S);
+  if (make_tmap_bf16_2d(mL, base, width, rows, width, HD, d.L)) return -1;
+  return make_tmap_bf16_2d(mM, base, width, rows, width, HD, d.M);
+}
+
+constexpr int FWD_SMEM = 3 * MAT_BYTES + 1024 + 64;
+constexpr int BWD_SMEM = 4 * MAT_BYTES + 2 * SROWS * 4 + 1024 + 64;
 
 }  // namespace xp
 
@@ -479,15 +485,15 @@ extern "C" int xp_vip_attention_fwd(const void* qkv, void* out, float* lse, floa
   XP_ENTER(qkv);
   AttnDims d;
   if (make_dims(d, B, H, T, L, M, C)) return -1;
-  const int smem = 3 * ROWS * 128 + 128;
+  CUtensorMap mL, mM;
+  if (make_row_maps(&mL, &mM, qkv, 3LL * C, d)) return -1;
   static bool attr = false;
   if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
     attr = true;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  vip_attn_fwd_kernel<<<dim3(T, H, B), ATT_THREADS, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                                               static_cast<__nv_bfloat16*>(out), lse, workspace, d);
+  vip_attn_fwd_kernel<<<dim3(T, H, B), ATT_THREADS, FWD_SMEM, st>>>(mL, mM, static_cast<__nv_bfloat16*>(out), lse, workspace, d);
   XP_CHECK_LAUNCH("vip_attn_fwd_kernel");
   vip_attn_fwd_combine_kernel<<<dim3(H, B), 64, 0, st>>>(workspace, static_cast<__nv_bfloat16*>(out), lse, d);
   XP_CHECK_LAUNCH("vip_attn_fwd_combine_kernel");
@@ -500,51 +506,19 @@ extern "C" int xp_vip_attention_bwd(const void* qkv, const void* out, const void
   XP_ENTER(qkv);
   AttnDims d;
   if (make_dims(d, B, H, T, L, M, C)) return -1;
-  const int smem = 4 * ROWS * 128 + 2 * ROWS * 4 + 128;
+  CUtensorMap mL, mM, gL, gM;
+  if (make_row_maps(&mL, &mM, qkv, 3LL * C, d) || make_row_maps(&gL, &gM, dout, C, d)) return -1;
   static bool attr = false;
   if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     attr = true;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  vip_attn_bwd_kernel<<<dim3(T, H, B), ATT_THREADS, smem, st>>>(
-      static_cast<const __nv_bfloat16*>(qkv), static_cast<const __nv_bfloat16*>(out),
-      static_cast<const __nv_bfloat16*>(dout), lse, static_cast<__nv_bfloat16*>(dqkv), workspace, d, q_scale);
+  vip_attn_bwd_kernel<<<dim3(T, H, B), ATT_THREADS, BWD_SMEM, st>>>(
+      mL, mM, gL, gM, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse,
+      static_cast<__nv_bfloat16*>(dqkv), workspace, d, q_scale);
   XP_CHECK_LAUNCH("vip_attn_bwd_kernel");
   vip_attn_bwd_combine_kernel<<<dim3(H, B), 192, 0, st>>>(workspace, static_cast<__nv_bfloat16*>(dqkv), d, q_scale);
-  XP_CHECK_LAUNCH("vip_attn_bwd_combine_kernel");
-  return 0;
-}
-
-// tcgen05 forward (vip_attention_tc.cu) + the shared combine kernel for the global-query rows.
-extern "C" int xp_vip_attention_fwd_tc_partial(const void* qkv, void* out, float* lse, float* workspace, int32_t B,
-                                               int32_t H, int32_t T, int32_t L, int32_t M, int32_t C, void* stream);
-extern "C" int xp_vip_attention_fwd_tc(const void* qkv, void* out, float* lse, float* workspace, int32_t B, int32_t H,
-                                       int32_t T, int32_t L, int32_t M, int32_t C, void* stream) {
-  XP_ENTER(qkv);
-  AttnDims d;
-  if (make_dims(d, B, H, T, L, M, C)) return -1;
-  if (xp_vip_attention_fwd_tc_partial(qkv, out, lse, workspace, B, H, T, L, M, C, stream)) return -1;
-  vip_attn_fwd_combine_kernel<<<dim3(H, B), 64, 0, static_cast<cudaStream_t>(stream)>>>(
-      workspace, static_cast<__nv_bfloat16*>(out), lse, d);
-  XP_CHECK_LAUNCH("vip_attn_fwd_combine_kernel");
-  return 0;
-}
-
-// tcgen05 backward (vip_attention_tc.cu) + the shared combine kernel for the M global rows.
-extern "C" int xp_vip_attention_bwd_tc_partial(const void* qkv, const void* out, const void* dout, const float* lse,
-                                               void* dqkv, float* workspace, float* delta, int32_t B, int32_t H,
-                                               int32_t T, int32_t L, int32_t M, int32_t C, float q_scale, void* stream);
-extern "C" int xp_vip_attention_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
-                                       float* workspace, float* delta, int32_t B, int32_t H, int32_t T, int32_t L,
-                                       int32_t M, int32_t C, float q_scale, void* stream) {
-  XP_ENTER(qkv);
-  AttnDims d;
-  if (make_dims(d, B, H, T, L, M, C)) return -1;
-  if (xp_vip_attention_bwd_tc_partial(qkv, out, dout, lse, dqkv, workspace, delta, B, H, T, L, M, C, q_scale, stream))
-    return -1;
-  vip_attn_bwd_combine_kernel<<<dim3(H, B), 192, 0, static_cast<cudaStream_t>(stream)>>>(
-      workspace, static_cast<__nv_bfloat16*>(dqkv), d, q_scale);
   XP_CHECK_LAUNCH("vip_attn_bwd_combine_kernel");
   return 0;
 }

@@ -1,11 +1,11 @@
-"""B200-native CLIP-ViP dual encoder (video tower with video-proxy tokens + CLIP text tower).
+"""H100-native CLIP-ViP dual encoder (video tower with video-proxy tokens + CLIP text tower).
 
 Drop-in for the reference's `CLIPModel` on the VidCLIP path (CLIP-ViP/src/modeling/CLIP_ViP.py): the
 module tree below exists only to hold parameters under the reference's exact `state_dict()` names
 (SURVEY.md §8b: `vision_model.pre_layrnorm` spelling included, q/k/v kept as separate parameters), so
 released checkpoints, `named_parameters()`-driven weight-decay groups and `load_state_dict_with_mismatch`
 work unchanged.  None of these nn.Modules' own forward() is ever called: forward and backward run in one
-`torch.autograd.Function` that drives the hand-written sm_100a kernels through the C ABI (xpretrain_b200.ops).
+`torch.autograd.Function` that drives the hand-written sm_90a kernels through the C ABI (xpretrain_b200.ops).
 There is no eager / CPU fallback.
 
 Reference call stack replaced (SURVEY.md §3.2):
@@ -487,7 +487,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool):
 
     def attn_fwd(qkv, out):
         lse = torch.empty(B, H, S, dtype=f32, device=dev)
-        ops.vip_attention_fwd_tc(qkv, out, lse, ws, B, H, T, L, M, C_)
+        ops.vip_attention_fwd(qkv, out, lse, ws, B, H, T, L, M, C_)
         return lse
 
     layer_saved = []
@@ -535,11 +535,8 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
     ops.layernorm_bwd(dpooled, plain, sv.post_in[0], sv.post_in[1], vm.post_layernorm.weight, sv.meanp, sv.rstdp, None, None,
                       dx, cls_map, grads["vision_model.post_layernorm.weight"], grads["vision_model.post_layernorm.bias"], B, C_)
 
-    delta = torch.empty(B, H, S, dtype=f32, device=dev)       # rowsum(dO * O), scratch of the attention backward
-
     def attn_bwd(qkv, a, da, lse, dqkv):
-        # pipelined tcgen05 / TMEM backward (csrc/vip_attention_tc.cu); the mma.sync kernel of round 1 stays as a cross-check in tests
-        ops.vip_attention_bwd_tc(qkv, a, da, lse, dqkv, sv.ws, delta, B, H, T, L, M, C_, pk.q_scale)
+        ops.vip_attention_bwd(qkv, a, da, lse, dqkv, sv.ws, B, H, T, L, M, C_, pk.q_scale)
 
     timer = getattr(model, "block_timer", None)
     aux = _aux_stream(model, dev)
@@ -794,7 +791,7 @@ def _aux_stream(model: CLIPModel, dev):
 
 def _run(model: CLIPModel, video, input_ids, attention_mask, normalize: bool = True):
     if not model.logit_scale.is_cuda:
-        raise _lib.XpError("xpretrain_b200.CLIPModel must live on a CUDA (B200) device: there is no CPU path")
+        raise _lib.XpError("xpretrain_b200.CLIPModel must live on a CUDA (H100) device: there is no CPU path")
     params = [p for n, p in model.named_parameters() if n != "logit_scale"]
     vis, txt = _ClipVipFunction.apply(model, video, input_ids, attention_mask, normalize, torch.is_grad_enabled(), *params)
     return (vis if video is not None else None), (txt if input_ids is not None else None)

@@ -1,12 +1,12 @@
-"""LF-VILA's hierarchical video encoder (Swin-3D with growing temporal windows) on the B200 kernels — BASELINE.json config #5.
+"""LF-VILA's hierarchical video encoder (Swin-3D with growing temporal windows) on the H100 kernels — BASELINE.json config #5.
 
-Drop-in for `SwinTransformer3D` of /root/reference/LF-VILA/src/models/video_encoder.py:450-620 as `LFVILA_Pretrain` builds it from
+Drop-in for `SwinTransformer3D` of LF-VILA/src/models/video_encoder.py:450-620 as `LFVILA_Pretrain` builds it from
 `VideoEncoder` (configs/pretrain_stage1.yaml:1-11): same constructor arguments, same `state_dict()` (parameters and the
 `relative_position_index` buffers), same `forward(x[B,3,D,H,W]) -> (x, x)` with x `[B, D, H', W', C]`.
 
 The module tree only holds parameters; forward/backward run as ONE autograd.Function over token-major bf16 matrices
 `[B*D*H*W, C]` (rows in the reference's channels-last (b, d, h, w) order):
-  * PatchEmbed3D (:431-448): im2col (`xp_vip_patchify`) + tcgen05 GEMM + LayerNorm;
+  * PatchEmbed3D (:431-448): im2col (`xp_vip_patchify`) + wgmma GEMM + LayerNorm;
   * every block (:209-268): LayerNorm -> fused-qkv GEMM -> window attention -> proj GEMM (+residual) -> LayerNorm -> MLP GEMMs
     (erf-GELU epilogue, +residual).  The reference's F.pad / torch.roll / window_partition / window_reverse / crop copies (:214-243)
     do not exist: the attention kernel (`xp_seg_attention_*` in its indexed mode) reads and writes token rows through an index
@@ -115,7 +115,7 @@ class SwinTransformer3D(nn.Module):
             raise NotImplementedError("patch_size[0] must be 1 and in_chans 3 (the LF-VILA configuration)")
         for i in range(len(depths)):
             if int(embed_dim * 2 ** stages[i]) != num_heads[i] * HEAD_DIM:
-                raise ValueError("the B200 window-attention kernels are built for head_dim 32 (dim == 32 * num_heads)")
+                raise ValueError("the window-attention kernels are built for head_dim 32 (dim == 32 * num_heads)")
         self.num_layers, self.embed_dim, self.patch_norm = len(depths), embed_dim, patch_norm
         self.depths, self.num_heads, self.stages = list(depths), list(num_heads), list(stages)
         self.downsample_stages, self.window_size = list(downsample_stages), [list(w) for w in window_size]
@@ -162,7 +162,7 @@ class SwinTransformer3D(nn.Module):
 
     def forward(self, x: torch.Tensor, only_local: bool = False):
         if not x.is_cuda:
-            raise _lib.XpError("xpretrain_b200 SwinTransformer3D needs CUDA tensors on a B200: there is no CPU path")
+            raise _lib.XpError("xpretrain_b200 SwinTransformer3D needs CUDA tensors on an H100: there is no CPU path")
         if only_local:
             raise NotImplementedError("only_local=True (the early local_feat return, :604-605) is not built")
         masks = None

@@ -1,13 +1,13 @@
-"""HD-VILA's TimeSformer (divided space-time attention) on the B200 kernels — BASELINE.json config #4.
+"""HD-VILA's TimeSformer (divided space-time attention) on the H100 kernels — BASELINE.json config #4.
 
-Drop-in for `TimeSformer` of /root/reference/hd-vila/src/modeling/timesformer.py:421-525 as `HDVILA.__init__` builds it
+Drop-in for `TimeSformer` of hd-vila/src/modeling/timesformer.py:421-525 as `HDVILA.__init__` builds it
 (e2e_model.py:53-55): same constructor arguments, same `state_dict()` names and shapes (`pos_embed`, `time_embed`,
 `blocks.N.{norm1,attn.qkv,attn.proj,temporal_norm1,temporal_attn.qkv,temporal_attn.proj,temporal_fc,norm2,mlp.fc1,
 mlp.fc2}`, and the never-applied `norm`), same `forward(x[B,T,C,H,W]) -> [B,T,C,H,W]`.
 
 The module tree only holds parameters.  forward/backward run as ONE autograd.Function over token-major bf16 matrices
 `[B*H*W*T, C]` in the reference's `(h w t)` row order:
-  * every Linear is the tcgen05 GEMM (`xp_gemm`) with bias / q-scale / erf-GELU / residual epilogues,
+  * every Linear is the wgmma GEMM (`xp_gemm`) with bias / q-scale / erf-GELU / residual epilogues,
   * both attentions are `xp_seg_attention_*` reading the fused qkv buffer through strides — the six einops rearranges
     per block of timesformer.py:210-219 never materialise,
   * LayerNorm fwd/bwd are the row kernels shared with CLIP-ViP.
@@ -68,7 +68,7 @@ class TimeSformer(nn.Module):
         if attention_type != 'divided_space_time':
             raise NotImplementedError("only attention_type='divided_space_time' (the one HD-VILA uses) is built")
         if embed_dim != num_heads * 64:
-            raise ValueError("the B200 attention kernels are built for head_dim 64 (embed_dim == 64 * num_heads)")
+            raise ValueError("the attention kernels are built for head_dim 64 (embed_dim == 64 * num_heads)")
         if qk_scale is not None or drop_rate or attn_drop_rate or dropout or not qkv_bias:
             raise NotImplementedError("qk_scale / dropout / qkv_bias=False are not used by HD-VILA and are not built")
         self.depth, self.H, self.W, self.embed_dim, self.num_heads = depth, H, W, embed_dim, num_heads
@@ -122,7 +122,7 @@ class TimeSformer(nn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
-            raise _lib.XpError("xpretrain_b200 TimeSformer needs CUDA tensors on a B200: there is no CPU path")
+            raise _lib.XpError("xpretrain_b200 TimeSformer needs CUDA tensors on an H100: there is no CPU path")
         masks = None
         if self.training and self.drop_path_rate > 0:
             B, T, _, H, W = x.shape

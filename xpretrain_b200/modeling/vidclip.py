@@ -1,5 +1,5 @@
 """VidCLIP wrapper with the reference's constructor, forward signature and output keys
-(CLIP-ViP/src/modeling/VidCLIP.py:8-103), over the B200-native CLIPModel."""
+(CLIP-ViP/src/modeling/VidCLIP.py:8-103), over the H100-native CLIPModel."""
 from __future__ import annotations
 
 import copy
@@ -47,7 +47,7 @@ def config_from_args(args) -> ClipVipConfig:
         cfg.patch_size = 32
     add = _get(args, "clip_vision_additional_config")
     if _get(add, "type", "ViP") != "ViP":
-        raise NotImplementedError("only vision_additional_config.type == 'ViP' is on the B200 hot path "
+        raise NotImplementedError("only vision_additional_config.type == 'ViP' is on the H100 hot path "
                                   "(the non-ViP twin CLIP.py is an ablation baseline, SURVEY.md §2.1)")
     cfg.temporal_size = int(_get(add, "temporal_size", 12))
     cfg.if_use_temporal_embed = int(_get(add, "if_use_temporal_embed", 1))

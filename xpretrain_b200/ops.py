@@ -1,5 +1,5 @@
 """Tensor-level wrappers over the C ABI.  PyTorch supplies device memory and the current stream only;
-every computation below runs in the hand-written sm_100a kernels of libxpretrain_b200.so."""
+every computation below runs in the hand-written sm_90a kernels of libxpretrain_b200.so."""
 from __future__ import annotations
 
 import ctypes as C
@@ -39,8 +39,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
          residual: Optional[torch.Tensor] = None, ldr: int = 0, aux: Optional[torch.Tensor] = None, ld_aux: int = 0,
          act: int = _lib.ACT_NONE, out_mode: int = _lib.OUT_BF16, splits: int = 1, scale_cols: int = 0,
          col_scale: float = 1.0, alpha: float = 1.0, c_group: int = 0, c_group_stride: int = 0, r_group: int = 0,
-         r_group_stride: int = 0, block_n: int = 0, a_offset: int = 0, b_offset: int = 0, c_offset: int = 0,
-         cta_pair: int = 0) -> None:
+         r_group_stride: int = 0, block_n: int = 0, a_offset: int = 0, b_offset: int = 0, c_offset: int = 0) -> None:
     """out = epilogue(alpha * A @ B^T); offsets are in elements from the tensors' data pointers."""
     assert a.dtype == bf16 and b.dtype == bf16
     if bias is not None:
@@ -57,7 +56,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     g.a_layout, g.b_layout, g.act, g.out = a_layout, b_layout, act, out_mode
     g.splits, g.scale_cols, g.alpha, g.col_scale = splits, scale_cols, alpha, col_scale
     g.c_group, g.c_group_stride, g.r_group, g.r_group_stride = c_group, c_group_stride, r_group, r_group_stride
-    g.block_n, g.max_ctas, g.cta_pair = block_n, _sm_limit, cta_pair
+    g.block_n, g.max_ctas = block_n, _sm_limit
     if _gemm_timer is None:
         check(lib().xp_gemm(C.byref(g), _stream()), "xp_gemm")
     else:  # bench.py's roofline leg: CUDA events on the launching stream around this launch
@@ -77,7 +76,7 @@ def set_sm_limit(n: int) -> None:
     kernels of the overlapped gradient all-reduce (NCCL_MAX_CTAS), so that they never displace a persistent GEMM CTA — whose
     tiles would then run as a second, nearly empty wave (VERDICT r1: `gemm_ms_per_step` 71.3 -> 74.7 ms from 1 to 8 GPUs)."""
     global _sm_limit
-    _sm_limit = max(0, int(n)) // 2 * 2       # CTA pairs: keep it even
+    _sm_limit = max(0, int(n))
 
 
 def set_gemm_timer(records) -> None:
@@ -101,15 +100,11 @@ def linear_dgrad(dy: torch.Tensor, w: torch.Tensor, dx: torch.Tensor, **kw) -> N
 
 
 def wgrad_plan(n_out: int, n_in: int, rows: int, sms: int = 0):
-    """(block_n, splits) for a weight-gradient GEMM: the split-K factor that fills whole waves of the persistent grid.
-    Outputs of at least 256 x 256 run on CTA pairs (256 x 256 tiles, sms/2 clusters), smaller ones on single CTAs."""
-    sms = sms or _sm_limit or 148
-    pair = n_out >= 256 and n_in >= 256
+    """(block_n, splits) for a weight-gradient GEMM: the split-K factor that fills whole waves of the persistent grid
+    (one 128 x block_n tile per CTA, one CTA per SM; H100 SXM has 132 SMs)."""
+    sms = sms or _sm_limit or 132
     bn = 256 if n_in >= 256 else 128
-    if pair:
-        tiles, slots = ((n_out + 255) // 256) * ((n_in + 255) // 256), sms // 2
-    else:
-        tiles, slots = ((n_out + 127) // 128) * ((n_in + bn - 1) // bn), sms
+    tiles, slots = ((n_out + 127) // 128) * ((n_in + bn - 1) // bn), sms
     best, best_eff = 1, 0.0
     for s in range(1, 33):
         if s > 1 and rows // s < 1024:
@@ -243,19 +238,9 @@ def vip_attention_fwd(qkv, out, lse, ws, B, H, T, L, M, C_):
           "xp_vip_attention_fwd")
 
 
-def vip_attention_fwd_tc(qkv, out, lse, ws, B, H, T, L, M, C_):
-    check(lib().xp_vip_attention_fwd_tc(_p(qkv), _p(out), _p(lse), _p(ws), B, H, T, L, M, C_, _stream()),
-          "xp_vip_attention_fwd_tc")
-
-
 def vip_attention_bwd(qkv, out, dout, lse, dqkv, ws, B, H, T, L, M, C_, q_scale):
     check(lib().xp_vip_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(dqkv), _p(ws), B, H, T, L, M, C_, q_scale,
                                      _stream()), "xp_vip_attention_bwd")
-
-
-def vip_attention_bwd_tc(qkv, out, dout, lse, dqkv, ws, delta, B, H, T, L, M, C_, q_scale):
-    check(lib().xp_vip_attention_bwd_tc(_p(qkv), _p(out), _p(dout), _p(lse), _p(dqkv), _p(ws), _p(delta), B, H, T, L, M,
-                                        C_, q_scale, _stream()), "xp_vip_attention_bwd_tc")
 
 
 def text_attention_fwd(qkv, mask, out, probs, B, H, Lt, C_):

@@ -1,4 +1,4 @@
-"""The reference's optimizer step on the B200: AdamW ("weight decay fix") + global-norm clipping + LR schedule + grouping.
+"""The reference's optimizer step on the H100: AdamW ("weight decay fix") + global-norm clipping + LR schedule + grouping.
 
 Drop-in for CLIP-ViP/src/optimization:
   * `AdamW(params, lr, betas, eps=1e-6, weight_decay, correct_bias)` — adamw.py:11-39 constructor, same `state`

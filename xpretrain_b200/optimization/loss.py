@@ -1,9 +1,9 @@
-"""In-batch video<->text InfoNCE with learnable temperature on the B200 kernels.
+"""In-batch video<->text InfoNCE with learnable temperature on the H100 kernels.
 
 API mirrors CLIP-ViP/src/optimization/loss.py: `build_loss_func(cfg)` (:326-328) returns a module whose
 `forward(vis_feat, text_feat, temp)` equals `NCELearnableTempLoss.forward` (:134-141):
     logits = vis @ text.T * exp(temp);  loss = CE(logits, arange) + CE(logits.T, arange)      (sum, no 1/2)
-The logits GEMM and both gradient GEMMs run on the tcgen05 GEMM; softmax / loss / dL/dZ in nce.cu.
+The logits GEMM and both gradient GEMMs run on the wgmma GEMM; softmax / loss / dL/dZ in nce.cu.
 `gather_nce_loss` is the fused multi-GPU form (embedding all-gather + loss, backward without a collective).
 """
 from __future__ import annotations
@@ -22,11 +22,11 @@ def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
-FUSED_MAX_N = 1536      # (N / 128)^2 tiles of the fused kernel must be co-resident on the 148 SMs
+FUSED_MAX_N = 1536      # (N / 128)^2 tiles of the fused kernel must be co-resident: up to two per SM on the 132 SMs of an H100
 
 
 def _nce_forward_unfused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor):
-    """Global batches above FUSED_MAX_N: split / tcgen05 GEMM / softmax-grad as separate launches.
+    """Global batches above FUSED_MAX_N: split / GEMM / softmax-grad as separate launches.
     vis, txt: [N, d] fp32 (gathered).  Returns (loss[1], g_scaled[N, Np] bf16, vis_hi, txt_hi, dscale[1])."""
     N, d = vis.shape
     Np = _pad8(N)
@@ -242,7 +242,7 @@ def _split_hi(x: torch.Tensor, rows_pad: int, pattern: int):
 
 
 class _NceVscFcFunction(torch.autograd.Function):
-    """NCELearnableTempLoss_vsc_fc (loss.py:288-324): three hi/lo-split tcgen05 logits GEMMs (V T^T, V C^T, I C^T), the
+    """NCELearnableTempLoss_vsc_fc (loss.py:288-324): three hi/lo-split logits GEMMs (V T^T, V C^T, I C^T), the
     six-term softmax / loss / dL/dZ kernels of nce.cu, and six gradient GEMMs in backward."""
 
     @staticmethod
@@ -307,6 +307,6 @@ def build_loss_func(cfg):
     """loss.py:326-328: `cfg.loss_name` selects the class."""
     name = cfg["loss_name"] if isinstance(cfg, dict) else cfg.loss_name
     if name not in _LOSSES:
-        raise NotImplementedError(f"loss {name!r} is outside the B200 hot path (SURVEY.md §8f lists it as 'next'); "
+        raise NotImplementedError(f"loss {name!r} is outside the H100 hot path (SURVEY.md §8f lists it as 'next'); "
                                   f"available: {sorted(_LOSSES)}")
     return _LOSSES[name](cfg)

@@ -1,4 +1,4 @@
-"""Data-parallel plumbing over torch.distributed (NCCL on B200 / gloo in CPU tests).
+"""Data-parallel plumbing over torch.distributed (NCCL on GPUs / gloo in CPU tests).
 
 Replaces the Horovod calls on the hot path (CLIP-ViP/src/utils/distributed.py, run_pretrain.py:226-232,344-353):
 one process per GPU, rank-major differentiable all-gather of the embeddings, bucketed gradient averaging.

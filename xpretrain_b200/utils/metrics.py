@@ -1,4 +1,4 @@
-"""Retrieval evaluation on the B200 (SURVEY.md §8f.3) — drop-in for CLIP-ViP/src/utils/metrics.py as validate() uses it
+"""Retrieval evaluation on the H100 (SURVEY.md §8f.3) — drop-in for CLIP-ViP/src/utils/metrics.py as validate() uses it
 (run_pretrain.py:173-176, tasks/run_video_retrieval.py:155-172).
 
     sim = cal_cossim(text_feats, vis_feats)        # CUDA fp32 tensors stay on the device (no .cpu().numpy() per batch)
