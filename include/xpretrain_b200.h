@@ -216,12 +216,50 @@ typedef struct XpNceGather {
 int64_t xp_nce_gather_exchange_bytes(int32_t b, int32_t d, int32_t world);
 int64_t xp_nce_gather_workspace_bytes(int32_t N);
 int xp_nce_gather_fused(const XpNceGather* args, void* stream);
-/* NCELearnableTempLoss_vsc_fc.forward, CLIP-ViP/src/optimization/loss.py:288-324 (the released pre-training default:
- * video x subtitle, video x caption, frame x caption): za = V T^T, zb = V C^T, zd = I C^T, fp32 [N, N] with row pitch ld,
- * unscaled.  Writes the scalar loss (overwritten), ACCUMULATES d_logit_scale, and the three gradient matrices
- * g* = exp(logit_scale) * dL/d(s z*) as bf16 [N, N] (row pitch ld).  stats: 6*N floats of scratch. */
-int xp_nce_vsc_fc(const float* za, const float* zb, const float* zd, const float* logit_scale, float* stats, void* ga_bf16,
-                  void* gb_bf16, void* gd_bf16, float* loss, float* d_logit_scale, int32_t N, int64_t ld, void* stream);
+/* The contrastive losses of CLIP-ViP/src/optimization/loss.py as one table: NCEContrastiveLoss (:67-83, fixed temperature),
+ * VidImgDivideNCELearnableTempLoss (:162-183), NCELearnableTempLoss_vs_vc (:204-225), _vs_vc_fc (:227-254), _vsc (:256-286)
+ * and _vsc_fc (:288-324).  z[m] is matrix m's UNSCALED logits, fp32 [n[m], n[m]] with row pitch ld[m] (>= n[m], a multiple
+ * of 4, 16-byte aligned), scaled by s = exp(*logit_scale) or, when logit_scale is NULL, by the host constant `scale`.
+ * A term is one cross-entropy averaged over its n rows (axis 0) or columns (axis 1): for index i,
+ *   LSE over the union of row / column i of every member matrix (bit m of `members`), without the diagonal entry of the
+ *   members in `excl_diag`, minus s * z[target][i, i].
+ * The members of a term share one n; the target is a member and keeps its diagonal.  Outputs: loss = sum of the terms
+ * (overwritten); d_logit_scale = dL/d logit_scale (overwritten; only with a device logit_scale, may be NULL otherwise);
+ * g[m] = s * dL/d(s z[m]) as bf16 [n[m], ld[m]] (8-byte aligned; columns n..ceil4(n) written as 0, the rest of the pitch
+ * untouched), which is what the two gradient GEMMs dX = g Y, dY = g^T X per matrix consume.  workspace:
+ * xp_nce_terms_workspace_bytes(args) bytes, no initialisation needed.  Four launches; loss, d_logit_scale and g are
+ * bit-identical across calls (fixed-order reductions, no float atomics). */
+typedef struct XpNceTerm {
+  int32_t axis;       /* 0 = rows, 1 = columns */
+  int32_t members;    /* bit m: matrix m is part of the union */
+  int32_t excl_diag;  /* bit m: matrix m enters without its diagonal entry */
+  int32_t target;     /* matrix whose diagonal entry is the label */
+} XpNceTerm;
+typedef struct XpNceTerms {
+  const float* z[3];
+  void* g[3];
+  int64_t ld[3];
+  int32_t n[3];
+  int32_t n_mats, n_terms;
+  XpNceTerm term[6];
+  const float* logit_scale;
+  float scale;
+  float* loss;
+  float* d_logit_scale;
+  float* workspace;
+} XpNceTerms;
+int64_t xp_nce_terms_workspace_bytes(const XpNceTerms* args);
+int xp_nce_terms(const XpNceTerms* args, void* stream);
+/* NCELearnableTempDSLLoss.forward, CLIP-ViP/src/optimization/loss.py:185-202 (the training-time dual softmax): with
+ * Z = exp(*logit_scale) * z, Pc / Pr its column / row softmax, A' = Z Pc and B' = Z Pr,
+ *   loss = mean_i(LSE_j A'_ij - A'_ii) + mean_j(LSE_i B'_ij - B'_jj)       (overwritten)
+ * and, the re-weighting not being detached, G_Z = Pc (GA (1 + Z) - u_j) + Pr (GB (1 + Z) - w_i) with GA, GB the two
+ * cross-entropy gradients, u_j = sum_i GA Z Pc, w_i = sum_j GB Z Pr.  g_bf16 = s * G_Z, bf16 [n, ld]; d_logit_scale =
+ * sum G_Z Z (overwritten).  z, ld, alignment as for xp_nce_terms; workspace: xp_nce_dsl_workspace_bytes(n) bytes.
+ * Eight launches, bit-identical across calls. */
+int64_t xp_nce_dsl_workspace_bytes(int32_t n);
+int xp_nce_dsl(const float* z, int64_t ld, int32_t n, const float* logit_scale, void* g_bf16, float* loss,
+               float* d_logit_scale, float* workspace, void* stream);
 
 /* ---- BASELINE.json config #4: HD-VILA TimeSformer (divided space-time attention), hd-vila/src/modeling/timesformer.py
  *

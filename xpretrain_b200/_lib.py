@@ -45,6 +45,16 @@ class XpNceGather(C.Structure):
                 ("d", c_int), ("epoch", C.c_uint32), ("mode", c_int), ("ld_g", c_i64)]
 
 
+class XpNceTerm(C.Structure):
+    _fields_ = [("axis", c_int), ("members", c_int), ("excl_diag", c_int), ("target", c_int)]
+
+
+class XpNceTerms(C.Structure):
+    _fields_ = [("z", c_void_p * 3), ("g", c_void_p * 3), ("ld", c_i64 * 3), ("n", c_int * 3), ("n_mats", c_int),
+                ("n_terms", c_int), ("term", XpNceTerm * 6), ("logit_scale", c_void_p), ("scale", c_float),
+                ("loss", c_void_p), ("d_logit_scale", c_void_p), ("workspace", c_void_p)]
+
+
 ACT_NONE, ACT_QUICK_GELU, ACT_DQUICK_GELU, ACT_GELU_ERF, ACT_DGELU_ERF = 0, 1, 2, 3, 4
 OUT_BF16, OUT_F32, OUT_F32_ATOMIC = 0, 1, 2
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
@@ -92,8 +102,10 @@ SIGNATURES = {
     "xp_nce_gather_exchange_bytes": (c_i64, [c_int, c_int, c_int]),
     "xp_nce_gather_workspace_bytes": (c_i64, [c_int]),
     "xp_nce_gather_fused": (c_int, [P(XpNceGather), c_void_p]),
-    "xp_nce_vsc_fc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                              c_void_p, c_int, c_i64, c_void_p]),
+    "xp_nce_terms_workspace_bytes": (c_i64, [P(XpNceTerms)]),
+    "xp_nce_terms": (c_int, [P(XpNceTerms), c_void_p]),
+    "xp_nce_dsl_workspace_bytes": (c_i64, [c_int]),
+    "xp_nce_dsl": (c_int, [c_void_p, c_i64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xp_seg_attention_fwd":(c_int, [c_void_p, c_void_p, c_void_p, P(XpSegAttn), c_void_p]),
     "xp_seg_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, P(XpSegAttn), c_float,
                                      c_void_p]),

@@ -265,11 +265,36 @@ def nce_softmax_grad(z, logit_scale, lse_r, lse_c, g_scaled, loss, d_logit_scale
                                     _p(d_logit_scale), N, ld, _stream()), "xp_nce_softmax_grad")
 
 
-def nce_vsc_fc(za, zb, zd, logit_scale, stats, ga, gb, gd, loss, d_logit_scale):
-    N, ld = za.shape[0], za.stride(0)
-    assert zb.stride(0) == ld and zd.stride(0) == ld and ga.stride(0) == ld and stats.numel() >= 6 * N
-    check(lib().xp_nce_vsc_fc(_p(za), _p(zb), _p(zd), _p(logit_scale), _p(stats), _p(ga), _p(gb), _p(gd), _p(loss),
-                              _p(d_logit_scale), N, ld, _stream()), "xp_nce_vsc_fc")
+def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logit_scale=None):
+    """Loss, d logit_scale and s * dL/dZ of a table of cross-entropy terms over up to three logits matrices (xp_nce_terms).
+    z: fp32 [n_m, ld_m] unscaled logits; g: matching bf16 outputs; terms: (axis, members, excl_diag, target) per term, with
+    members / excl_diag as bit masks over the matrices.  The scale is exp(logit_scale[0]) or, without logit_scale, `scale`."""
+    a = _lib.XpNceTerms()
+    a.n_mats, a.n_terms = len(z), len(terms)
+    for m, (zm, gm) in enumerate(zip(z, g)):
+        assert zm.dtype == f32 and gm.dtype == bf16 and zm.stride(1) == 1 and gm.stride(0) == zm.stride(0)
+        a.z[m], a.g[m], a.ld[m], a.n[m] = _p(zm), _p(gm), zm.stride(0), zm.shape[0]
+    for t, (axis, members, excl, target) in enumerate(terms):
+        a.term[t].axis, a.term[t].members, a.term[t].excl_diag, a.term[t].target = axis, members, excl, target
+    a.logit_scale, a.scale, a.loss, a.d_logit_scale = _p(logit_scale), scale, _p(loss), _p(d_logit_scale)
+    nbytes = int(lib().xp_nce_terms_workspace_bytes(C.byref(a)))
+    if nbytes < 0:
+        raise _lib.XpError("xp_nce_terms_workspace_bytes: invalid matrix sizes")
+    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z[0].device)
+    a.workspace = _p(ws)
+    check(lib().xp_nce_terms(C.byref(a), _stream()), "xp_nce_terms")
+
+
+def nce_dsl(z, logit_scale, g, loss, d_logit_scale):
+    """NCELearnableTempDSLLoss on the unscaled logits z fp32 [n, ld]: loss, d logit_scale and s * dL/dZ (bf16, pitch ld)."""
+    n, ld = z.shape[0], z.stride(0)
+    assert z.dtype == f32 and g.dtype == bf16 and g.stride(0) == ld
+    nbytes = int(lib().xp_nce_dsl_workspace_bytes(n))
+    if nbytes < 0:
+        raise _lib.XpError("xp_nce_dsl_workspace_bytes: n must be positive")
+    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z.device)
+    check(lib().xp_nce_dsl(_p(z), ld, n, _p(logit_scale), _p(g), _p(loss), _p(d_logit_scale), _p(ws), _stream()),
+          "xp_nce_dsl")
 
 
 # ------------------------------------------------------------- config #4: TimeSformer (HD-VILA)

@@ -1,4 +1,4 @@
-"""In-batch video<->text InfoNCE with learnable temperature on the H100 kernels.
+"""The contrastive losses of CLIP-ViP/src/optimization/loss.py on the H100 kernels.
 
 API mirrors CLIP-ViP/src/optimization/loss.py: `build_loss_func(cfg)` (:326-328) returns a module whose
 `forward(vis_feat, text_feat, temp)` equals `NCELearnableTempLoss.forward` (:134-141):
@@ -241,72 +241,211 @@ def _split_hi(x: torch.Tensor, rows_pad: int, pattern: int):
     return x3, hi
 
 
-class _NceVscFcFunction(torch.autograd.Function):
-    """NCELearnableTempLoss_vsc_fc (loss.py:288-324): three hi/lo-split logits GEMMs (V T^T, V C^T, I C^T), the
-    six-term softmax / loss / dL/dZ kernels of nce.cu, and six gradient GEMMs in backward."""
+# ------------------------------------------------------------------------------------------------------------------------
+# The other contrastive losses of loss.py.  Each one is a table: the logits matrices as (row features, column features)
+# indices into the forward's arguments, and the cross-entropy terms as (axis, members, excl_diag, target) with members /
+# excl_diag bit masks over the matrices (include/xpretrain_b200.h, XpNceTerms).  Forward: one hi/lo-split logits GEMM per
+# matrix, then xp_nce_terms (loss, d logit_scale and s * dL/dZ per matrix); backward: two gradient GEMMs per matrix.
+ROW, COL = 0, 1
+_A, _B, _D = 1, 2, 4          # matrix bits: A = s V T^T, B = s V C^T, D = s I C^T (in this order in each table below)
+_VTCI = ((0, 1), (0, 3), (2, 3))
+
+TERM_TABLES = {
+    # loss.py:76-83 (fixed temperature) and :162-183: rows and columns of V T^T (and of I C^T, whose n may differ)
+    "NCEContrastiveLoss": (((0, 1),), ((ROW, _A, 0, 0), (COL, _A, 0, 0))),
+    "VidImgDivideNCELearnableTempLoss": (((0, 1), (2, 3)), ((ROW, 1, 0, 0), (COL, 1, 0, 0), (ROW, 2, 0, 1), (COL, 2, 0, 1))),
+    # loss.py:212-225, :235-254: rows and columns of each matrix
+    "NCELearnableTempLoss_vs_vc": (_VTCI[:2], ((ROW, _A, 0, 0), (COL, _A, 0, 0), (ROW, _B, 0, 1), (COL, _B, 0, 1))),
+    "NCELearnableTempLoss_vs_vc_fc": (_VTCI, ((ROW, _A, 0, 0), (COL, _A, 0, 0), (ROW, _B, 0, 1), (COL, _B, 0, 1),
+                                              (ROW, _D, 0, 2), (COL, _D, 0, 2))),
+    # loss.py:264-286: columns of A and B; per row i, [A_ii | A_i,j!=i | B_i,j!=i] and [B_ii | A_i,j!=i | B_i,j!=i]
+    "NCELearnableTempLoss_vsc": (_VTCI[:2], ((COL, _A, 0, 0), (COL, _B, 0, 1), (ROW, _A | _B, _B, 0),
+                                             (ROW, _A | _B, _A, 1))),
+    # loss.py:296-324: the _vsc terms plus the columns and rows of D
+    "NCELearnableTempLoss_vsc_fc": (_VTCI, ((COL, _A, 0, 0), (COL, _B, 0, 1), (ROW, _A | _B, _B, 0), (ROW, _A | _B, _A, 1),
+                                            (COL, _D, 0, 2), (ROW, _D, 0, 2))),
+}
+
+
+def _check_square(name: str, feats, pairs) -> None:
+    """ValueError (before any launch) unless every features matrix used is 2-D with one width and every logits matrix
+    X Y^T is square, as the reference's arange labels require."""
+    used = sorted({i for pr in pairs for i in pr})
+    for i in used:
+        if feats[i].dim() != 2:
+            raise ValueError(f"{name}: argument {i} must be a 2-D [rows, dim] feature matrix, got shape {tuple(feats[i].shape)}")
+    if len({feats[i].shape[1] for i in used}) != 1:
+        raise ValueError(f"{name}: feature widths differ: {[tuple(feats[i].shape) for i in used]}")
+    for r, c in pairs:
+        if feats[r].shape[0] != feats[c].shape[0]:
+            raise ValueError(f"{name}: argument {r} has {feats[r].shape[0]} rows but argument {c} has {feats[c].shape[0]}; "
+                             f"their logits matrix must be square")
+
+
+class _NceTermsFunction(torch.autograd.Function):
+    """Any TERM_TABLES entry.  temp: the learnable log-scale tensor (s = exp(temp)), or None with s = `scale`."""
 
     @staticmethod
-    def forward(ctx, vis, txt, img, cap, temp):
-        assert txt.shape[0] == cap.shape[0]                                   # loss.py:290
-        N, d = vis.shape
-        Np, dev = _pad8(N), vis.device
-        v3, vh = _split_hi(vis.to(f32), N, 0)
-        i3, ih = _split_hi(img.to(f32), N, 0)
-        t3, th = _split_hi(txt.to(f32), Np, 1)
-        c3, ch = _split_hi(cap.to(f32), Np, 1)
-        z = torch.empty(3, N, Np, dtype=f32, device=dev)
-        for k, (a, b) in enumerate(((v3, t3), (v3, c3), (i3, c3))):
-            ops.gemm(a, b, z[k], M=N, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
-        g = torch.empty(3, N, Np, dtype=bf16, device=dev)
-        stats = torch.empty(6 * N, dtype=f32, device=dev)
+    def forward(ctx, table, scale, temp, *feats):
+        pairs, terms = table
+        d, dev = next(feats[i] for pr in pairs for i in pr).shape[1], feats[pairs[0][0]].device
+        role = {}
+        for r, c in pairs:
+            role[r], role[c] = 0, 1
+        assert len(role) == len({i for pr in pairs for i in pr})                # no feature is both a row and a column side
+        split = {i: _split_hi(feats[i].to(f32), feats[i].shape[0] if pat == 0 else _pad8(feats[i].shape[0]), pat)
+                 for i, pat in role.items()}
+        z, g = [], []
+        for r, c in pairs:
+            n = feats[r].shape[0]
+            Np = _pad8(n)
+            zk = torch.empty(n, Np, dtype=f32, device=dev)
+            ops.gemm(split[r][0], split[c][0], zk, M=n, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
+            z.append(zk)
+            g.append(torch.empty(n, Np, dtype=bf16, device=dev))
         loss = torch.empty(1, dtype=f32, device=dev)
-        dscale = torch.zeros(1, dtype=f32, device=dev)
-        ops.nce_vsc_fc(z[0], z[1], z[2], temp.detach().reshape(1).to(f32), stats, g[0], g[1], g[2], loss, dscale)
-        ctx.saved = (g, vh, th, ih, ch, dscale)
-        ctx.in_meta = (vis.dtype, txt.dtype, img.dtype, cap.dtype, temp.dtype, temp.shape)
+        dscale = torch.empty(1, dtype=f32, device=dev) if temp is not None else None
+        ops.nce_terms(z, g, terms, loss, logit_scale=temp.detach().reshape(1).to(f32) if temp is not None else None,
+                      scale=scale, d_logit_scale=dscale)
+        ctx.saved = (g, {i: hi for i, (_, hi) in split.items()}, dscale)
+        ctx.meta = (pairs, len(feats), [f.dtype for f in feats], None if temp is None else (temp.dtype, temp.shape))
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx, dloss):
-        g, vh, th, ih, ch, dscale = ctx.saved
-        N, d = vh.shape
-        Np, dev = g.shape[2], g.device
-        out = torch.zeros(4, N, d, dtype=f32, device=dev)                     # d_vis, d_txt, d_img, d_cap (atomic accumulation)
-
-        def rows_times(gk, feat, dst):       # dst += G_k  @ feat   (A = G_k rows, K-major; B = feat [K=N, d] MN-major)
-            ops.gemm(gk, feat, dst, M=N, N=d, K=N, lda=Np, ldb=d, ldc=d, b_layout=1, out_mode=_lib.OUT_F32_ATOMIC)
-
-        def cols_times(gk, feat, dst):       # dst += G_k^T @ feat  (A = G_k^T: MN-major)
-            ops.gemm(gk, feat, dst, M=N, N=d, K=N, lda=Np, ldb=d, ldc=d, a_layout=1, b_layout=1,
+        g, hi, dscale = ctx.saved
+        pairs, n_feats, dtypes, tmeta = ctx.meta
+        out = {i: torch.zeros(h.shape[0], h.shape[1], dtype=f32, device=h.device) for i, h in hi.items()}
+        for gk, (r, c) in zip(g, pairs):
+            n, Np, d = gk.shape[0], gk.shape[1], hi[r].shape[1]
+            # d_row += G_k @ col_feats (A = G_k rows, K-major);  d_col += G_k^T @ row_feats (A = G_k^T, MN-major)
+            ops.gemm(gk, hi[c], out[r], M=n, N=d, K=n, lda=Np, ldb=d, ldc=d, b_layout=1, out_mode=_lib.OUT_F32_ATOMIC)
+            ops.gemm(gk, hi[r], out[c], M=n, N=d, K=n, lda=Np, ldb=d, ldc=d, a_layout=1, b_layout=1,
                      out_mode=_lib.OUT_F32_ATOMIC)
-
-        rows_times(g[0], th, out[0]); rows_times(g[1], ch, out[0])            # dV = s (G_a T + G_b C)
-        cols_times(g[0], vh, out[1])                                          # dT = s G_a^T V
-        rows_times(g[2], ch, out[2])                                          # dI = s G_d C
-        cols_times(g[1], vh, out[3]); cols_times(g[2], ih, out[3])            # dC = s (G_b^T V + G_d^T I)
-        vd, td, idt, cd, pd, pshape = ctx.in_meta
-        return ((out[0] * dloss).to(vd), (out[1] * dloss).to(td), (out[2] * dloss).to(idt), (out[3] * dloss).to(cd),
-                (dscale * dloss).reshape(pshape).to(pd))
+        grads = [(out[i] * dloss).to(dtypes[i]) if i in out else None for i in range(n_feats)]
+        dtemp = None if tmeta is None else (dscale * dloss).reshape(tmeta[1]).to(tmeta[0])
+        return (None, None, dtemp, *grads)
 
 
-class NCELearnableTempLoss_vsc_fc(nn.Module):
-    """Drop-in for loss.py:280-324 — the released pre-training default (pretrain_vip_base_16.json:74-77):
-    forward(vis_feat, text_feat, img_feat, cap_feat, temp) on the (gathered) feature matrices."""
+def _table_loss(name: str, feats, temp=None, scale: float = 1.0):
+    table = TERM_TABLES[name]
+    _check_square(name, feats, table[0])
+    return _NceTermsFunction.apply(table, scale, temp, *feats)
+
+
+class _NceDslFunction(torch.autograd.Function):
+    """NCELearnableTempDSLLoss (loss.py:185-202): hi/lo-split logits GEMM, the DSL chain of xp_nce_dsl, and the two
+    gradient GEMMs of the plain InfoNCE in backward (the re-weighting's own gradient is inside G_Z)."""
+
+    @staticmethod
+    def forward(ctx, vis, txt, temp):
+        N, d = vis.shape
+        Np, dev = _pad8(N), vis.device
+        v3, vh = _split_hi(vis.to(f32), N, 0)
+        t3, th = _split_hi(txt.to(f32), Np, 1)
+        z = torch.empty(N, Np, dtype=f32, device=dev)
+        ops.gemm(v3, t3, z, M=N, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
+        g = torch.empty(N, Np, dtype=bf16, device=dev)
+        loss = torch.empty(1, dtype=f32, device=dev)
+        dscale = torch.empty(1, dtype=f32, device=dev)
+        ops.nce_dsl(z, temp.detach().reshape(1).to(f32), g, loss, dscale)
+        ctx.saved = (g, vh, th, dscale)
+        ctx.in_dtypes = (vis.dtype, txt.dtype, temp.dtype, temp.shape)
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, dloss):
+        g, vh, th, dscale = ctx.saved
+        d_vis, d_txt = _nce_backward(g, vh, th, 0, vh.shape[0], 1.0)
+        vd, td, pd, pshape = ctx.in_dtypes
+        return (d_vis * dloss).to(vd), (d_txt * dloss).to(td), (dscale * dloss).reshape(pshape).to(pd)
+
+
+def _cfg_value(cfg, key):
+    return cfg[key] if isinstance(cfg, dict) else getattr(cfg, key)
+
+
+class NCEContrastiveLoss(nn.Module):
+    """Drop-in for loss.py:67-83: InfoNCE at the fixed temperature cfg.temp (logits / temp), no temperature gradient."""
+
+    def __init__(self, cfg):
+        super().__init__()
+        self.temp = _cfg_value(cfg, "temp")
+
+    def forward(self, vis_feat, text_feat):
+        return _table_loss("NCEContrastiveLoss", (vis_feat, text_feat), scale=1.0 / float(self.temp))
+
+
+class NCELearnableTempDSLLoss(nn.Module):
+    """Drop-in for loss.py:185-202: InfoNCE over the dual-softmax re-weighted logits Z * softmax(Z, 0) (rows) and
+    Z^T * softmax(Z^T, 0) (columns); the retrieval fine-tuning loss (run_video_retrieval.py:333-338)."""
+
+    def __init__(self, cfg=None):
+        super().__init__()
+
+    def forward(self, vis_feat, text_feat, temp):
+        _check_square("NCELearnableTempDSLLoss", (vis_feat, text_feat), ((0, 1),))
+        return _NceDslFunction.apply(vis_feat, text_feat, temp)
+
+
+class VidImgNCELearnableTempLoss(nn.Module):
+    """Drop-in for loss.py:143-160: NCELearnableTempLoss over [V; I] x [T; C]."""
 
     def __init__(self, cfg=None):
         super().__init__()
 
     def forward(self, vis_feat, text_feat, img_feat, cap_feat, temp):
-        return _NceVscFcFunction.apply(vis_feat, text_feat, img_feat, cap_feat, temp)
+        feats = (vis_feat, text_feat, img_feat, cap_feat)
+        for f in feats:
+            if f.dim() != 2 or f.shape[1] != vis_feat.shape[-1]:
+                raise ValueError(f"VidImgNCELearnableTempLoss: every input must be [rows, {vis_feat.shape[-1]}], got "
+                                 f"{[tuple(x.shape) for x in feats]}")
+        if vis_feat.shape[0] + img_feat.shape[0] != text_feat.shape[0] + cap_feat.shape[0]:
+            raise ValueError("VidImgNCELearnableTempLoss: len(vis) + len(img) must equal len(text) + len(cap)")
+        if not all(f.is_cuda for f in feats):
+            raise _lib.XpError("xpretrain_b200 kernels need CUDA tensors (there is no CPU path)")
+        return _NceFunction.apply(torch.cat([vis_feat, img_feat], 0), torch.cat([text_feat, cap_feat], 0), temp)
 
 
-_LOSSES = {"NCELearnableTempLoss": NCELearnableTempLoss, "NCELearnableTempLoss_vsc_fc": NCELearnableTempLoss_vsc_fc}
+def _table_module(name: str, doc: str):
+    class _M(nn.Module):
+        __doc__ = doc
+
+        def __init__(self, cfg=None):
+            super().__init__()
+
+        def forward(self, vis_feat, text_feat, img_feat, cap_feat, temp):
+            return _table_loss(name, (vis_feat, text_feat, img_feat, cap_feat), temp)
+
+    _M.__name__ = _M.__qualname__ = name
+    return _M
+
+
+VidImgDivideNCELearnableTempLoss = _table_module(
+    "VidImgDivideNCELearnableTempLoss", "Drop-in for loss.py:162-183: InfoNCE of V T^T plus InfoNCE of I C^T (I, C may have "
+    "their own batch size).")
+NCELearnableTempLoss_vs_vc = _table_module(
+    "NCELearnableTempLoss_vs_vc", "Drop-in for loss.py:204-225: InfoNCE of video x subtitle plus video x caption.")
+NCELearnableTempLoss_vs_vc_fc = _table_module(
+    "NCELearnableTempLoss_vs_vc_fc", "Drop-in for loss.py:227-254: InfoNCE of video x subtitle, video x caption and frame x "
+    "caption.")
+NCELearnableTempLoss_vsc = _table_module(
+    "NCELearnableTempLoss_vsc", "Drop-in for loss.py:256-286: column InfoNCE of V T^T and V C^T, and per video the joint "
+    "softmax over its subtitle and caption negatives.")
+NCELearnableTempLoss_vsc_fc = _table_module(
+    "NCELearnableTempLoss_vsc_fc", "Drop-in for loss.py:288-324 — the released pre-training default "
+    "(pretrain_vip_base_16.json:74-77): the _vsc terms plus InfoNCE of frame x caption.")
+
+_LOSSES = {c.__name__: c for c in (
+    NCELearnableTempLoss, NCEContrastiveLoss, NCELearnableTempDSLLoss, VidImgNCELearnableTempLoss,
+    VidImgDivideNCELearnableTempLoss, NCELearnableTempLoss_vs_vc, NCELearnableTempLoss_vs_vc_fc, NCELearnableTempLoss_vsc,
+    NCELearnableTempLoss_vsc_fc)}
 
 
 def build_loss_func(cfg):
-    """loss.py:326-328: `cfg.loss_name` selects the class."""
+    """loss.py:326-328: `cfg.loss_name` selects the class.  TripletContrastiveLoss, HardNegLoss and MILNCEContrastiveLoss
+    (legacy two-argument losses no released config selects) are not built."""
     name = cfg["loss_name"] if isinstance(cfg, dict) else cfg.loss_name
     if name not in _LOSSES:
-        raise NotImplementedError(f"loss {name!r} is outside the H100 hot path (SURVEY.md §8f lists it as 'next'); "
-                                  f"available: {sorted(_LOSSES)}")
+        raise NotImplementedError(f"loss {name!r} is not built on the H100 path; available: {sorted(_LOSSES)}")
     return _LOSSES[name](cfg)
