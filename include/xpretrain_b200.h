@@ -65,7 +65,7 @@ typedef struct XpGemm {
    * C (and aux) use c_group; residual uses r_group (r_group_stride = 0 makes the residual a
    * periodic [r_group, N] table, used for the patch-embedding position+temporal add). */
   int64_t c_group, c_group_stride, r_group, r_group_stride;
-  int32_t block_n;    /* 0 = auto, else 128 or 256 */
+  int32_t block_n;    /* 0 = auto, 128 = ping-pong 128x128 tiles, 256 = cooperative 128x256 tiles */
   int32_t max_ctas;   /* 0 = one persistent CTA per SM */
   int32_t cta_pair;   /* 0 or 1: single-CTA tiles (sm_90 has no CTA pairs; other values are rejected) */
   int32_t reserved;

@@ -173,6 +173,25 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "n"(TB));
 }
 
+// ------------------------------------------------------- warpgroup registers / named barriers
+// Move per-thread registers between the warpgroups of a CTA (sm_90a).  Every warp of the warpgroup executes it; the
+// count is a multiple of 8 in [24, 256].
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+// Named barrier `id` (1-15; 0 is __syncthreads) over `threads` threads: bar.sync waits, bar.arrive only counts.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor, sm_90 wgmma format (cute/arch/mma_sm90_desc.hpp documents the bit layout):
 // start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64) with SWIZZLE_128B = 1.
@@ -189,6 +208,25 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
 }
 
 // ------------------------------------------------------------------- misc
+// Transpose a 4 x 4 matrix of 32-bit words held by the four lanes of each quad (lanes 4m .. 4m + 3): afterwards lane q
+// holds in v[j] what lane j held in v[q].  Every lane of the warp must call it.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4]) {
+  const int q = threadIdx.x & 3;
+  uint32_t out[4];
+  out[0] = out[1] = out[2] = out[3] = 0u;
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int j = q ^ t;   // the partner lane: it wants my v[j], I want its v[q]
+    const uint32_t send = j == 0 ? v[0] : j == 1 ? v[1] : j == 2 ? v[2] : v[3];
+    const uint32_t got = t == 0 ? send : __shfl_xor_sync(0xffffffffu, send, t);
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+      if (c == j) out[c] = got;
+  }
+#pragma unroll
+  for (int c = 0; c < 4; ++c) v[c] = out[c];
+}
+
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
