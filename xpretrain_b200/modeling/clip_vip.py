@@ -91,6 +91,9 @@ class _Encoder(nn.Module):
     def __init__(self, tc: TowerConfig, eps):
         super().__init__()
         self.layers = nn.ModuleList([_EncoderLayer(tc, eps) for _ in range(tc.num_hidden_layers)])
+        # CLIPEncoder.gradient_checkpointing (CLIP_ViP.py:626,676-690): in training mode the tower keeps only each block's
+        # input and recomputes the block during the backward (_layer_fwd's `keep_input` / `upto_fc1`)
+        self.gradient_checkpointing = False
 
 
 class _VisionViPEmbeddings(nn.Module):
@@ -144,6 +147,8 @@ def _tower_param_list(tower_prefix: str, n_layers: int) -> List[str]:
 
 class CLIPModel(nn.Module):
     """Same constructor argument style, attribute names and output keys as the reference CLIPModel."""
+
+    supports_gradient_checkpointing = True      # CLIPPreTrainedModel, CLIP_ViP.py:478
 
     def __init__(self, config: ClipVipConfig):
         super().__init__()
@@ -201,6 +206,26 @@ class CLIPModel(nn.Module):
         """CLIP_ViP.py:992-1041."""
         _, text_embeds = _run(self, None, input_ids, attention_mask, normalize=bool(if_norm))
         return text_embeds
+
+    # ------------------------------------------------------------------- gradient checkpointing
+    def gradient_checkpointing_enable(self, gradient_checkpointing_kwargs=None):
+        """Set `gradient_checkpointing` on both encoders, as the reference's `_set_gradient_checkpointing` does
+        (CLIP_ViP.py:524-526).  A tower in training mode then keeps only each block's input (one [rows, C] tensor in the
+        residual stream's storage type) and reruns the block's forward kernels, through fc1, before the block's backward.
+        Results are bit-identical to a run without checkpointing.  `gradient_checkpointing_kwargs` is accepted so Hugging
+        Face call sites work and has no effect: the recompute runs inside this model's own backward, not through
+        `torch.utils.checkpoint`."""
+        for enc in (self.vision_model.encoder, self.text_model.encoder):
+            enc.gradient_checkpointing = True
+
+    def gradient_checkpointing_disable(self):
+        """Clear `gradient_checkpointing` on both encoders: every block keeps its whole forward state again."""
+        for enc in (self.vision_model.encoder, self.text_model.encoder):
+            enc.gradient_checkpointing = False
+
+    @property
+    def is_gradient_checkpointing(self) -> bool:
+        return any(getattr(m, "gradient_checkpointing", False) for m in self.modules())
 
 
 # -------------------------------------------------------------------- bf16 compute copies
@@ -278,10 +303,14 @@ def _stream_dtype(model) -> torch.dtype:
     return torch.float16 if str(name) in ("fp16", "float16", "half") else f32
 
 
-def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, rows: int, save: bool, stream_dt):
+def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, rows: int, save: bool, stream_dt,
+               keep_input: bool = False, upto_fc1: bool = False):
     """One pre-LN residual block (CLIP_ViP.py:445-460).  x: residual stream [rows, C] in `stream_dt` (fp32 / fp16), or bf16 when
     stream_dt is None (round-1 path); pend: the previous block's bf16 branch output that still has to be added to it.
-    Returns (x_out, pend_out, saved)."""
+    Returns (x_out, pend_out, saved): saved is the tuple _layer_bwd reads when `save`; otherwise, with `keep_input`, the
+    LayerNorm-1 input alone (x + pend as the fused add stored it), the checkpoint from which a plain call with `save` and
+    `upto_fc1` rebuilds that tuple bit for bit.  `upto_fc1` stops after fc1 + QuickGELU and returns (None, None, saved): the
+    backward never reads fc2's output."""
     fp32res = stream_dt is not None
     C_, I = pk.C, pk.I
     dev = x.device
@@ -317,8 +346,10 @@ def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, ro
     pre = torch.empty(rows, I, dtype=bf16, device=dev) if save else None
     f1 = torch.empty(rows, I, dtype=bf16, device=dev)
     ops.linear_fwd(h2, pk.w1[i], layer.mlp.fc1.bias, f1, act=_lib.ACT_QUICK_GELU, aux=pre, ld_aux=I)
+    saved = (x, mean1, rstd1, h, qkv, att_saved, a, x1, mean2, rstd2, h2, pre, f1) if save else (x if keep_input else None)
+    if upto_fc1:
+        return None, None, saved
     out = torch.empty(rows, C_, dtype=bf16, device=dev)
-    saved = (x, mean1, rstd1, h, qkv, att_saved, a, x1, mean2, rstd2, h2, pre, f1) if save else None
     if fp32res:
         ops.linear_fwd(f1, pk.w2[i], layer.mlp.fc2.bias, out)                           # branch; added by the next LayerNorm
         return x1, out, saved
@@ -438,7 +469,15 @@ def _finish_layer_grads(prefix: str, grads: Dict[str, torch.Tensor], C_: int):
 
 
 # ------------------------------------------------------------------------------ vision tower
-def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool):
+def _block_saved(sv, i: int):
+    """Block i's saved tensors for its backward, released from `sv`.  A checkpointed tower kept only the block's input:
+    rebuild the rest now by rerunning the block's forward kernels from it, on the stream and under the SM limit of the backward."""
+    s, sv.layers[i] = sv.layers[i], None
+    return s if sv.recompute is None else sv.recompute(i, s)
+
+
+def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = False):
+    """ckpt (with save): keep each block's input only (gradient checkpointing); the backward rebuilds the rest per block."""
     cfg = model.config
     vm = model.vision_model
     emb = vm.embeddings
@@ -497,7 +536,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool):
         if timer is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save, stream_dt)
+        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
         if timer is not None:
             e1.record()
             timer.append(("fwd", e0, e1))
@@ -510,9 +549,13 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool):
     ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
     saved = None
     if save:
+        recompute = None
+        if ckpt:
+            def recompute(i, xin):
+                return _layer_fwd(xin, None, vm.encoder.layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
         saved = SimpleNamespace(B=B, T=T, S=S, rows=rows, patches=patches, x0=x0, stats0=(mean0p, rstd0p, mean0g, rstd0g),
                                 layers=layer_saved, x_last=(x, pend), post_in=post_in, pooled=pooled, meanp=meanp, rstdp=rstdp,
-                                ws=ws)
+                                ws=ws, recompute=recompute)
     return proj, saved
 
 
@@ -545,11 +588,10 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
         if timer is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        dx = _layer_bwd(dx, sv.layers[i], vm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows, aux)
+        dx = _layer_bwd(dx, _block_saved(sv, i), vm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows, aux)
         if timer is not None:
             e1.record()
             timer.append(("bwd", e0, e1))
-        sv.layers[i] = None
         _grads_ready(model, grads, prefix)
     # pre_layrnorm backward, written as two compact halves: patch rows [B, T*L, C] and global rows [B, M, C]
     d_patch = torch.empty(B * T * L, C_, dtype=bf16, device=dev)
@@ -571,7 +613,8 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
 
 
 # -------------------------------------------------------------------------------- text tower
-def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor], save: bool):
+def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor], save: bool,
+              ckpt: bool = False):
     cfg = model.config
     tm = model.text_model
     B, Lt = input_ids.shape
@@ -601,7 +644,7 @@ def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optiona
     if stream_dt is not None:
         x = x.to(stream_dt)          # [B*Lt, 512]: the token + position embeddings enter the stream in its storage type
     for i, layer in enumerate(tm.encoder.layers):
-        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save, stream_dt)
+        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
         layer_saved.append(sv)
     # final_layer_norm is per-row, so it is applied to the pooled EOS row only (first argmax of the ids, :776)
     eos = torch.empty(B, dtype=torch.int64, device=dev)
@@ -614,8 +657,12 @@ def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optiona
     ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
     saved = None
     if save:
+        recompute = None
+        if ckpt:
+            def recompute(i, xin):
+                return _layer_fwd(xin, None, tm.encoder.layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
         saved = SimpleNamespace(B=B, Lt=Lt, rows=rows, ids=ids, layers=layer_saved, x_last=(x, pend), post_in=post_in, eos=eos,
-                                pooled=pooled, meanp=meanp, rstdp=rstdp, err=err)
+                                pooled=pooled, meanp=meanp, rstdp=rstdp, err=err, recompute=recompute)
     return proj, saved
 
 
@@ -641,8 +688,7 @@ def _text_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, t
 
     for i in reversed(range(len(tm.encoder.layers))):
         prefix = f"text_model.encoder.layers.{i}."
-        dx = _layer_bwd(dx, sv.layers[i], tm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows)
-        sv.layers[i] = None
+        dx = _layer_bwd(dx, _block_saved(sv, i), tm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows)
         _grads_ready(model, grads, prefix)
     ops.text_embed_bwd(sv.ids, dx, grads["text_model.embeddings.token_embedding.weight"],
                        grads["text_model.embeddings.position_embedding.weight"], Lt, C_, cfg.vocab_size)
@@ -664,13 +710,18 @@ class _ClipVipFunction(torch.autograd.Function):
         dev = params[0].device
 
         def run_tower(which):
+            # gradient checkpointing applies in training mode only (the reference's `self.gradient_checkpointing and
+            # self.training`), and only to a tower that saves anything for the backward at all
             if which == "vis":
                 tower_save = save and any(r for n, r in need.items() if n.startswith(("vision_model.", "visual_projection.")))
-                proj, sv = _vision_fwd(model, video, tower_save)
+                enc = model.vision_model.encoder
+                proj, sv = _vision_fwd(model, video, tower_save, tower_save and enc.gradient_checkpointing and enc.training)
             else:
                 # a frozen text tower (VidCLIP.freeze_text_encoder) keeps nothing and runs no backward
                 tower_save = save and any(r for n, r in need.items() if n.startswith(("text_model.", "text_projection.")))
-                proj, sv = _text_fwd(model, input_ids, attention_mask, tower_save)
+                enc = model.text_model.encoder
+                proj, sv = _text_fwd(model, input_ids, attention_mask, tower_save,
+                                     tower_save and enc.gradient_checkpointing and enc.training)
             if normalize:
                 feat = torch.empty_like(proj)
                 inv = torch.empty(proj.shape[0], dtype=f32, device=dev)
