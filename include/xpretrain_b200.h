@@ -119,13 +119,15 @@ int xp_cast_f32_bf16(const float* src, void* dst_bf16, int64_t n, void* stream);
 enum { XP_DTYPE_F32 = 0, XP_DTYPE_BF16 = 1, XP_DTYPE_F16 = 2 };
 
 /* im2col of nn.Conv2d(3, width, kernel=stride=patch, bias=False) (CLIP_ViP.py:157-159,178-179):
- * video [frames,3,H,W] -> patches bf16 [frames*(H/p)*(W/p), 3*p*p]; the conv itself then runs as xp_gemm. */
+ * video [frames,3,H,W] -> patches bf16 [frames*(H/p)*(W/p), ld]; the conv itself then runs as xp_gemm with K = 3*p*p.
+ * Row pitch ld = round_up(3*p*p, 8) elements (16-byte rows, as TMA and xp_gemm need); columns [3*p*p, ld) are written
+ * as zero.  ld = 3*p*p for p = 16 and 32; p = 14 (ViT-L/14) gives 588 columns in a pitch of 592.  Any p dividing H and W. */
 int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_t frames, int32_t H, int32_t W,
                     int32_t patch, void* stream);
 /* The reference's input transform fused into the patch extraction (SURVEY.md §8f.4): frames_hwc uint8 [frames, H, W, 3] as
  * the decoder delivers them -> `.permute(0,3,1,2).float() / 255.` (CLIP-ViP/src/datasets/dataset_pretrain_stage1_all_source.py:182)
  * -> Normalize(mean, std) (init_transform_dict_simple, CLIP-ViP/src/datasets/dataloader.py:209-233; Resize / CenterCrop are
- * the identity at the input resolution) -> the bf16 patch matrix of xp_vip_patchify.  IEEE fp32 arithmetic, one rounding to
+ * the identity at the input resolution) -> the bf16 patch matrix of xp_vip_patchify (same pitch).  IEEE fp32 arithmetic, one rounding to
  * bf16: bit-identical to casting the reference's fp32 tensor.  mean3 / std3 are HOST arrays of 3 floats. */
 int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W, int32_t patch,
                        const float* mean3, const float* std3, void* stream);
@@ -155,7 +157,9 @@ int xp_eos_offsets(const int64_t* ids, int64_t* offsets, int32_t* index, int32_t
  *   qkv  bf16 [B*S, 3C]  columns [q | k | v], head h at [h*64, h*64+64), q already scaled by 64**-0.5
  *   out  bf16 [B*S, C]   (the tensor out_proj consumes; rows ordered [M global, frame0 L, frame1 L, ...])
  *   lse  f32  [B, H, S]  log-sum-exp of every query row (saved for backward)
- * S = M + T*L, head_dim 64, M + L <= 208.  workspace: xp_vip_attention_workspace_bytes() bytes. */
+ * S = M + T*L, head_dim 64, 1 <= M <= 8, any L >= 1: M + L <= 208 stages a whole frame per CTA, longer frames (ViT-L/14:
+ * L = 256 at 224 px, 576 at 336 px) stream 64-row blocks.  workspace: xp_vip_attention_workspace_bytes() bytes for both.
+ * No float atomics: out, lse and dqkv are bit-identical across calls. */
 int64_t xp_vip_attention_workspace_bytes(int32_t B, int32_t H, int32_t T, int32_t M);
 int xp_vip_attention_fwd(const void* qkv, void* out, float* lse, float* workspace, int32_t B, int32_t H, int32_t T,
                          int32_t L, int32_t M, int32_t C, void* stream);

@@ -120,6 +120,49 @@ patchify_u8_kernel(const uint8_t* __restrict__ frames, __nv_bfloat16* __restrict
   }
 }
 
+// Any patch size dividing H and W (ViT-L/14: p = 14).  The patch matrix row pitch is ld = round_up(3 p^2, 8) (16-byte rows
+// for TMA and the GEMM); columns [3 p^2, ld) are written as zero.  One thread per 8 consecutive columns of a patch row: a
+// gather of 8 input values (the same conversion and rounding as the vectorised kernels above) and one 16-byte store.
+template <typename T>
+__device__ __forceinline__ float to_f32(T v) { return static_cast<float>(v); }
+template <>
+__device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <>
+__device__ __forceinline__ float to_f32<__half>(__half v) { return __half2float(v); }
+
+template <typename T, bool U8>
+__global__ void __launch_bounds__(256)
+patchify_any_kernel(const T* __restrict__ src, __nv_bfloat16* __restrict__ out, long long frames, int H, int W, int p,
+                    float m0, float m1, float m2, float s0, float s1, float s2) {
+  const int kp = 3 * p * p, ld = (kp + 7) & ~7, cchunks = ld / 8;
+  const int gw = W / p, gh = H / p;
+  const long long total = frames * gh * gw * cchunks;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int cc = static_cast<int>(idx % cchunks);
+  const long long row = idx / cchunks;
+  const int pw = static_cast<int>(row % gw), ph = static_cast<int>((row / gw) % gh);
+  const long long f = row / (static_cast<long long>(gw) * gh);
+  const float mean[3] = {m0, m1, m2}, sd[3] = {s0, s1, s2};
+  float v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int col = cc * 8 + i;
+    v[i] = 0.f;
+    if (col < kp) {
+      const int c = col / (p * p), kh = (col / p) % p, kw = col % p;
+      const int y = ph * p + kh, x = pw * p + kw;
+      if (U8) {
+        const float u = static_cast<float>(reinterpret_cast<const uint8_t*>(src)[((f * H + y) * W + x) * 3 + c]);
+        v[i] = __fdiv_rn(__fsub_rn(__fdiv_rn(u, 255.f), mean[c]), sd[c]);
+      } else {
+        v[i] = to_f32<T>(src[((f * 3 + c) * H + y) * W + x]);
+      }
+    }
+  }
+  *reinterpret_cast<uint4*>(out + row * ld + cc * 8) = pack8f(v);
+}
+
 // ------------------------------------------------------------ embedding tables
 // table[t*L + l, :] = interp(temporal)[t, :] + pos[1 + l, :]      (bf16; the patch GEMM adds it as a periodic residual)
 // x[b, m, :]       = (m == 0 ? class_embedding : added_cls[m-1]) + pos[0, :]   for m < M
@@ -269,12 +312,30 @@ using namespace xp;
 extern "C" int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_t frames, int32_t H,
                                int32_t W, int32_t patch, void* stream) {
   XP_ENTER(video);
-  if (patch % 8 || W % patch || H % patch) return fail("xp_vip_patchify: patch must be a multiple of 8 dividing H and W");
+  if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify: patch must divide H and W");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  __nv_bfloat16* out = static_cast<__nv_bfloat16*>(patches_bf16);
+  if (patch % 8) {
+    const long long total = frames * (H / patch) * (W / patch) * (((3 * patch * patch + 7) & ~7) / 8);
+    if (total <= 0) return 0;
+    const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+    if (dtype == XP_DTYPE_F32)
+      patchify_any_kernel<float, false><<<grid, 256, 0, st>>>(static_cast<const float*>(video), out, frames, H, W, patch,
+                                                              0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
+    else if (dtype == XP_DTYPE_BF16)
+      patchify_any_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(video), out, frames,
+                                                                      H, W, patch, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
+    else if (dtype == XP_DTYPE_F16)
+      patchify_any_kernel<__half, false><<<grid, 256, 0, st>>>(static_cast<const __half*>(video), out, frames, H, W, patch,
+                                                               0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
+    else
+      return fail("xp_vip_patchify: dtype must be XP_DTYPE_F32 / BF16 / F16");
+    XP_CHECK_LAUNCH("patchify_any_kernel");
+    return 0;
+  }
   const long long total = frames * 3 * H * (W / 8);
   if (total <= 0) return 0;
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  __nv_bfloat16* out = static_cast<__nv_bfloat16*>(patches_bf16);
   if (dtype == XP_DTYPE_F32)
     patchify_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(video), out, frames, H, W, patch);
   else if (dtype == XP_DTYPE_BF16)
@@ -290,7 +351,16 @@ extern "C" int xp_vip_patchify(const void* video, int32_t dtype, void* patches_b
 extern "C" int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W,
                                   int32_t patch, const float* mean3, const float* std3, void* stream) {
   XP_ENTER(frames_hwc);
-  if (patch % 8 || W % patch || H % patch) return fail("xp_vip_patchify_u8: patch must be a multiple of 8 dividing H and W");
+  if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify_u8: patch must divide H and W");
+  if (patch % 8) {
+    const long long total = frames * (H / patch) * (W / patch) * (((3 * patch * patch + 7) & ~7) / 8);
+    if (total <= 0) return 0;
+    patchify_any_kernel<uint8_t, true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        frames_hwc, static_cast<__nv_bfloat16*>(patches_bf16), frames, H, W, patch, mean3[0], mean3[1], mean3[2], std3[0],
+        std3[1], std3[2]);
+    XP_CHECK_LAUNCH("patchify_any_kernel");
+    return 0;
+  }
   if ((reinterpret_cast<uintptr_t>(frames_hwc) & 7) != 0) return fail("xp_vip_patchify_u8: frames must be 8-byte aligned");
   const long long total = frames * H * (W / 8);
   if (total <= 0) return 0;

@@ -1,4 +1,5 @@
-// Video-proxy (ViP) attention of CLIP-ViP, forward and backward, one CTA per (batch, head, frame).
+// Video-proxy (ViP) attention of CLIP-ViP, forward and backward, one CTA per (batch, head, frame), for frames of
+// M + L <= 208 rows (ViT-B/16 and B/32); longer frames run the streamed kernels of vip_attention_long.cu.
 //
 // Reference: CLIPAttention.forward2, CLIP_ViP.py:332-381.  Patch queries of frame t attend to
 // [M global keys ; L keys of frame t] (:352-363); the M global queries (cls + video proxies) attend to
@@ -20,6 +21,7 @@
 #include "common.h"
 #include "ptx.cuh"
 #include "mma_frag.cuh"
+#include "vip_attention.h"
 
 namespace xp {
 
@@ -29,17 +31,6 @@ constexpr int MAT_BYTES = SROWS * 128;     // one [256][64] bf16 matrix, 128B-sw
 constexpr int TILE_BYTES = 64 * 128;       // 64 rows
 constexpr int ATT_THREADS = 256;           // two warpgroups
 
-struct AttnDims {
-  int B, H, T, L, M;
-  long long S;       // M + T*L
-  long long ld_qkv;  // 3*C
-  long long ld_o;    // C
-  int C;
-};
-
-__device__ __forceinline__ long long token_row(const AttnDims& d, int b, int t, int i) {
-  return static_cast<long long>(b) * d.S + (i < d.M ? i : d.M + static_cast<long long>(t) * d.L + (i - d.M));
-}
 // shared-memory row r: a frame token (r < L), a global token (GROW <= r < GROW + M) or zero padding
 __device__ __forceinline__ bool row_valid(int r, const AttnDims& d) { return r < d.L || (r >= GROW && r < GROW + d.M); }
 __device__ __forceinline__ bool row_global(int r) { return r >= GROW; }
@@ -451,7 +442,7 @@ vip_attn_bwd_combine_kernel(const float* __restrict__ gpart, __nv_bfloat16* __re
 
 static int make_dims(AttnDims& d, int B, int H, int T, int L, int M, int C) {
   if (C != H * HD) return fail("vip_attention: head_dim must be 64 (C == 64*H)");
-  if (M + L > 208) return fail("vip_attention: M + L must be <= 208");
+  if (L < 1) return fail("vip_attention: L must be >= 1");
   if (M < 1 || M > 8) return fail("vip_attention: 1 <= M <= 8 global tokens");
   d.B = B; d.H = H; d.T = T; d.L = L; d.M = M;
   d.S = static_cast<long long>(M) + static_cast<long long>(T) * L;
@@ -485,16 +476,20 @@ extern "C" int xp_vip_attention_fwd(const void* qkv, void* out, float* lse, floa
   XP_ENTER(qkv);
   AttnDims d;
   if (make_dims(d, B, H, T, L, M, C)) return -1;
-  CUtensorMap mL, mM;
-  if (make_row_maps(&mL, &mM, qkv, 3LL * C, d)) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-    attr = true;
-  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  vip_attn_fwd_kernel<<<dim3(T, H, B), ATT_THREADS, FWD_SMEM, st>>>(mL, mM, static_cast<__nv_bfloat16*>(out), lse, workspace, d);
-  XP_CHECK_LAUNCH("vip_attn_fwd_kernel");
+  if (M + L > VIP_STAGED_MAX_ROWS) {   // frames too long to stage whole: the streamed kernel (vip_attention_long.cu)
+    if (vip_long_attn_fwd(d, qkv, out, lse, workspace, st)) return -1;
+  } else {
+    CUtensorMap mL, mM;
+    if (make_row_maps(&mL, &mM, qkv, 3LL * C, d)) return -1;
+    static bool attr = false;
+    if (!attr) {
+      XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
+      attr = true;
+    }
+    vip_attn_fwd_kernel<<<dim3(T, H, B), ATT_THREADS, FWD_SMEM, st>>>(mL, mM, static_cast<__nv_bfloat16*>(out), lse, workspace, d);
+    XP_CHECK_LAUNCH("vip_attn_fwd_kernel");
+  }
   vip_attn_fwd_combine_kernel<<<dim3(H, B), 64, 0, st>>>(workspace, static_cast<__nv_bfloat16*>(out), lse, d);
   XP_CHECK_LAUNCH("vip_attn_fwd_combine_kernel");
   return 0;
@@ -506,18 +501,22 @@ extern "C" int xp_vip_attention_bwd(const void* qkv, const void* out, const void
   XP_ENTER(qkv);
   AttnDims d;
   if (make_dims(d, B, H, T, L, M, C)) return -1;
-  CUtensorMap mL, mM, gL, gM;
-  if (make_row_maps(&mL, &mM, qkv, 3LL * C, d) || make_row_maps(&gL, &gM, dout, C, d)) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    attr = true;
-  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  vip_attn_bwd_kernel<<<dim3(T, H, B), ATT_THREADS, BWD_SMEM, st>>>(
-      mL, mM, gL, gM, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse,
-      static_cast<__nv_bfloat16*>(dqkv), workspace, d, q_scale);
-  XP_CHECK_LAUNCH("vip_attn_bwd_kernel");
+  if (M + L > VIP_STAGED_MAX_ROWS) {
+    if (vip_long_attn_bwd(d, qkv, out, dout, lse, dqkv, workspace, q_scale, st)) return -1;
+  } else {
+    CUtensorMap mL, mM, gL, gM;
+    if (make_row_maps(&mL, &mM, qkv, 3LL * C, d) || make_row_maps(&gL, &gM, dout, C, d)) return -1;
+    static bool attr = false;
+    if (!attr) {
+      XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
+      attr = true;
+    }
+    vip_attn_bwd_kernel<<<dim3(T, H, B), ATT_THREADS, BWD_SMEM, st>>>(
+        mL, mM, gL, gM, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse,
+        static_cast<__nv_bfloat16*>(dqkv), workspace, d, q_scale);
+    XP_CHECK_LAUNCH("vip_attn_bwd_kernel");
+  }
   vip_attn_bwd_combine_kernel<<<dim3(H, B), 192, 0, st>>>(workspace, static_cast<__nv_bfloat16*>(dqkv), d, q_scale);
   XP_CHECK_LAUNCH("vip_attn_bwd_combine_kernel");
   return 0;

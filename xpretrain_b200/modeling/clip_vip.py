@@ -492,8 +492,9 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     pk = _pack(model, "vision")
     eps = cfg.layer_norm_eps
     Kp = 3 * cfg.patch_size * cfg.patch_size
+    ldp = ops.patch_pitch(cfg.patch_size)    # patch-matrix row pitch: Kp rounded up to 8 columns, pad columns zero
 
-    patches = torch.empty(B * T * L, Kp, dtype=bf16, device=dev)
+    patches = torch.empty(B * T * L, ldp, dtype=bf16, device=dev)
     if video.dtype == torch.uint8:      # raw decoder frames: the reference's /255 + Normalize is fused into the patch extraction
         ops.vip_patchify_u8(video.contiguous(), patches, cfg.patch_size, getattr(model, "pixel_mean", ops.CLIP_MEAN),
                             getattr(model, "pixel_std", ops.CLIP_STD))
@@ -505,8 +506,14 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     ops.vip_embed_tables(emb.position_embedding.weight, temporal, emb.class_embedding, emb.added_cls, table, x0, B, T, L,
                          M, C_, cfg.temporal_size)
     wp = _small_bf16(model, "patch", emb.patch_embedding.weight).view(C_, Kp)
+    if ldp != Kp:   # e.g. p = 14: the GEMM's B operand needs the same 16-byte row pitch as the patch matrix
+        wpad = model._packs.get("pad:patch")
+        if wpad is None or wpad.shape != (C_, ldp) or wpad.device != dev:
+            wpad = model._packs["pad:patch"] = torch.zeros(C_, ldp, dtype=bf16, device=dev)
+        wpad[:, :Kp].copy_(wp)
+        wp = wpad
     # conv-as-GEMM; epilogue adds the periodic [T*L, C] position+temporal table and writes past the M global rows
-    ops.gemm(patches, wp, x0, M=B * T * L, N=C_, K=Kp, lda=Kp, ldb=Kp, ldc=C_, residual=table, ldr=C_, r_group=T * L,
+    ops.gemm(patches, wp, x0, M=B * T * L, N=C_, K=Kp, lda=ldp, ldb=ldp, ldc=C_, residual=table, ldr=C_, r_group=T * L,
              r_group_stride=0, c_group=T * L, c_group_stride=S * C_, c_offset=M * C_)
     plain = ops.rowmap(C_)
     # pre_layrnorm (CLIP_ViP.py:881) in two launches so that its statistics are stored compactly per half
@@ -609,7 +616,12 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
                       grads.get(emb + "temporal_embedding"), grads[emb + "class_embedding"], grads[emb + "added_cls"],
                       B, T, L, M, C_, cfg.temporal_size)
     Kp = 3 * cfg.patch_size * cfg.patch_size
-    ops.linear_wgrad(d_patch, sv.patches, grads[emb + "patch_embedding.weight"].view(C_, Kp))
+    if sv.patches.shape[1] == Kp:
+        ops.linear_wgrad(d_patch, sv.patches, grads[emb + "patch_embedding.weight"].view(C_, Kp))
+    else:           # padded pitch (xp_gemm needs N % 8 == 0): the GEMM fills [C, pitch], the Kp real columns are the gradient
+        dw = torch.zeros(C_, sv.patches.shape[1], dtype=f32, device=dev)
+        ops.linear_wgrad(d_patch, sv.patches, dw)
+        grads[emb + "patch_embedding.weight"].view(C_, Kp).add_(dw[:, :Kp])
 
 
 # -------------------------------------------------------------------------------- text tower

@@ -22,8 +22,9 @@ def _get(obj, key, default=None):
 
 def config_from_args(args) -> ClipVipConfig:
     """Build the model config the way VidCLIP.__init__ does (VidCLIP.py:11-13): the CLIP hyper-parameters come from
-    `args.clip_config` (a local HF-style config.json / directory if it exists, else the ViT-B/16 defaults that
-    "openai/clip-vit-base-patch16" names — there is no network) and the ViP additions from
+    `args.clip_config` (a local HF-style config.json / directory if it exists, else the built-in hyper-parameters of the
+    name: "openai/clip-vit-large-patch14" / "-patch14-336" (ViT-L/14 at 224 / 336 px), "...patch32" (ViT-B/32), and
+    otherwise the ViT-B/16 defaults of "openai/clip-vit-base-patch16" — there is no network) and the ViP additions from
     `args.clip_vision_additional_config`."""
     src = _get(args, "clip_config")
     cfg = copy.deepcopy(src) if isinstance(src, ClipVipConfig) else ClipVipConfig()
@@ -43,6 +44,13 @@ def config_from_args(args) -> ClipVipConfig:
         cfg.projection_dim = hf.get("projection_dim", 512)
         cfg.vocab_size = t.get("vocab_size", 49408)
         cfg.max_position_embeddings = t.get("max_position_embeddings", 77)
+    elif isinstance(src, str) and "clip-vit-large-patch14" in src:
+        # openai/clip-vit-large-patch14 and openai/clip-vit-large-patch14-336 (their Hugging Face config.json)
+        cfg.vision = TowerConfig(1024, 16, 24, 4096)
+        cfg.text = TowerConfig(768, 12, 12, 3072)
+        cfg.patch_size = 14
+        cfg.image_size = 336 if src.rstrip("/").endswith("-336") else 224
+        cfg.projection_dim = 768
     elif isinstance(src, str) and "patch32" in src:
         cfg.patch_size = 32
     add = _get(args, "clip_vision_additional_config")

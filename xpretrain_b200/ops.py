@@ -183,6 +183,12 @@ def cast_bf16(src: torch.Tensor, dst: torch.Tensor, dst_offset: int = 0):
 _DT = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_F16}
 
 
+def patch_pitch(patch: int) -> int:
+    """Row pitch (elements) of the bf16 patch matrix: 3*p*p rounded up to a multiple of 8, so that rows are 16-byte aligned
+    for TMA; the pad columns are zero.  Equal to 3*p*p for p = 16 and 32; 592 for p = 14."""
+    return (3 * patch * patch + 7) // 8 * 8
+
+
 def vip_patchify(video: torch.Tensor, patches: torch.Tensor, patch: int):
     frames = video.numel() // (3 * video.shape[-2] * video.shape[-1])
     check(lib().xp_vip_patchify(_p(video), _DT[video.dtype], _p(patches), frames, video.shape[-2], video.shape[-1], patch,
