@@ -110,6 +110,15 @@ int xp_layernorm_bwd(const void* dy, const XpRowMap* dymap, const void* x, const
 int xp_l2norm_fwd(const float* x, float* y, float* inv_norm, int32_t rows, int32_t C, void* stream);
 int xp_l2norm_bwd(const float* dy, const float* y, const float* inv_norm, void* dx_bf16, int32_t rows, int32_t C,
                   float scale, void* stream);
+/* Frame-mean head of the per-frame CLIP model (VidCLIP.py:62-65), fp32: for each of B videos with T frame projections
+ * proj [B*T, P], u_t = p_t/||p_t||, m = mean_t u_t, feat [B, P] = m/||m||; inv_frame [B*T] = 1/||p_t|| and
+ * inv_video [B] = 1/||m|| are saved for the backward.  The backward writes dproj [B*T, P] bf16 = scale * d(feat)/d(proj)^T
+ * dfeat, exact through both normalisations.  One CTA per video, no atomics: repeated calls are bitwise equal.
+ * T + P <= 12288. */
+int xp_frame_pool_fwd(const float* proj, float* feat, float* inv_frame, float* inv_video, int32_t B, int32_t T, int32_t P,
+                      void* stream);
+int xp_frame_pool_bwd(const float* dfeat, const float* feat, const float* proj, const float* inv_frame,
+                      const float* inv_video, void* dproj_bf16, int32_t B, int32_t T, int32_t P, float scale, void* stream);
 /* out[c] += scale * sum_r x[r,c]: bias gradients of every nn.Linear. */
 int xp_colsum_bf16(const void* x, int64_t ld, float* out, int64_t rows, int32_t C, float scale, void* stream);
 /* fp32 master parameter -> bf16 compute copy. */

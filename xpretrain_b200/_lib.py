@@ -76,6 +76,9 @@ SIGNATURES = {
                                  P(XpRowMap), c_void_p, P(XpRowMap), c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p]),
     "xp_l2norm_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "xp_l2norm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
+    "xp_frame_pool_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "xp_frame_pool_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                  c_float, c_void_p]),
     "xp_colsum_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_int, c_float, c_void_p]),
     "xp_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_void_p]),
     "xp_vip_patchify": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_void_p]),

@@ -321,6 +321,87 @@ l2norm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, con
   }
 }
 
+// ------------------------------------------------------------------------ frame-mean head
+// The per-frame CLIP model's video feature (VidCLIP.py:62-65), per video b over its T frame projections p_t [P]:
+//   u_t = p_t / ||p_t||,  m = mean_t u_t,  f = m / ||m||          (fp32)
+// One CTA per video.  Every reduction runs in a fixed order and nothing is accumulated atomically, so two calls give
+// bitwise-equal results.  A zero-norm row gives inf / NaN, as the reference's division does.
+constexpr int FP_THREADS = 256, FP_WARPS = FP_THREADS / 32;
+
+// Sum of v over the CTA, the same value in every thread; warp partials are added in warp order.
+__device__ __forceinline__ float frame_pool_block_sum(float v, float* red) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < FP_WARPS; ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
+__global__ void __launch_bounds__(FP_THREADS)
+frame_pool_fwd_kernel(const float* __restrict__ proj, float* __restrict__ feat, float* __restrict__ inv_frame,
+                      float* __restrict__ inv_video, int T, int P) {
+  extern __shared__ float fp_smem[];      // inverse frame norms [T] | frame mean [P]
+  __shared__ float red[FP_WARPS];
+  float* s_inv = fp_smem;
+  float* s_m = fp_smem + T;
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* pb = proj + static_cast<long long>(b) * T * P;
+  for (int t = warp; t < T; t += FP_WARPS) {          // one warp per frame
+    const float* p = pb + static_cast<long long>(t) * P;
+    float s = 0.f;
+    for (int c = lane; c < P; c += 32) s += p[c] * p[c];
+    const float inv = 1.f / sqrtf(warp_sum(s));
+    if (lane == 0) {
+      s_inv[t] = inv;
+      inv_frame[static_cast<long long>(b) * T + t] = inv;
+    }
+  }
+  __syncthreads();
+  float ss = 0.f;
+  for (int c = threadIdx.x; c < P; c += FP_THREADS) {
+    float acc = 0.f;
+    for (int t = 0; t < T; ++t) acc += pb[static_cast<long long>(t) * P + c] * s_inv[t];
+    const float m = acc / static_cast<float>(T);
+    s_m[c] = m;                                        // read back below by the same thread
+    ss += m * m;
+  }
+  const float inv2 = 1.f / sqrtf(frame_pool_block_sum(ss, red));
+  for (int c = threadIdx.x; c < P; c += FP_THREADS) feat[static_cast<long long>(b) * P + c] = s_m[c] * inv2;
+  if (threadIdx.x == 0) inv_video[b] = inv2;
+}
+
+// Exact backward through both normalisations, times `scale`, written as bf16 (it feeds the projection GEMMs):
+//   du = (df - f (f . df)) / (||m|| T)   (the same for every frame),   dp_t = (du - u_t (u_t . du)) / ||p_t||
+// u_t is rebuilt as p_t * inv_frame[t], the product the forward formed.
+__global__ void __launch_bounds__(FP_THREADS)
+frame_pool_bwd_kernel(const float* __restrict__ dfeat, const float* __restrict__ feat, const float* __restrict__ proj,
+                      const float* __restrict__ inv_frame, const float* __restrict__ inv_video,
+                      __nv_bfloat16* __restrict__ dproj, int T, int P, float scale) {
+  extern __shared__ float fp_smem[];      // du [P]
+  __shared__ float red[FP_WARPS];
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* df = dfeat + static_cast<long long>(b) * P;
+  const float* f = feat + static_cast<long long>(b) * P;
+  float s = 0.f;
+  for (int c = threadIdx.x; c < P; c += FP_THREADS) s += df[c] * f[c];
+  const float dot = frame_pool_block_sum(s, red);
+  const float k = inv_video[b] * scale / static_cast<float>(T);
+  for (int c = threadIdx.x; c < P; c += FP_THREADS) fp_smem[c] = (df[c] - f[c] * dot) * k;
+  __syncthreads();
+  for (int t = warp; t < T; t += FP_WARPS) {          // one warp per frame
+    const long long r = static_cast<long long>(b) * T + t;
+    const float* p = proj + r * P;
+    const float inv = inv_frame[r];
+    float d = 0.f;
+    for (int c = lane; c < P; c += 32) d += p[c] * inv * fp_smem[c];
+    d = warp_sum(d);
+    for (int c = lane; c < P; c += 32) dproj[r * P + c] = __float2bfloat16((fp_smem[c] - p[c] * inv * d) * inv);
+  }
+}
+
 // ------------------------------------------------------------------------- column sums
 // out[c] += sum_r x[r, c]   (bias gradients).  grid.x covers column chunks of 256, grid.y splits rows.
 __global__ void __launch_bounds__(256)
@@ -707,6 +788,37 @@ extern "C" int xp_l2norm_bwd(const float* dy, const float* y, const float* inv_n
   l2norm_bwd_kernel<<<(rows + 3) / 4, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       dy, y, inv_norm, static_cast<__nv_bfloat16*>(dx_bf16), rows, C, scale);
   XP_CHECK_LAUNCH("l2norm_bwd_kernel");
+  return 0;
+}
+
+static int frame_pool_check(const char* what, int32_t B, int32_t T, int32_t P, size_t smem) {
+  if (B < 0 || T < 1 || P < 1) return fail(std::string(what) + ": need B >= 0, T >= 1 and P >= 1");
+  if (B > 0x7fffffff / T) return fail(std::string(what) + ": B*T must fit in int32");
+  if (smem > 48 * 1024) return fail(std::string(what) + ": T + P must be at most 12288");
+  return 0;
+}
+
+extern "C" int xp_frame_pool_fwd(const float* proj, float* feat, float* inv_frame, float* inv_video, int32_t B, int32_t T,
+                                 int32_t P, void* stream) {
+  XP_ENTER(proj);
+  const size_t smem = (static_cast<size_t>(T) + P) * sizeof(float);
+  if (frame_pool_check("xp_frame_pool_fwd", B, T, P, smem)) return -1;
+  if (B == 0) return 0;
+  frame_pool_fwd_kernel<<<B, FP_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(proj, feat, inv_frame, inv_video, T, P);
+  XP_CHECK_LAUNCH("frame_pool_fwd_kernel");
+  return 0;
+}
+
+extern "C" int xp_frame_pool_bwd(const float* dfeat, const float* feat, const float* proj, const float* inv_frame,
+                                 const float* inv_video, void* dproj_bf16, int32_t B, int32_t T, int32_t P, float scale,
+                                 void* stream) {
+  XP_ENTER(dfeat);
+  const size_t smem = static_cast<size_t>(P) * sizeof(float);
+  if (frame_pool_check("xp_frame_pool_bwd", B, T, P, smem)) return -1;
+  if (B == 0) return 0;
+  frame_pool_bwd_kernel<<<B, FP_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      dfeat, feat, proj, inv_frame, inv_video, static_cast<__nv_bfloat16*>(dproj_bf16), T, P, scale);
+  XP_CHECK_LAUNCH("frame_pool_bwd_kernel");
   return 0;
 }
 

@@ -8,6 +8,10 @@ work unchanged.  None of these nn.Modules' own forward() is ever called: forward
 `torch.autograd.Function` that drives the hand-written sm_90a kernels through the C ABI (xpretrain_b200.ops).
 There is no eager / CPU fallback.
 
+With `config.vision_type` other than "ViP" the same class is the per-frame CLIP model VidCLIP builds from CLIP-ViP/src/modeling/
+CLIP.py (VidCLIP.py:14-23,54-65): plain CLIPVisionEmbeddings, every frame a sequence of its own, and the frame-mean head
+(xp_frame_pool_fwd / _bwd) in place of the single L2 normalisation of the video feature.
+
 Reference call stack replaced (SURVEY.md §3.2):
   CLIPModel.forward            CLIP_ViP.py:1089-1172
   CLIPVisionTransformer.forward :861-903, CLIPVisionViPEmbeddings.forward :168-197
@@ -55,10 +59,22 @@ class ClipVipConfig:
     if_use_temporal_embed: int = 1
     add_cls_num: int = 3
     logit_scale_init_value: float = 4.60
+    # `vision_additional_config.type` (VidCLIP.py:14-23): "ViP" is the video-proxy tower; any other value builds the
+    # per-frame CLIP model of CLIP.py, whose video feature is the mean of its frames' normalised features
+    vision_type: str = "ViP"
 
     @property
     def num_patches(self) -> int:
         return (self.image_size // self.patch_size) ** 2
+
+    @property
+    def per_frame(self) -> bool:
+        return self.vision_type != "ViP"
+
+    @property
+    def num_global_tokens(self) -> int:
+        """Rows in front of each sequence's patch rows: CLS + the proxy tokens (ViP), or the CLS row alone (per frame)."""
+        return 1 if self.per_frame else 1 + self.add_cls_num
 
 
 # ----------------------------------------------------------------------- parameter containers
@@ -109,10 +125,23 @@ class _VisionViPEmbeddings(nn.Module):
             self.temporal_embedding = nn.Parameter(torch.zeros(1, cfg.temporal_size, w))
 
 
+class _VisionEmbeddings(nn.Module):
+    """CLIPVisionEmbeddings of the per-frame model (CLIP.py:113-140): a CLS row and the patch rows of one frame, plus
+    position_embedding[0..L]; no proxy tokens and no temporal table."""
+
+    def __init__(self, cfg: ClipVipConfig):
+        super().__init__()
+        w = cfg.vision.hidden_size
+        self.class_embedding = nn.Parameter(torch.randn(w))
+        self.patch_embedding = nn.Conv2d(3, w, kernel_size=cfg.patch_size, stride=cfg.patch_size, bias=False)
+        self.position_embedding = nn.Embedding(cfg.num_patches + 1, w)
+        self.register_buffer("position_ids", torch.arange(cfg.num_patches + 1).expand((1, -1)))
+
+
 class _VisionTransformer(nn.Module):
     def __init__(self, cfg: ClipVipConfig):
         super().__init__()
-        self.embeddings = _VisionViPEmbeddings(cfg)
+        self.embeddings = _VisionEmbeddings(cfg) if cfg.per_frame else _VisionViPEmbeddings(cfg)
         self.pre_layrnorm = nn.LayerNorm(cfg.vision.hidden_size, eps=cfg.layer_norm_eps)  # sic (reference spelling)
         self.encoder = _Encoder(cfg.vision, cfg.layer_norm_eps)
         self.post_layernorm = nn.LayerNorm(cfg.vision.hidden_size, eps=cfg.layer_norm_eps)
@@ -193,17 +222,24 @@ class CLIPModel(nn.Module):
 
     # ------------------------------------------------------------------------------ public API
     def forward(self, input_ids=None, pixel_values=None, attention_mask=None, return_loss=False, **_unused):
-        """CLIPModel.forward, CLIP_ViP.py:1089-1172 (return_loss is accepted and ignored, as VidCLIP passes False)."""
+        """CLIPModel.forward, CLIP_ViP.py:1089-1172 (return_loss is accepted and ignored, as VidCLIP passes False).
+        Per-frame model: images [N, 3, H, W] give CLIP.py's per-image features; video [B, T, 3, H, W] gives the feature
+        VidCLIP.py:54-65 forms from them, normalise(mean_t normalise(projection of frame t))."""
         image_embeds, text_embeds = _run(self, pixel_values, input_ids, attention_mask)
         return {"image_embeds": image_embeds, "text_embeds": text_embeds}
 
     def get_image_features(self, pixel_values=None, if_norm=None, **_unused):
-        """CLIP_ViP.py:1043-1085: projected (and, if if_norm, L2-normalised) video features."""
+        """CLIP_ViP.py:1043-1085: projected (and, if if_norm, L2-normalised) video features.  Per-frame model: CLIP.py:943-985,
+        the unnormalised projection of every image (or frame); like CLIP.py it takes no `if_norm`."""
+        if self.config.per_frame and if_norm is not None:
+            raise TypeError("get_image_features() got an unexpected keyword argument 'if_norm'")
         image_embeds, _ = _run(self, pixel_values, None, None, normalize=bool(if_norm))
         return image_embeds
 
     def get_text_features(self, input_ids=None, attention_mask=None, if_norm=None, **_unused):
-        """CLIP_ViP.py:992-1041."""
+        """CLIP_ViP.py:992-1041.  Per-frame model: CLIP.py:900-941, which takes no `if_norm`."""
+        if self.config.per_frame and if_norm is not None:
+            raise TypeError("get_text_features() got an unexpected keyword argument 'if_norm'")
         _, text_embeds = _run(self, None, input_ids, attention_mask, normalize=bool(if_norm))
         return text_embeds
 
@@ -477,14 +513,21 @@ def _block_saved(sv, i: int):
 
 
 def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = False):
-    """ckpt (with save): keep each block's input only (gradient checkpointing); the backward rebuilds the rest per block."""
+    """ckpt (with save): keep each block's input only (gradient checkpointing); the backward rebuilds the rest per block.
+    The per-frame model folds the frames into the batch (CLIP.py sees [B*T, 3, H, W]): B*T sequences of one frame and one
+    global (CLS) row each, where the proxy-token attention is exactly dense attention over 1 + L rows."""
     cfg = model.config
     vm = model.vision_model
     emb = vm.embeddings
-    B, T = video.shape[0], video.shape[1]
-    if video.dtype == torch.uint8 and (video.dim() != 5 or video.shape[-1] != 3):
+    if cfg.per_frame:
+        if video.dim() not in (4, 5):
+            raise ValueError("the per-frame model takes images [N, 3, H, W] or video [B, T, 3, H, W] (uint8: channels-last)")
+        B, T = video.numel() // (video.shape[-3] * video.shape[-2] * video.shape[-1]), 1
+    else:
+        B, T = video.shape[0], video.shape[1]
+    if video.dtype == torch.uint8 and ((video.dim() != 5 and not cfg.per_frame) or video.shape[-1] != 3):
         raise ValueError("uint8 video must be channels-last [B, T, H, W, 3] (decoder layout)")
-    C_, L, M = cfg.vision.hidden_size, cfg.num_patches, 1 + cfg.add_cls_num
+    C_, L, M = cfg.vision.hidden_size, cfg.num_patches, cfg.num_global_tokens
     H = cfg.vision.num_attention_heads
     S = M + T * L
     rows = B * S
@@ -502,8 +545,9 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
         ops.vip_patchify(video.contiguous(), patches, cfg.patch_size)
     table = torch.empty(T * L, C_, dtype=bf16, device=dev)
     x0 = torch.empty(rows, C_, dtype=bf16, device=dev)
-    temporal = emb.temporal_embedding if cfg.if_use_temporal_embed else None
-    ops.vip_embed_tables(emb.position_embedding.weight, temporal, emb.class_embedding, emb.added_cls, table, x0, B, T, L,
+    temporal = emb.temporal_embedding if cfg.if_use_temporal_embed and not cfg.per_frame else None
+    added = None if cfg.per_frame else emb.added_cls       # M = 1: the kernel reads no added_cls row
+    ops.vip_embed_tables(emb.position_embedding.weight, temporal, emb.class_embedding, added, table, x0, B, T, L,
                          M, C_, cfg.temporal_size)
     wp = _small_bf16(model, "patch", emb.patch_embedding.weight).view(C_, Kp)
     if ldp != Kp:   # e.g. p = 14: the GEMM's B operand needs the same 16-byte row pitch as the patch matrix
@@ -570,7 +614,7 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
     """dproj_bf16 [B, proj] = gradient w.r.t. the un-normalised projection output."""
     cfg = model.config
     vm = model.vision_model
-    C_, L, M = cfg.vision.hidden_size, cfg.num_patches, 1 + cfg.add_cls_num
+    C_, L, M = cfg.vision.hidden_size, cfg.num_patches, cfg.num_global_tokens
     H = cfg.vision.num_attention_heads
     B, T, S, rows = sv.B, sv.T, sv.S, sv.rows
     dev = dproj_bf16.device
@@ -613,7 +657,7 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
                       B * M, C_)
     emb = "vision_model.embeddings."
     ops.vip_embed_bwd(d_patch, d_glob, grads[emb + "position_embedding.weight"],
-                      grads.get(emb + "temporal_embedding"), grads[emb + "class_embedding"], grads[emb + "added_cls"],
+                      grads.get(emb + "temporal_embedding"), grads[emb + "class_embedding"], grads.get(emb + "added_cls"),
                       B, T, L, M, C_, cfg.temporal_size)
     Kp = 3 * cfg.patch_size * cfg.patch_size
     if sv.patches.shape[1] == Kp:
@@ -734,7 +778,13 @@ class _ClipVipFunction(torch.autograd.Function):
                 enc = model.text_model.encoder
                 proj, sv = _text_fwd(model, input_ids, attention_mask, tower_save,
                                      tower_save and enc.gradient_checkpointing and enc.training)
-            if normalize:
+            # per-frame model, video input: the frame-mean head (VidCLIP.py:62-65) over each video's T frame projections
+            pool_t = video.shape[1] if which == "vis" and model.config.per_frame and video.dim() == 5 else 0
+            if normalize and pool_t:
+                feat = torch.empty(proj.shape[0] // pool_t, proj.shape[1], dtype=f32, device=dev)
+                inv = (torch.empty(proj.shape[0], dtype=f32, device=dev), torch.empty(feat.shape[0], dtype=f32, device=dev))
+                ops.frame_pool_fwd(proj, feat, inv[0], inv[1], pool_t)
+            elif normalize:
                 feat = torch.empty_like(proj)
                 inv = torch.empty(proj.shape[0], dtype=f32, device=dev)
                 ops.l2norm_fwd(proj, feat, inv)
@@ -742,6 +792,7 @@ class _ClipVipFunction(torch.autograd.Function):
                 feat, inv = proj, None
             if sv is not None:
                 sv.feat, sv.inv = feat, inv
+                sv.pool = (proj, pool_t) if normalize and pool_t else None
                 setattr(ctx, which, sv)
             return feat
 
@@ -818,12 +869,18 @@ def _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, nam
     rest = {n: tuple(named[n].shape) for n in names if n.startswith(tower + ".") and ".encoder.layers." not in n}
     rest[proj_name] = tuple(named[proj_name].shape)
     grads["__flat__" + tower] = _alloc_flat(rest, grads, dev)
-    dproj = torch.empty(dfeat.shape, dtype=bf16, device=dev)
-    dfeat = dfeat.contiguous().to(f32)
-    if ctx.normalize:
-        ops.l2norm_bwd(dfeat, sv.feat, sv.inv, dproj)
+    pool = getattr(sv, "pool", None)
+    if pool is not None:        # frame-mean head: d(video feature) [B, P] -> d(frame projections) [B*T, P]
+        proj, pool_t = pool
+        dproj = torch.empty(proj.shape, dtype=bf16, device=dev)
+        ops.frame_pool_bwd(dfeat.contiguous().to(f32), sv.feat, proj, sv.inv[0], sv.inv[1], dproj, pool_t)
     else:
-        dproj.copy_(dfeat)
+        dproj = torch.empty(dfeat.shape, dtype=bf16, device=dev)
+        dfeat = dfeat.contiguous().to(f32)
+        if ctx.normalize:
+            ops.l2norm_bwd(dfeat, sv.feat, sv.inv, dproj)
+        else:
+            dproj.copy_(dfeat)
     bwd(model, dproj, sv, grads)
     _grads_ready(model, grads, tower)
     for i in range(len(tw.encoder.layers)):

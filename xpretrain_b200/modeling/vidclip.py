@@ -25,7 +25,9 @@ def config_from_args(args) -> ClipVipConfig:
     `args.clip_config` (a local HF-style config.json / directory if it exists, else the built-in hyper-parameters of the
     name: "openai/clip-vit-large-patch14" / "-patch14-336" (ViT-L/14 at 224 / 336 px), "...patch32" (ViT-B/32), and
     otherwise the ViT-B/16 defaults of "openai/clip-vit-base-patch16" — there is no network) and the ViP additions from
-    `args.clip_vision_additional_config`."""
+    `args.clip_vision_additional_config`.  Its `type` picks the vision model (VidCLIP.py:14-23): "ViP" (the default) is
+    the video-proxy tower; any other value is the per-frame CLIP model of CLIP.py, which ignores temporal_size,
+    add_cls_num and if_use_temporal_embed."""
     src = _get(args, "clip_config")
     cfg = copy.deepcopy(src) if isinstance(src, ClipVipConfig) else ClipVipConfig()
     path = None
@@ -54,9 +56,7 @@ def config_from_args(args) -> ClipVipConfig:
     elif isinstance(src, str) and "patch32" in src:
         cfg.patch_size = 32
     add = _get(args, "clip_vision_additional_config")
-    if _get(add, "type", "ViP") != "ViP":
-        raise NotImplementedError("only vision_additional_config.type == 'ViP' is on the H100 hot path "
-                                  "(the non-ViP twin CLIP.py is an ablation baseline, SURVEY.md §2.1)")
+    cfg.vision_type = str(_get(add, "type", cfg.vision_type))
     cfg.temporal_size = int(_get(add, "temporal_size", 12))
     cfg.if_use_temporal_embed = int(_get(add, "if_use_temporal_embed", 1))
     cfg.add_cls_num = int(_get(add, "add_cls_num", 3))
@@ -72,7 +72,8 @@ class VidCLIP(nn.Module):
         self.clipmodel = CLIPModel(cfg)
         weights = _get(args, "clip_weights")
         if weights and os.path.exists(str(weights)):
-            # VidCLIP.py:14-18 loads plain OpenAI-CLIP weights; added_cls / temporal_embedding keep their init
+            # VidCLIP.py:14-18 loads plain OpenAI-CLIP weights; the ViP tower's added_cls / temporal_embedding keep their
+            # init, and the per-frame model takes every key of such a checkpoint
             path = weights if os.path.isfile(weights) else os.path.join(weights, "pytorch_model.bin")
             sd = torch.load(path, map_location="cpu")
             sd = {k[len("clipmodel."):] if k.startswith("clipmodel.") else k: v for k, v in sd.items()}
@@ -86,6 +87,9 @@ class VidCLIP(nn.Module):
 
     def forward(self, video, text_input_ids, text_input_mask, image=None, caption_ids=None, caption_masks=None):
         """video [B, T, C, H, W]; text_input_ids / text_input_mask [B, L] (VidCLIP.py:32-81)."""
+        if image is not None and self.clipmodel.config.per_frame:
+            # the reference's per-frame CLIP model is handed a 5-D image tensor here and fails inside Conv2d
+            raise ValueError("the per-frame CLIP model (vision_additional_config.type != 'ViP') has no image/caption branch")
         out = self.clipmodel(input_ids=text_input_ids, attention_mask=text_input_mask, pixel_values=video,
                              return_loss=False)
         results = {"text_features": out["text_embeds"], "vis_features": out["image_embeds"]}

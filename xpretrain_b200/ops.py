@@ -169,6 +169,26 @@ def l2norm_bwd(dy, y, inv_norm, dx_bf16, scale: float = 1.0):
     check(lib().xp_l2norm_bwd(_p(dy), _p(y), _p(inv_norm), _p(dx_bf16), rows, C_, scale, _stream()), "xp_l2norm_bwd")
 
 
+def frame_pool_fwd(proj, feat, inv_frame, inv_video, T: int):
+    """Frame-mean head (VidCLIP.py:62-65): proj fp32 [B*T, P] -> feat fp32 [B, P] = normalise(mean_t normalise(p_t)),
+    with the inverse norms inv_frame [B*T] and inv_video [B] saved for the backward."""
+    rows, P = proj.shape
+    B = feat.shape[0]
+    assert proj.dtype == f32 and feat.dtype == f32 and proj.is_contiguous() and feat.is_contiguous()
+    assert rows == B * T and feat.shape[1] == P and inv_frame.numel() == rows and inv_video.numel() == B
+    check(lib().xp_frame_pool_fwd(_p(proj), _p(feat), _p(inv_frame), _p(inv_video), B, T, P, _stream()),
+          "xp_frame_pool_fwd")
+
+
+def frame_pool_bwd(dfeat, feat, proj, inv_frame, inv_video, dproj_bf16, T: int, scale: float = 1.0):
+    """dproj bf16 [B*T, P] = scale * gradient of the frame-mean head w.r.t. proj, given dfeat fp32 [B, P]."""
+    B, P = feat.shape
+    assert dfeat.dtype == f32 and dfeat.is_contiguous() and dfeat.shape == feat.shape
+    assert dproj_bf16.dtype == bf16 and dproj_bf16.is_contiguous() and dproj_bf16.shape == (B * T, P)
+    check(lib().xp_frame_pool_bwd(_p(dfeat), _p(feat), _p(proj), _p(inv_frame), _p(inv_video), _p(dproj_bf16), B, T, P,
+                                  scale, _stream()), "xp_frame_pool_bwd")
+
+
 def colsum(x: torch.Tensor, out: torch.Tensor, scale: float = 1.0):
     rows, C_ = x.shape
     check(lib().xp_colsum_bf16(_p(x), x.stride(0), _p(out), rows, C_, scale, _stream()), "xp_colsum_bf16")
