@@ -40,7 +40,10 @@ void xp_launch_count_reset(void);
  * a_layout: 0 = A stored [M,K] (K contiguous), 1 = A stored [K,M] (M contiguous)
  * b_layout: 0 = B stored [N,K] (K contiguous, nn.Linear.weight), 1 = B stored [K,N]
  * Epilogue, in this order:  v = alpha*acc; v += bias[n]; if n < scale_cols: v *= col_scale
- *   (CLIP_ViP.py:341 scales q AFTER the bias); act; v += residual[m,n]; store.
+ *   (CLIP_ViP.py:341 scales q AFTER the bias); then EITHER act OR v += residual[m,n]; store.
+ * Refused with an error: a residual together with any activation, aux together with c_group > 0, an odd or negative
+ * scale_cols, split-K without XP_OUT_F32_ATOMIC, an activation with an fp32 output.  Any K >= 1 is computed exactly as
+ * K rounded up to the 64-wide k-block with zeros (TMA fills the missing k-columns with 0), so K < 64 is supported.
  */
 enum { XP_ACT_NONE = 0, XP_ACT_QUICK_GELU = 1, XP_ACT_DQUICK_GELU = 2, XP_ACT_GELU_ERF = 3, XP_ACT_DGELU_ERF = 4 };
 enum { XP_OUT_BF16 = 0, XP_OUT_F32 = 1, XP_OUT_F32_ATOMIC = 2 };
@@ -62,7 +65,8 @@ typedef struct XpGemm {
   float alpha, col_scale;
   /* Optional grouped row addressing (0 = plain row*ld): element offset of row r is
    *   (r / group) * group_stride + (r % group) * ld.
-   * C (and aux) use c_group; residual uses r_group (r_group_stride = 0 makes the residual a
+   * C uses c_group (aux is always addressed row * ld_aux, so it is refused with c_group > 0); residual uses r_group
+   * (r_group_stride = 0 makes the residual a
    * periodic [r_group, N] table, used for the patch-embedding position+temporal add). */
   int64_t c_group, c_group_stride, r_group, r_group_stride;
   int32_t block_n;    /* 0 = auto, 128 = ping-pong 128x128 tiles, 256 = cooperative 128x256 tiles */

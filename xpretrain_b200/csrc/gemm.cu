@@ -436,8 +436,12 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
   if ((g->act == XP_ACT_DQUICK_GELU || g->act == XP_ACT_DGELU_ERF) && !g->aux)
     return fail("xp_gemm: dGELU epilogue needs aux (the forward pre-activation)");
   if (g->act != XP_ACT_NONE && g->out != XP_OUT_BF16) return fail("xp_gemm: activation epilogues need a bf16 output");
-  if ((g->act == XP_ACT_DQUICK_GELU || g->act == XP_ACT_DGELU_ERF) && g->residual)
-    return fail("xp_gemm: a dGELU epilogue cannot be combined with a residual add");
+  // The epilogue adds a residual only after no activation, addresses aux as plain rows, and tests `n < scale_cols` once
+  // per column pair: the combinations below would silently compute something else, so they are refused.
+  if (g->act != XP_ACT_NONE && g->residual)
+    return fail("xp_gemm: a residual add cannot be combined with an activation epilogue");
+  if (g->aux && g->c_group > 0) return fail("xp_gemm: aux cannot be combined with grouped rows (c_group > 0)");
+  if (g->scale_cols < 0 || g->scale_cols % 2) return fail("xp_gemm: scale_cols must be even and non-negative");
   const int elem_c = g->out == XP_OUT_BF16 ? 2 : 4;
   if ((reinterpret_cast<uintptr_t>(g->c) & 15) || (g->ldc * elem_c) % 16)
     return fail("xp_gemm: C must be 16-byte aligned with a 16-byte multiple row pitch");

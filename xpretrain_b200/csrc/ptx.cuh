@@ -243,9 +243,14 @@ __device__ __forceinline__ float fast_sigmoid(float y) {
 }
 // QuickGELU = x * sigmoid(1.702 x) (transformers QuickGELUActivation, selected at CLIP_ViP.py:389)
 __device__ __forceinline__ float quick_gelu(float x) { return x * fast_sigmoid(1.702f * x); }
+// y is clamped to [-64, 64]: beyond |y| ~ 17 the fp32 sigmoid is already exactly 0 or 1, so no finite result changes,
+// but for |x| >~ 2e38 (within bf16 range) the unclamped 1.702 x overflows and y * (1 - s) becomes inf * 0 = NaN.
+// Comparisons rather than fminf / fmaxf, so that a NaN x still gives NaN.
 __device__ __forceinline__ float quick_gelu_grad(float x) {
-  const float s = fast_sigmoid(1.702f * x);
-  return s * fmaf(1.702f * x, 1.f - s, 1.f);
+  float y = 1.702f * x;
+  y = y > 64.f ? 64.f : (y < -64.f ? -64.f : y);
+  const float s = fast_sigmoid(y);
+  return s * fmaf(y, 1.f - s, 1.f);
 }
 
 }  // namespace xp
