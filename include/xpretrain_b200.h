@@ -192,28 +192,29 @@ int xp_text_attention_bwd(const void* qkv, const void* dout, const float* probs,
                           int32_t Lt, int32_t C, float q_scale, void* stream);
 
 /* ------------------------------------------------------------------ InfoNCE --
- * NCELearnableTempLoss.forward (loss.py:134-141) on the gathered [N, d] fp32 embeddings.  The logits GEMM and the
- * two gradient GEMMs run through xp_gemm; these are the pieces around them:
+ * NCELearnableTempLoss.forward (loss.py:134-141) on the gathered [N, d] fp32 embeddings: xp_nce_gather_fused below, or,
+ * for global batches beyond it, the logits GEMM through xp_gemm on the split operands and xp_nce_terms with the table
+ * ((rows, A), (columns, A)); the two gradient GEMMs run through xp_gemm.
  *   xp_nce_split:        x f32 [rows, d] -> x3 bf16 [rows, 3d] = [hi|hi|lo] (pattern 0) or [hi|lo|hi] (pattern 1),
  *                        so that x3_a . x3_b^T = hi*hi + hi*lo + lo*hi (fp32-grade logits on bf16 tensor cores);
- *                        hi_bf16 (optional) receives the plain bf16 copy used by the gradient GEMMs.
- *   xp_nce_softmax_grad: z f32 [N, N] (row pitch ld, shared with g_scaled) = V T^T (unscaled) -> row/col LSE of exp(logit_scale)*z, the scalar loss
- *                        (overwritten), d_logit_scale (ACCUMULATED) and g_scaled bf16 [N,N] = exp(logit_scale) * dL/dZ. */
+ *                        hi_bf16 (optional) receives the plain bf16 copy used by the gradient GEMMs. */
 int xp_nce_split(const float* x, void* x3_bf16, void* hi_bf16, int32_t rows, int32_t d, int32_t pattern, void* stream);
-int xp_nce_softmax_grad(const float* z, const float* logit_scale, float* lse_rows, float* lse_cols, void* g_scaled_bf16,
-                        float* loss, float* d_logit_scale, int32_t N, int64_t ld, void* stream);
 /* Fused exchange + loss: replaces `hvd.allgather(vis)`, `hvd.allgather(txt)` (CLIP-ViP/src/pretrain/run_pretrain.py:344-345;
  * rank-major concat, semantics pinned by LF-VILA/src/utils/dist.py:21-41) AND NCELearnableTempLoss.forward (loss.py:134-141)
  * with ONE cooperative kernel (csrc/nce_fused.cu): device-side flag barrier over peer-mapped exchange buffers, logits tiles
  * on wgmma whose operand rows are loaded straight from the owning peer's memory over NVLink (hi/lo split in the producer),
  * row/column log-sum-exps, loss (overwritten), d logit_scale (overwritten), g_scaled bf16 [N, ld_g] = exp(logit_scale)*dL/dZ,
- * and the bf16 copies vis_hi / txt_hi [N, d] that the local gradient GEMMs use.  N = world * b <= 1536.
+ * and the bf16 copies vis_hi / txt_hi [N, d] that the local gradient GEMMs use.  N = world * b <= 1536.  It writes
+ * exactly the N x N block of g_scaled (columns N..ld_g untouched) and all of vis_hi / txt_hi; loss, d_logit_scale, g_scaled
+ * and the copies are bit-identical across calls and, in mode 0, on every rank.  vis_local / txt_local and the rows
+ * behind peer_bufs are read with 16-byte vector loads: every row pointer must be 16-byte aligned.
  *   mode 0: peer_bufs = device array of `world` exchange-buffer base pointers (own buffer at [rank]); every buffer is
  *           xp_nce_gather_exchange_bytes() large, zero-initialised once, and mapped by all ranks (symmetric memory);
  *           vis_local / txt_local fp32 [b, d] are published by the kernel; `epoch` must increase by 1 per call (from 1).
  *   mode 1: no exchange: peer_bufs = device array of 2*world pointers, [r] = rank r's vis rows, [world + r] = its txt rows
  *           (fp32 [b, d]) in local memory (single process, or rows pre-gathered by another transport).
- * workspace: xp_nce_gather_workspace_bytes(N) bytes, zero-initialised once (it holds the kernel's barrier counters). */
+ * workspace: xp_nce_gather_workspace_bytes(N) bytes: per-tile partials, which need no initialisation, followed by three
+ * barrier counters, which must be zero before the first call; every call leaves them zero. */
 typedef struct XpNceGather {
   const float* vis_local;
   const float* txt_local;

@@ -100,8 +100,6 @@ SIGNATURES = {
     "xp_text_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
                                       c_void_p]),
     "xp_nce_split": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "xp_nce_softmax_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                    c_i64, c_void_p]),
     "xp_nce_gather_exchange_bytes": (c_i64, [c_int, c_int, c_int]),
     "xp_nce_gather_workspace_bytes": (c_i64, [c_int]),
     "xp_nce_gather_fused": (c_int, [P(XpNceGather), c_void_p]),

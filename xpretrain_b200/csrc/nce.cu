@@ -1,15 +1,14 @@
-// In-batch video<->text InfoNCE with a learnable temperature: NCELearnableTempLoss.forward, loss.py:134-141,
-// on the rank-major gathered embeddings (hvd.allgather, run_pretrain.py:344-345).
-//
+// The contrastive losses of loss.py around the wgmma GEMM (gemm.cu): the hi/lo split that makes the logits GEMM
+// fp32-grade, and the table-driven InfoNCE family and dual-softmax loss on its fp32 logits.  NCELearnableTempLoss
+// (loss.py:134-141) beyond the fused kernel's reach is the table ((rows, A), (columns, A)):
 //   Z = exp(logit_scale) * V T^T                     [N, N]   (rows = videos)
 //   loss = mean_i(LSE_j Z_ij - Z_ii) + mean_j(LSE_i Z_ij - Z_jj)        (SUM of the two CEs, no 1/2)
 //   G = dL/dZ = (softmax_rows(Z) + softmax_cols(Z) - 2I) / N
 //   dV = s G T,  dT = s G^T V,  d logit_scale = sum_ij G_ij Z_ij         (SURVEY.md §8e closed form)
 //
-// The two GEMM-shaped steps run on the wgmma GEMM (gemm.cu).  To keep fp32-level logits out of bf16
-// tensor-core inputs, V and T are split into bf16 hi + lo parts and the three significant cross terms are
-// concatenated along K:  [Vh | Vh | Vl] . [Th | Tl | Th]^T  (K = 3d), i.e. one GEMM, ~2^-16 relative error.
-// The kernels here are the prep / softmax / gradient pieces around those GEMMs.
+// To keep fp32-level logits out of bf16 tensor-core inputs, V and T are split into bf16 hi + lo parts and the three
+// significant cross terms are concatenated along K:  [Vh | Vh | Vl] . [Th | Tl | Th]^T  (K = 3d), i.e. one GEMM,
+// ~2^-16 relative error.
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "ptx.cuh"
@@ -30,51 +29,6 @@ nce_split_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ x3, __
     o[d + c] = pattern == 0 ? hi : lo;
     o[2 * d + c] = pattern == 0 ? lo : hi;
     if (hi_out) hi_out[r * d + c] = hi;
-  }
-}
-
-// lse[i] = log sum_j exp(s * Z[i*si + j*sj]) ; one warp per output, 4 per CTA.
-__global__ void __launch_bounds__(128)
-nce_lse_kernel(const float* __restrict__ z, const float* __restrict__ logit_scale, float* __restrict__ lse, int N,
-               long long si, long long sj) {
-  const int i = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (i >= N) return;
-  const float s = expf(*logit_scale);
-  float mx = -INFINITY;
-  for (int j = lane; j < N; j += 32) mx = fmaxf(mx, s * z[i * si + j * sj]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-  for (int j = lane; j < N; j += 32) sum += expf(s * z[i * si + j * sj] - mx);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if (lane == 0) lse[i] = mx + logf(sum);
-}
-
-// One CTA per row i: G'[i,j] = s * G[i,j] (bf16), loss += (lse_r[i] + lse_c[i] - 2 Z_ii)/N, dscale += sum_j G_ij Z_ij.
-__global__ void __launch_bounds__(128)
-nce_grad_kernel(const float* __restrict__ z, const float* __restrict__ logit_scale, const float* __restrict__ lse_r,
-                const float* __restrict__ lse_c, __nv_bfloat16* __restrict__ g_scaled, float* __restrict__ loss,
-                float* __restrict__ dscale, int N, long long ld) {
-  __shared__ float red[4];
-  const int i = blockIdx.x;
-  const float s = expf(*logit_scale);
-  const float inv_n = 1.f / N;
-  float acc = 0.f;
-  for (int j = threadIdx.x; j < N; j += blockDim.x) {
-    const float zz = s * z[static_cast<long long>(i) * ld + j];
-    float g = (expf(zz - lse_r[i]) + expf(zz - lse_c[j]) - (i == j ? 2.f : 0.f)) * inv_n;
-    acc += g * zz;
-    if (g_scaled) g_scaled[static_cast<long long>(i) * ld + j] = __float2bfloat16(g * s);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (dscale) atomicAdd(dscale, red[0] + red[1] + red[2] + red[3]);
-    const float zii = s * z[static_cast<long long>(i) * ld + i];
-    atomicAdd(loss, (lse_r[i] + lse_c[i] - 2.f * zii) * inv_n);
   }
 }
 
@@ -585,22 +539,5 @@ extern "C" int xp_nce_split(const float* x, void* x3_bf16, void* hi_bf16, int32_
   nce_split_kernel<<<rows, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       x, static_cast<__nv_bfloat16*>(x3_bf16), static_cast<__nv_bfloat16*>(hi_bf16), d, pattern);
   XP_CHECK_LAUNCH("nce_split_kernel");
-  return 0;
-}
-
-extern "C" int xp_nce_softmax_grad(const float* z, const float* logit_scale, float* lse_rows, float* lse_cols,
-                                   void* g_scaled_bf16, float* loss, float* d_logit_scale, int32_t N, int64_t ld,
-                                   void* stream) {
-  XP_ENTER(z);
-  if (N <= 0) return fail("xp_nce_softmax_grad: N must be positive");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  XP_CHECK_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
-  nce_lse_kernel<<<(N + 3) / 4, 128, 0, st>>>(z, logit_scale, lse_rows, N, ld, 1);
-  XP_CHECK_LAUNCH("nce_lse_kernel");
-  nce_lse_kernel<<<(N + 3) / 4, 128, 0, st>>>(z, logit_scale, lse_cols, N, 1, ld);
-  XP_CHECK_LAUNCH("nce_lse_kernel");
-  nce_grad_kernel<<<N, 128, 0, st>>>(z, logit_scale, lse_rows, lse_cols, static_cast<__nv_bfloat16*>(g_scaled_bf16),
-                                     loss, d_logit_scale, N, ld);
-  XP_CHECK_LAUNCH("nce_grad_kernel");
   return 0;
 }

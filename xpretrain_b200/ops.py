@@ -285,16 +285,11 @@ def nce_split(x, x3, hi, pattern: int):
     check(lib().xp_nce_split(_p(x), _p(x3), _p(hi), rows, d, pattern, _stream()), "xp_nce_split")
 
 
-def nce_softmax_grad(z, logit_scale, lse_r, lse_c, g_scaled, loss, d_logit_scale):
-    N, ld = z.shape[0], z.stride(0)
-    check(lib().xp_nce_softmax_grad(_p(z), _p(logit_scale), _p(lse_r), _p(lse_c), _p(g_scaled), _p(loss),
-                                    _p(d_logit_scale), N, ld, _stream()), "xp_nce_softmax_grad")
-
-
-def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logit_scale=None):
+def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logit_scale=None, workspace=None):
     """Loss, d logit_scale and s * dL/dZ of a table of cross-entropy terms over up to three logits matrices (xp_nce_terms).
     z: fp32 [n_m, ld_m] unscaled logits; g: matching bf16 outputs; terms: (axis, members, excl_diag, target) per term, with
-    members / excl_diag as bit masks over the matrices.  The scale is exp(logit_scale[0]) or, without logit_scale, `scale`."""
+    members / excl_diag as bit masks over the matrices.  The scale is exp(logit_scale[0]) or, without logit_scale, `scale`.
+    workspace: fp32, at least xp_nce_terms_workspace_bytes; allocated here when None."""
     a = _lib.XpNceTerms()
     a.n_mats, a.n_terms = len(z), len(terms)
     for m, (zm, gm) in enumerate(zip(z, g)):
@@ -306,19 +301,24 @@ def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logi
     nbytes = int(lib().xp_nce_terms_workspace_bytes(C.byref(a)))
     if nbytes < 0:
         raise _lib.XpError("xp_nce_terms_workspace_bytes: invalid matrix sizes")
-    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z[0].device)
+    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z[0].device) if workspace is None else workspace
+    if ws.numel() * 4 < nbytes:
+        raise _lib.XpError(f"xp_nce_terms: the workspace needs {nbytes} bytes")
     a.workspace = _p(ws)
     check(lib().xp_nce_terms(C.byref(a), _stream()), "xp_nce_terms")
 
 
-def nce_dsl(z, logit_scale, g, loss, d_logit_scale):
-    """NCELearnableTempDSLLoss on the unscaled logits z fp32 [n, ld]: loss, d logit_scale and s * dL/dZ (bf16, pitch ld)."""
+def nce_dsl(z, logit_scale, g, loss, d_logit_scale, workspace=None):
+    """NCELearnableTempDSLLoss on the unscaled logits z fp32 [n, ld]: loss, d logit_scale and s * dL/dZ (bf16, pitch ld).
+    workspace: fp32, at least xp_nce_dsl_workspace_bytes(n); allocated here when None."""
     n, ld = z.shape[0], z.stride(0)
     assert z.dtype == f32 and g.dtype == bf16 and g.stride(0) == ld
     nbytes = int(lib().xp_nce_dsl_workspace_bytes(n))
     if nbytes < 0:
         raise _lib.XpError("xp_nce_dsl_workspace_bytes: n must be positive")
-    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z.device)
+    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z.device) if workspace is None else workspace
+    if ws.numel() * 4 < nbytes:
+        raise _lib.XpError(f"xp_nce_dsl: the workspace needs {nbytes} bytes")
     check(lib().xp_nce_dsl(_p(z), ld, n, _p(logit_scale), _p(g), _p(loss), _p(d_logit_scale), _p(ws), _stream()),
           "xp_nce_dsl")
 

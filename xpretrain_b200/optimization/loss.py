@@ -25,26 +25,29 @@ def _pad8(n: int) -> int:
 FUSED_MAX_N = 1536      # (N / 128)^2 tiles of the fused kernel must be co-resident: up to two per SM on the 132 SMs of an H100
 
 
-def _nce_forward_unfused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor):
-    """Global batches above FUSED_MAX_N: split / GEMM / softmax-grad as separate launches.
-    vis, txt: [N, d] fp32 (gathered).  Returns (loss[1], g_scaled[N, Np] bf16, vis_hi, txt_hi, dscale[1])."""
+def _split_logits(vis: torch.Tensor, txt: torch.Tensor):
+    """The unscaled logits V T^T of fp32 [N, d] rows as one hi/lo-split GEMM (fp32-grade on bf16 tensor cores).
+    Returns (z fp32 [N, Np], vis_hi [N, d], txt_hi [N, d]); the pad columns N..Np of z are zero."""
     N, d = vis.shape
     Np = _pad8(N)
-    dev = vis.device
-    a3 = torch.empty(N, 3 * d, dtype=bf16, device=dev)
-    b3 = torch.zeros(Np, 3 * d, dtype=bf16, device=dev) if Np != N else torch.empty(N, 3 * d, dtype=bf16, device=dev)
-    vh = torch.empty(N, d, dtype=bf16, device=dev)
-    th = torch.empty(N, d, dtype=bf16, device=dev)
-    ops.nce_split(vis.contiguous(), a3, vh, 0)
-    ops.nce_split(txt.contiguous(), b3, th, 1)
-    z = torch.empty(N, Np, dtype=f32, device=dev)
-    ops.gemm(a3, b3, z, M=N, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
-    lse_r = torch.empty(N, dtype=f32, device=dev)
-    lse_c = torch.empty(N, dtype=f32, device=dev)
-    g = torch.empty(N, Np, dtype=bf16, device=dev)
-    loss = torch.empty(1, dtype=f32, device=dev)
-    dscale = torch.zeros(1, dtype=f32, device=dev)
-    ops.nce_softmax_grad(z, temp.detach().reshape(1).to(f32), lse_r, lse_c, g, loss, dscale)
+    v3, vh = _split_hi(vis, N, 0)
+    t3, th = _split_hi(txt, Np, 1)
+    z = torch.empty(N, Np, dtype=f32, device=vis.device)
+    ops.gemm(v3, t3, z, M=N, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
+    return z, vh, th
+
+
+def _nce_forward_unfused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor):
+    """Global batches above FUSED_MAX_N, and widths the fused kernel does not take: the split logits GEMM, then
+    xp_nce_terms with the two-term table at the device logit_scale (fixed-order reductions, so loss and d logit_scale are
+    bit-identical across calls and across ranks).  vis, txt: [N, d] fp32 (gathered).
+    Returns (loss[1], g_scaled[N, Np] bf16, vis_hi, txt_hi, dscale[1])."""
+    z, vh, th = _split_logits(vis, txt)
+    g = torch.empty(z.shape, dtype=bf16, device=z.device)
+    loss = torch.empty(1, dtype=f32, device=z.device)
+    dscale = torch.empty(1, dtype=f32, device=z.device)
+    ops.nce_terms([z], [g], TERM_TABLES["NCEContrastiveLoss"][1], loss, logit_scale=temp.detach().reshape(1).to(f32),
+                  d_logit_scale=dscale)
     return loss, g, vh, th, dscale
 
 
@@ -90,6 +93,13 @@ class _Exchange:
 _local_ws = {}
 
 
+def _aligned(x: torch.Tensor) -> torch.Tensor:
+    """x contiguous and 16-byte aligned: the fused kernel reads caller rows with 16-byte vector loads, and a contiguous
+    view may start anywhere in its allocation."""
+    x = x.contiguous()
+    return x if x.data_ptr() % 16 == 0 else x.clone()
+
+
 def _nce_forward_fused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor, exchange: "_Exchange" = None, group=None):
     """One launch of csrc/nce_fused.cu.  vis, txt: this rank's [b, d] fp32 rows.  Returns (loss[1], g_scaled[N, Np] bf16,
     vis_hi[N, d], txt_hi[N, d], dscale[1]) for the global batch N = world * b."""
@@ -98,7 +108,7 @@ def _nce_forward_fused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor,
     world = exchange.world if exchange is not None else 1
     N = world * b
     Np = _pad8(N)
-    vis, txt = vis.contiguous(), txt.contiguous()
+    vis, txt = _aligned(vis), _aligned(txt)
     g = (torch.zeros if Np != N else torch.empty)(N, Np, dtype=bf16, device=dev)
     vh = torch.empty(N, d, dtype=bf16, device=dev)
     th = torch.empty(N, d, dtype=bf16, device=dev)
@@ -339,12 +349,8 @@ class _NceDslFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, vis, txt, temp):
-        N, d = vis.shape
-        Np, dev = _pad8(N), vis.device
-        v3, vh = _split_hi(vis.to(f32), N, 0)
-        t3, th = _split_hi(txt.to(f32), Np, 1)
-        z = torch.empty(N, Np, dtype=f32, device=dev)
-        ops.gemm(v3, t3, z, M=N, N=Np, K=3 * d, lda=3 * d, ldb=3 * d, ldc=Np, out_mode=_lib.OUT_F32)
+        z, vh, th = _split_logits(vis.to(f32), txt.to(f32))
+        N, Np, dev = z.shape[0], z.shape[1], z.device
         g = torch.empty(N, Np, dtype=bf16, device=dev)
         loss = torch.empty(1, dtype=f32, device=dev)
         dscale = torch.empty(1, dtype=f32, device=dev)
