@@ -318,6 +318,26 @@ int xp_seg_attention_fwd(const void* qkv, void* out, float* lse, const XpSegAttn
 int xp_seg_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta, void* dqkv,
                          const XpSegAttn* desc, float q_scale, void* stream);
 
+/* xp_dense_attention_{fwd,bwd}: non-causal, unmasked multi-head attention (head_dim 64) over n_seq sequences of seq_len
+ * CONSECUTIVE rows of a token-major fused [n_rows, ld_qkv] bf16 buffer (columns [q|k|v], head h at h*64, q pre-scaled by
+ * head_dim**-0.5): sequence s is rows [s*seq_len, (s+1)*seq_len).  Replaces Attention.forward (timesformer.py:156-173)
+ * for attention_type 'joint_space_time' (one sequence per clip of H*W*T rows, :202-205) and 'space_only' (one per frame).
+ *   n_rows >= n_seq * seq_len; seq_len >= 1 (any length: the 64-row tiles are masked at the end of each sequence, and
+ *   rows of the next sequence never enter); n_seq <= 65535; heads * (n_seq * seq_len) < 2^31.
+ *   ld_qkv >= 3*heads*64 and ld_out >= heads*64, both multiples of 8; qkv, dout 16-byte aligned (TMA).
+ * out: [n_rows, ld_out] bf16, columns [0, 64*heads) of the sequences' rows overwritten, nothing else written;
+ * lse: [heads, n_rows] fp32 (natural log).  bwd: delta [heads, n_rows] fp32 scratch (rowsum(dO * O), written first);
+ * dqkv [n_rows, ld_qkv] bf16, columns [0, 3*64*heads) of the sequences' rows overwritten; dq is multiplied by q_scale.
+ * TMA + wgmma, warp-specialised; no float atomics, so results are bitwise repeatable. */
+typedef struct XpDenseAttn {
+  int64_t n_rows;
+  int64_t ld_qkv, ld_out;
+  int32_t heads, n_seq, seq_len, reserved;
+} XpDenseAttn;
+int xp_dense_attention_fwd(const void* qkv, void* out, float* lse, const XpDenseAttn* desc, void* stream);
+int xp_dense_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta,
+                           void* dqkv, const XpDenseAttn* desc, float q_scale, void* stream);
+
 /* Token assembly, TimeSformer.forward timesformer.py:481-509: x [B,T,C,H*W] (XP_DTYPE_*) -> tokens bf16 [(b, p, t), C]
  * (rows in the reference's (h w t) order) = x[b,t,:,p] + pos[p,:] + time[t,:]; pos [H*W, C] / time [T, C] fp32 are the
  * (already interpolated) tables, NULL = no table (plain tokenisation, used for the output gradient).

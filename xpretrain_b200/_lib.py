@@ -38,6 +38,11 @@ class XpSegAttn(C.Structure):
                 ("bias_windows", c_int), ("head_dim", c_int)]
 
 
+class XpDenseAttn(C.Structure):
+    _fields_ = [("n_rows", c_i64), ("ld_qkv", c_i64), ("ld_out", c_i64), ("heads", c_int), ("n_seq", c_int),
+                ("seq_len", c_int), ("reserved", c_int)]
+
+
 class XpNceGather(C.Structure):
     _fields_ = [("vis_local", c_void_p), ("txt_local", c_void_p), ("peer_bufs", c_void_p), ("logit_scale", c_void_p),
                 ("g_scaled", c_void_p), ("vis_hi", c_void_p), ("txt_hi", c_void_p), ("loss", c_void_p),
@@ -110,6 +115,9 @@ SIGNATURES = {
     "xp_seg_attention_fwd":(c_int, [c_void_p, c_void_p, c_void_p, P(XpSegAttn), c_void_p]),
     "xp_seg_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, P(XpSegAttn), c_float,
                                      c_void_p]),
+    "xp_dense_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, P(XpDenseAttn), c_void_p]),
+    "xp_dense_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, P(XpDenseAttn),
+                                       c_float, c_void_p]),
     "xp_tsf_embed_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "xp_tsf_untokenize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "xp_layernorm_wide_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_float,

@@ -106,6 +106,24 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64
   return 0;
 }
 
+int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t mid, uint64_t outer,
+                      uint64_t row_stride, uint64_t mid_stride, uint32_t box_inner, uint32_t box_mid) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return fail("cuTensorMapEncodeTiled unavailable (no CUDA driver / no GPU): this library has no CPU path");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("tensor map: base pointer must be 16-byte aligned");
+  if ((row_stride * 2) % 16 != 0 || (mid_stride * 2) % 16 != 0)
+    return fail("tensor map: strides must be multiples of 8 bf16 elements");
+  cuuint64_t dims[3] = {inner, mid, outer};
+  cuuint64_t strides[2] = {row_stride * 2, mid_stride * 2};
+  cuuint32_t box[3] = {box_inner, box_mid, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed with CUresult " + std::to_string(int(r)));
+  return 0;
+}
+
 }  // namespace xp
 
 extern "C" {

@@ -20,6 +20,10 @@ int sm_count();  // SMs of the current device (cached per device)
 // elements, row_stride in elements, box = {box_inner, box_outer}.
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride,
                       uint32_t box_inner, uint32_t box_outer);
+// 3-D bf16 tensor map with 128-byte swizzle: extents {inner, mid, outer} in elements, strides of the mid and outer
+// dimensions in elements, box = {box_inner, box_mid, 1}.  Box rows past `mid` read as zero (TMA out-of-bounds fill).
+int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t mid, uint64_t outer,
+                      uint64_t row_stride, uint64_t mid_stride, uint32_t box_inner, uint32_t box_mid);
 
 // Bind the CUDA context that owns `device_ptr` to the calling thread if the thread has none.  PyTorch runs
 // autograd backward on worker threads that may not have touched CUDA yet; this library links its own

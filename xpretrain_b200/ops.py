@@ -8,7 +8,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import XpGemm, XpRowMap, XpSegAttn, check, lib
+from ._lib import XpDenseAttn, XpGemm, XpRowMap, XpSegAttn, check, lib
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -374,6 +374,24 @@ def seg_attention_fwd(qkv, out, lse, desc: XpSegAttn):
 def seg_attention_bwd(qkv, out, dout, lse, delta, dqkv, desc: XpSegAttn, q_scale: float):
     check(lib().xp_seg_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale,
                                      _stream()), "xp_seg_attention_bwd")
+
+
+def dense_desc(n_rows: int, heads: int, ld_qkv: int, ld_out: int, *, n_seq: int, seq_len: int) -> XpDenseAttn:
+    """n_seq sequences of seq_len consecutive rows, every row attending to every row of its sequence: one clip of H*W*T
+    tokens ('joint_space_time', timesformer.py:202-205) or one frame of H*W tokens ('space_only')."""
+    d = XpDenseAttn()
+    d.n_rows, d.ld_qkv, d.ld_out = n_rows, ld_qkv, ld_out
+    d.heads, d.n_seq, d.seq_len, d.reserved = heads, n_seq, seq_len, 0
+    return d
+
+
+def dense_attention_fwd(qkv, out, lse, desc: XpDenseAttn):
+    check(lib().xp_dense_attention_fwd(_p(qkv), _p(out), _p(lse), C.byref(desc), _stream()), "xp_dense_attention_fwd")
+
+
+def dense_attention_bwd(qkv, out, dout, lse, delta, dqkv, desc: XpDenseAttn, q_scale: float):
+    check(lib().xp_dense_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale,
+                                       _stream()), "xp_dense_attention_bwd")
 
 
 def tsf_embed_fwd(x, pos, time, tokens, B, T, C_, HW):
