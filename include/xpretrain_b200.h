@@ -134,34 +134,49 @@ enum { XP_DTYPE_F32 = 0, XP_DTYPE_BF16 = 1, XP_DTYPE_F16 = 2 };
 /* im2col of nn.Conv2d(3, width, kernel=stride=patch, bias=False) (CLIP_ViP.py:157-159,178-179):
  * video [frames,3,H,W] -> patches bf16 [frames*(H/p)*(W/p), ld]; the conv itself then runs as xp_gemm with K = 3*p*p.
  * Row pitch ld = round_up(3*p*p, 8) elements (16-byte rows, as TMA and xp_gemm need); columns [3*p*p, ld) are written
- * as zero.  ld = 3*p*p for p = 16 and 32; p = 14 (ViT-L/14) gives 588 columns in a pitch of 592.  Any p dividing H and W. */
+ * as zero.  ld = 3*p*p for p = 16 and 32; p = 14 (ViT-L/14) gives 588 columns in a pitch of 592.  Any p dividing H and W.
+ * Overwrites exactly the frames*(H/p)*(W/p) x ld patch matrix (pad columns included) and nothing else; every element is one
+ * conversion of an input value to bf16 (round to nearest even), bit-exact.  Alignment: patches_bf16 16 bytes (16-byte
+ * stores); for p % 8 == 0 also video 16 bytes (16-byte loads).  Misaligned pointers are refused before any launch. */
 int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_t frames, int32_t H, int32_t W,
                     int32_t patch, void* stream);
 /* The reference's input transform fused into the patch extraction (SURVEY.md §8f.4): frames_hwc uint8 [frames, H, W, 3] as
  * the decoder delivers them -> `.permute(0,3,1,2).float() / 255.` (CLIP-ViP/src/datasets/dataset_pretrain_stage1_all_source.py:182)
  * -> Normalize(mean, std) (init_transform_dict_simple, CLIP-ViP/src/datasets/dataloader.py:209-233; Resize / CenterCrop are
  * the identity at the input resolution) -> the bf16 patch matrix of xp_vip_patchify (same pitch).  IEEE fp32 arithmetic, one rounding to
- * bf16: bit-identical to casting the reference's fp32 tensor.  mean3 / std3 are HOST arrays of 3 floats. */
+ * bf16: bit-identical to casting the reference's fp32 tensor.  mean3 / std3 are HOST arrays of 3 floats.  Overwrites the
+ * patch matrix as xp_vip_patchify does.  Alignment: patches_bf16 16 bytes; for p % 8 == 0 also frames_hwc 8 bytes. */
 int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W, int32_t patch,
                        const float* mean3, const float* std3, void* stream);
 /* CLIP_ViP.py:170-176,183-195: table[t*L+l] = interp(temporal_embedding)[t] + position_embedding[1+l] (bf16,
  * [T*L, C]) and the M = 1 + add_cls_num global rows x[b, m] = (class_embedding | added_cls[m-1]) + position_embedding[0]
- * written into x_bf16 [B, M+T*L, C].  temporal may be NULL (if_use_temporal_embed = 0). */
+ * written into x_bf16 [B, M+T*L, C].  temporal may be NULL (if_use_temporal_embed = 0); added is read only when M > 1.
+ * Overwrites all of table_bf16 and ONLY the M global rows of each sequence of x_bf16 (its patch rows are left to the patch
+ * GEMM).  Each element is one fp32 sum then one bf16 rounding; the interpolation taps are those of F.interpolate(
+ * mode="linear", align_corners=False), the weight computed in fp32.  No alignment needs (scalar accesses). */
 int xp_vip_embed_tables(const float* pos, const float* temporal, const float* cls, const float* added,
                         void* table_bf16, void* x_bf16, int32_t B, int32_t T, int32_t L, int32_t M, int32_t C,
                         int32_t temporal_size, void* stream);
 /* Backward of the above: d_patch bf16 [B, T*L, C] and d_global bf16 [B, M, C] (the two compact halves of
- * d_embeddings) accumulated (fp32) into the four parameter gradients. */
+ * d_embeddings) ACCUMULATED (+=, fp32 atomics) into the parameter gradients: d_pos is required; d_temporal, d_cls and
+ * d_added are optional (NULL = not wanted).  The atomics make the result bits depend on scheduling: not bitwise
+ * repeatable.  C % 8 == 0 and C <= 1024; d_patch_bf16 / d_global_bf16 16-byte aligned (16-byte loads).  Refusals happen
+ * before any launch. */
 int xp_vip_embed_bwd(const void* d_patch_bf16, const void* d_global_bf16, float* d_pos, float* d_temporal, float* d_cls,
                      float* d_added, int32_t B, int32_t T, int32_t L, int32_t M, int32_t C, int32_t temporal_size,
                      void* stream);
 /* CLIPTextEmbeddings.forward (CLIP_ViP.py:222-225): x[r] = token_embedding[ids[r]] + position_embedding[r % Lt].
- * ids are int64 and indexed bit-exactly; *err_flag is set to 1 if any id is outside [0, vocab). */
+ * ids are int64 and indexed bit-exactly; *err_flag is set to 1 if any id is outside [0, vocab) (that row then uses id 0).
+ * Overwrites the rows x C block of x_bf16; each element is one fp32 sum then one bf16 rounding.  C % 4 == 0; tok and pos
+ * 16-byte aligned (float4 loads), x_bf16 8-byte aligned (8-byte stores).
+ * xp_text_embed_bwd ACCUMULATES (+=, fp32 atomics, not bitwise repeatable) dx into d_tok[ids[r]] and d_pos[r % Lt] (either
+ * may be NULL); rows with an out-of-range id are skipped.  Scalar accesses, no alignment needs. */
 int xp_text_embed_fwd(const int64_t* ids, const float* tok, const float* pos, void* x_bf16, int32_t rows, int32_t Lt,
                       int32_t C, int32_t vocab, int32_t* err_flag, void* stream);
 int xp_text_embed_bwd(const int64_t* ids, const void* dx_bf16, float* d_tok, float* d_pos, int32_t rows, int32_t Lt,
                       int32_t C, int32_t vocab, void* stream);
-/* EOS pooling row (CLIP_ViP.py:776): offsets[b] = (b*Lt + first argmax_s ids[b,s]) * C; index[b] optional. */
+/* EOS pooling row (CLIP_ViP.py:776): offsets[b] = (b*Lt + first argmax_s ids[b,s]) * C; index[b] optional.  Overwrites
+ * B entries of each; exact. */
 int xp_eos_offsets(const int64_t* ids, int64_t* offsets, int32_t* index, int32_t B, int32_t Lt, int32_t C,
                    void* stream);
 
@@ -341,7 +356,10 @@ int xp_dense_attention_bwd(const void* qkv, const void* out, const void* dout, c
 /* Token assembly, TimeSformer.forward timesformer.py:481-509: x [B,T,C,H*W] (XP_DTYPE_*) -> tokens bf16 [(b, p, t), C]
  * (rows in the reference's (h w t) order) = x[b,t,:,p] + pos[p,:] + time[t,:]; pos [H*W, C] / time [T, C] fp32 are the
  * (already interpolated) tables, NULL = no table (plain tokenisation, used for the output gradient).
- * xp_tsf_untokenize is the inverse layout change (tokens -> [B,T,C,H*W]): the module output (:523) and d(x). */
+ * xp_tsf_untokenize is the inverse layout change (tokens -> [B,T,C,H*W]): the module output (:523) and d(x).
+ * Both overwrite exactly their B*T*C*HW output elements.  Forward: (x + pos) + time in fp32, one bf16 rounding; untokenize:
+ * one conversion bf16 -> x_dtype (exact for fp32).  Scalar accesses, no alignment needs; B*T <= 65535 (grid z), refused
+ * before any launch otherwise. */
 int xp_tsf_embed_fwd(const void* x, int32_t x_dtype, const float* pos, const float* time, void* tokens_bf16, int32_t B,
                      int32_t T, int32_t C, int32_t HW, void* stream);
 int xp_tsf_untokenize(const void* tokens_bf16, void* x, int32_t x_dtype, int32_t B, int32_t T, int32_t C, int32_t HW,
@@ -386,9 +404,17 @@ int xp_rank_counts(const float* sim, int32_t N, int64_t ld, int32_t transpose, i
  * block_map_dev: device array of n_blocks {tensor index, chunk index} int32 pairs; chunk c of a tensor covers elements
  *                [c * xp_opt_chunk_elems(), ...).  Built once per parameter set by the host.
  * xp_opt_grad_norm:  norm_out_dev[0] = 2-norm over every g in the table, norm_out_dev[1] = min(1, max_norm/(norm+1e-6))
- *                    (1 if max_norm <= 0); partial_dev is n_blocks floats of scratch.  Deterministic.
- * xp_opt_scale_grads: g *= norm_dev[1] in place (clip_grad_norm_ used on its own).
- * xp_opt_adamw_step:  the fused update; norm_dev (optional) = the pair above, its coefficient is applied to g on the fly. */
+ *                    (1 if max_norm <= 0); partial_dev is n_blocks floats of scratch.  Deterministic for a given
+ *                    table and block map: fixed-order fp32 sums per block, the block partials summed in double in
+ *                    block-map order.  Reads g only.
+ * xp_opt_scale_grads: g *= norm_dev[1] in place (clip_grad_norm_ used on its own); leaves g untouched when the
+ *                    coefficient is >= 1.
+ * xp_opt_adamw_step:  the fused update; norm_dev (optional) = the pair above, its coefficient is applied to g on the fly.
+ *                    Overwrites the n elements of p, m, v (and p_bf16 when set) of every row, nothing else; reads g.
+ * Alignment: none required.  Each chunk uses 16-byte vectors when all of its row's pointers allow it (p_bf16: 8 bytes)
+ * and a scalar loop otherwise; the step, the scaling and the cast compute the same bits on both paths (the norm's fp32
+ * summation order differs between them, within its rounding bound).  Refused before any launch: an empty block map, betas
+ * outside [0, 1), eps < 0. */
 typedef struct XpOptTensor {
   void* p;
   const void* g;
@@ -409,7 +435,8 @@ int xp_opt_adamw_step(const XpOptTensor* table_dev, const int32_t* block_map_dev
                       float beta1, float beta2, float eps, void* stream);
 /* Multi-tensor refresh of the bf16 compute copies (replaces the reference's implicit "the module reads its own fp32
  * parameters", CLIP_ViP.py:445-460): per row, g = fp32 source, p_bf16 = bf16 destination, or if that is null p = fp32
- * destination (plain copy); n elements.  One launch for all weights of a tower, run on every forward. */
+ * destination (plain copy); n elements.  One launch for all weights of a tower, run on every forward.  Overwrites exactly
+ * the n destination elements per row; bit-exact (round to nearest even, or a copy).  No alignment needs. */
 int xp_cast_table(const XpOptTensor* table_dev, const int32_t* block_map_dev, int32_t n_blocks, void* stream);
 
 #ifdef __cplusplus

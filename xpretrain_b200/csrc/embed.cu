@@ -215,10 +215,11 @@ vip_embed_bwd_kernel(const __nv_bfloat16* __restrict__ d_patch, const __nv_bfloa
     for (int i = 0; i < 8; ++i) acc[i] += v[i];
   }
   if (j < M) {
-    float* dst = (j == 0) ? d_cls : d_added + static_cast<long long>(j - 1) * C;
+    // d_cls / d_added are optional like d_temporal: a caller without that gradient passes NULL
+    float* dst = (j == 0) ? d_cls : (d_added != nullptr ? d_added + static_cast<long long>(j - 1) * C : nullptr);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      atomicAdd(dst + c0 + i, acc[i]);
+      if (dst != nullptr) atomicAdd(dst + c0 + i, acc[i]);
       atomicAdd(d_pos + c0 + i, acc[i]);
     }
   } else {
@@ -309,10 +310,15 @@ eos_offsets_kernel(const long long* __restrict__ ids, long long* __restrict__ of
 
 using namespace xp;
 
+static bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 extern "C" int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_t frames, int32_t H,
                                int32_t W, int32_t patch, void* stream) {
   XP_ENTER(video);
   if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify: patch must divide H and W");
+  // every path stores the patch matrix in 16-byte vectors; the p % 8 == 0 path also loads the video in 16-byte vectors
+  if (!aligned_to(patches_bf16, 16)) return fail("xp_vip_patchify: patches must be 16-byte aligned");
+  if (patch % 8 == 0 && !aligned_to(video, 16)) return fail("xp_vip_patchify: video must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   __nv_bfloat16* out = static_cast<__nv_bfloat16*>(patches_bf16);
   if (patch % 8) {
@@ -352,6 +358,7 @@ extern "C" int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16,
                                   int32_t patch, const float* mean3, const float* std3, void* stream) {
   XP_ENTER(frames_hwc);
   if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify_u8: patch must divide H and W");
+  if (!aligned_to(patches_bf16, 16)) return fail("xp_vip_patchify_u8: patches must be 16-byte aligned");
   if (patch % 8) {
     const long long total = frames * (H / patch) * (W / patch) * (((3 * patch * patch + 7) & ~7) / 8);
     if (total <= 0) return 0;
@@ -389,6 +396,9 @@ extern "C" int xp_vip_embed_bwd(const void* d_patch_bf16, const void* d_global_b
                                 int32_t temporal_size, void* stream) {
   XP_ENTER(d_patch_bf16);
   if (C % 8 || C > 1024) return fail("xp_vip_embed_bwd: C must be a multiple of 8 and <= 1024");
+  if (d_pos == nullptr) return fail("xp_vip_embed_bwd: d_pos is required");
+  if (!aligned_to(d_patch_bf16, 16) || !aligned_to(d_global_bf16, 16))
+    return fail("xp_vip_embed_bwd: d_patch and d_global must be 16-byte aligned");
   const long long S = static_cast<long long>(M) + static_cast<long long>(T) * L;
   vip_embed_bwd_kernel<<<static_cast<unsigned>(S), 128, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(d_patch_bf16), static_cast<const __nv_bfloat16*>(d_global_bf16), d_pos,
@@ -401,6 +411,8 @@ extern "C" int xp_text_embed_fwd(const int64_t* ids, const float* tok, const flo
                                  int32_t Lt, int32_t C, int32_t vocab, int32_t* err_flag, void* stream) {
   XP_ENTER(ids);
   if (C % 4) return fail("xp_text_embed_fwd: C must be a multiple of 4");
+  if (!aligned_to(tok, 16) || !aligned_to(pos, 16)) return fail("xp_text_embed_fwd: tok and pos must be 16-byte aligned");
+  if (!aligned_to(x_bf16, 8)) return fail("xp_text_embed_fwd: x must be 8-byte aligned");
   if (rows <= 0) return 0;
   text_embed_fwd_kernel<<<rows, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(ids), tok, pos, static_cast<__nv_bfloat16*>(x_bf16), Lt, C, vocab, err_flag);

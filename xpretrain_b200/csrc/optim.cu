@@ -74,7 +74,8 @@ opt_norm_finalize_kernel(const float* __restrict__ partial, int n, float max_nor
     const float total = static_cast<float>(sqrt(s));
     norm_out[0] = total;
     const float coef = max_norm > 0.f ? __fdiv_rn(max_norm, total + 1e-6f) : 1.f;
-    norm_out[1] = coef < 1.f ? coef : 1.f;
+    // clamp(coef, max=1) as clip_grad_norm_ does it: a NaN norm gives a NaN coefficient, which then reaches every gradient
+    norm_out[1] = coef > 1.f ? 1.f : coef;
   }
 }
 

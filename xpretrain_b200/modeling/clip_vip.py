@@ -411,14 +411,24 @@ def _pooled_ln(x, pend, rmap, ln, B: int, C_: int, eps: float):
 
 def _colsum(x: torch.Tensor, out: torch.Tensor, aux) -> None:
     """Bias gradient = column sum of x (HBM-bound).  With an auxiliary stream it runs UNDER the tensor-bound GEMMs that follow
-    (its 256-thread CTAs co-reside with the persistent GEMM CTAs); the caller joins the stream before the gradients are used."""
+    (its 256-thread CTAs co-reside with the persistent GEMM CTAs); the caller joins the stream before the gradients are used.
+    The caller drops x only after that join (_join_aux), so that x's memory returns to the current stream's pool in stream
+    order behind the column sum.  (`x.record_stream(aux)` would defer the reuse until the allocator sees the aux event
+    complete: with the host running ahead of the GPU, each layer's dpre / dqkv blocks then stayed unusable, the pool grew to
+    the whole card and allocation retries — cudaFree of every cached block plus a device synchronise — made the step time
+    vary by tens of percent.)"""
     if aux is None:
         ops.colsum(x, out)
         return
     aux.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(aux):
         ops.colsum(x, out)
-    x.record_stream(aux)
+
+
+def _join_aux(aux) -> None:
+    """The current stream waits for the work queued on aux so far (a device-side wait, no host synchronise)."""
+    if aux is not None:
+        torch.cuda.current_stream().wait_stream(aux)
 
 
 def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch.Tensor], prefix: str, attn_bwd,
@@ -437,6 +447,7 @@ def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch
     ops.linear_wgrad(dpre, h2, g("mlp.fc1.weight"))
     dh2 = torch.empty(rows, C_, dtype=bf16, device=dev)
     ops.linear_dgrad(dpre, pk.w1[i], dh2)
+    _join_aux(aux)          # dpre's column sum is complete: its memory may return to this stream's pool (see _colsum)
     del dpre
     dx1 = torch.empty(rows, C_, dtype=bf16, device=dev)
     # LN2 backward streams dx as the residual-branch gradient: its column sum (= fc2.bias gradient) comes out of the same pass
@@ -454,12 +465,11 @@ def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch
     ops.linear_wgrad(dqkv, h, dwqkv)
     dh = da
     ops.linear_dgrad(dqkv, pk.wqkv[i], dh)
+    _join_aux(aux)          # the qkv bias gradient is complete, and dqkv may be released
     del dqkv
     dxin = torch.empty(rows, C_, dtype=bf16, device=dev)
     ops.layernorm_bwd(dh, plain, x, plain, layer.layer_norm1.weight, mean1, rstd1, dx1, plain, dxin, plain,
                       g("layer_norm1.weight"), g("layer_norm1.bias"), rows, C_, dres_colsum=g("self_attn.out_proj.bias"))
-    if aux is not None:
-        torch.cuda.current_stream().wait_stream(aux)      # this layer's bias gradients are complete
     return dxin
 
 

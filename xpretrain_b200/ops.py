@@ -209,7 +209,24 @@ def patch_pitch(patch: int) -> int:
     return (3 * patch * patch + 7) // 8 * 8
 
 
+def _aligned_input(x: torch.Tensor, nbytes: int = 16) -> torch.Tensor:
+    """x contiguous with an nbytes-aligned data pointer: the embedding kernels read their inputs in vectors, and a contiguous
+    view (e.g. `video[:, 1:]` of a one-frame-longer buffer, or an offset slice of a flat buffer) need not start aligned.
+    A misaligned input is copied; the kernel computes the same bits from the copy."""
+    x = x.contiguous()
+    return x if x.data_ptr() % nbytes == 0 else x.clone()
+
+
+def _aligned_output(x: torch.Tensor, nbytes: int, what: str) -> None:
+    """Outputs are written in place, so a misaligned one cannot be copied: it is refused before any launch."""
+    if x.data_ptr() % nbytes != 0:
+        raise _lib.XpError(f"{what}: the output must be {nbytes}-byte aligned (got data_ptr % {nbytes} = "
+                           f"{x.data_ptr() % nbytes})")
+
+
 def vip_patchify(video: torch.Tensor, patches: torch.Tensor, patch: int):
+    _aligned_output(patches, 16, "vip_patchify")
+    video = _aligned_input(video)
     frames = video.numel() // (3 * video.shape[-2] * video.shape[-1])
     check(lib().xp_vip_patchify(_p(video), _DT[video.dtype], _p(patches), frames, video.shape[-2], video.shape[-1], patch,
                                 _stream()), "xp_vip_patchify")
@@ -221,6 +238,8 @@ CLIP_MEAN, CLIP_STD = (0.48145466, 0.4578275, 0.40821073), (0.26862954, 0.261302
 def vip_patchify_u8(frames_hwc: torch.Tensor, patches: torch.Tensor, patch: int, mean=CLIP_MEAN, std=CLIP_STD):
     """frames_hwc uint8 [..., H, W, 3] -> normalised bf16 patch matrix (the reference's /255 + Normalize fused in)."""
     assert frames_hwc.dtype == torch.uint8 and frames_hwc.is_contiguous() and frames_hwc.shape[-1] == 3
+    _aligned_output(patches, 16, "vip_patchify_u8")
+    frames_hwc = _aligned_input(frames_hwc, 8)
     H, W = frames_hwc.shape[-3], frames_hwc.shape[-2]
     n = frames_hwc.numel() // (3 * H * W)
     m3, s3 = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
@@ -233,11 +252,16 @@ def vip_embed_tables(pos, temporal, cls, added, table, x, B, T, L, M, C_, tempor
 
 
 def vip_embed_bwd(d_patch, d_global, d_pos, d_temporal, d_cls, d_added, B, T, L, M, C_, temporal_size):
+    """Adds (fp32 atomics: not bitwise repeatable) the embedding gradients into d_pos and the optional d_temporal, d_cls,
+    d_added (None = not wanted)."""
+    d_patch, d_global = _aligned_input(d_patch), _aligned_input(d_global)
     check(lib().xp_vip_embed_bwd(_p(d_patch), _p(d_global), _p(d_pos), _p(d_temporal), _p(d_cls), _p(d_added), B, T, L, M,
                                  C_, temporal_size, _stream()), "xp_vip_embed_bwd")
 
 
 def text_embed_fwd(ids, tok, pos, x, Lt, err_flag):
+    _aligned_output(x, 8, "text_embed_fwd")
+    tok, pos = _aligned_input(tok), _aligned_input(pos)
     rows = ids.numel()
     check(lib().xp_text_embed_fwd(_p(ids), _p(tok), _p(pos), _p(x), rows, Lt, tok.shape[1], tok.shape[0], _p(err_flag),
                                   _stream()), "xp_text_embed_fwd")
