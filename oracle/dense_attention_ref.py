@@ -2,8 +2,8 @@
 
 Same conventions as oracle/attention_ref.py, whose `sdpa` it uses: the kernel's own operands (fused token-major qkv with q
 pre-scaled by head_dim**-0.5, the output gradient), float64 results, `q_scale` applied to dq.  With `arm="dense"` the
-computation rounds to bf16 where the kernel does: P·V with P = hi + lo (dense_attention.cu forward, as vip_attention_long.cu),
-P and dS rounded as MMA operands in the backward, delta from the bf16 O and dO, outputs rounded once.
+computation rounds to bf16 where the kernel does: P·V with P = hi + lo (fwd_step of attn_wgmma.cuh, shared with the ViP
+kernels), P and dS rounded as MMA operands in the backward, delta from the bf16 O and dO, outputs rounded once.
 
   dense_ref   n_seq sequences of seq_len consecutive rows; every row attends to every row of its own sequence
               ('joint_space_time': one clip of H*W*T tokens, timesformer.py:202-205; 'space_only': one frame)

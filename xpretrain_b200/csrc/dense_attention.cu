@@ -3,16 +3,9 @@
 // timesformer.py:156-173, on x of shape [B, H*W*T, C] or [B*T, H*W, C], :202-205).  See xp_dense_attention_* in
 // include/xpretrain_b200.h for the ABI.
 //
-// Hopper path, FlashAttention-3 shaped, like vip_attention_long.cu: a CTA of three warpgroups per two 64-row tiles of
-// one (sequence, head).  Warpgroup 0 is the producer (setmaxnreg down to 40): one thread streams 64-row blocks by TMA
-// into 128B-swizzled shared memory through an LSTAGES-deep full / empty mbarrier ring.  Warpgroups 1 and 2 are consumers
-// (setmaxnreg up to 232), each owning one tile, with every product on wgmma:
-//   forward    query-stationary: S = Q·Kᵀ, online softmax over the 64-key blocks in registers, O += P·V with P in
-//              registers, split into bf16 hi + lo (rounding P is the largest error of a plain bf16 P·V);
-//   backward   delta = rowsum(dO * O) by a small kernel, then
-//              key-stationary kernel: Sᵀ = K·Qᵀ and dPᵀ = V·dOᵀ per streamed query block, dV += Pᵀ·dO, dK += dSᵀ·Q;
-//              the producer warpgroup also loads each block's LSE and delta;
-//              query-stationary kernel: S = Q·Kᵀ and dP = dO·Vᵀ per streamed key block, dQ += dS·K.
+// Runs the streamed pipeline of attn_wgmma.cuh with a three-stage ring, one CTA per two 64-row tiles of one (sequence,
+// head).  delta = rowsum(dO * O) is computed by a small kernel ahead of the two backward kernels, whose producer warpgroup
+// loads it with the LSE.
 //
 // Sequences are ragged against the 64-row tiles (392, 1120 and 6272 rows are not multiples of 64), and the next sequence
 // sits directly behind the last one.  Every tile is loaded through a 3-D tensor map {columns, seq_len, n_seq}: box rows
@@ -24,197 +17,93 @@
 
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
-#include "ptx.cuh"
-#include "mma_frag.cuh"
+#include "attn_wgmma.cuh"
 
 namespace xp {
 
 namespace {
-
-constexpr int DTILE = 64;                   // rows per tile / streamed block
-constexpr int DTILE_BYTES = DTILE * 128;    // one [64][64] bf16 tile, 128B-swizzled
-constexpr int DENSE_THREADS = 384;          // producer warpgroup + two consumer warpgroups
-constexpr int DSTAGES = 3;                  // ring depth of the streamed blocks
 
 struct DenseDims {
   long long n_rows, ld_qkv, ld_o;
   int H, n_seq, L, C;
 };
 
-__device__ __forceinline__ uint64_t kdesc(uint32_t addr) { return make_smem_desc_sw128(addr, 16, 1024); }     // K-major
-__device__ __forceinline__ uint64_t mndesc(uint32_t addr) { return make_smem_desc_sw128(addr, 8192, 1024); }  // MN-major
+// Layout of a CTA of grid (ceil(ntiles / 2), H, n_seq): the 64-row tiles of sequence blockIdx.z.
+struct Dense {
+  static constexpr int STAGES = 3;
+  static constexpr bool ZERO_FILL = true;   // 3-D tensor map: box rows past the sequence end read as zero
+  DenseDims d;
 
-__device__ __forceinline__ int num_tiles(const DenseDims& d) { return (d.L + DTILE - 1) / DTILE; }
-__device__ __forceinline__ int live_rows(const DenseDims& d, int j) { return min(DTILE, d.L - j * DTILE); }
-
-__device__ __forceinline__ void acc_to_afrag(const float (&x)[32], uint32_t (&a)[4][4]) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = pack_bf16(x[8 * ks + 0], x[8 * ks + 1]);
-    a[ks][1] = pack_bf16(x[8 * ks + 2], x[8 * ks + 3]);
-    a[ks][2] = pack_bf16(x[8 * ks + 4], x[8 * ks + 5]);
-    a[ks][3] = pack_bf16(x[8 * ks + 6], x[8 * ks + 7]);
+  __device__ void bind() {}
+  __device__ int h() const { return blockIdx.y; }
+  __device__ long long row0() const { return static_cast<long long>(blockIdx.z) * d.L; }   // first row of the sequence
+  __device__ int ntiles() const { return (d.L + ATILE - 1) / ATILE; }
+  __device__ int rows(int j) const { return min(ATILE, d.L - j * ATILE); }
+  __device__ bool skip(int, int) const { return false; }
+  __device__ void load(void* dst, const CUtensorMap* tm, uint64_t* bar, int m, int j) const {
+    tma_load_3d(dst, tm, bar, m * d.C + h() * HD, j * ATILE, blockIdx.z);
   }
-}
-
-// Barrier set-up of the ring; `full_count` arrivals complete a fill, every live consumer warp releases a stage.
-__device__ __forceinline__ void init_ring(uint64_t* q_full, uint64_t* full, uint64_t* empty, uint32_t full_count,
-                                          int nlive, const CUtensorMap* tm0, const CUtensorMap* tm1) {
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(tm0);
-    tma_prefetch_desc(tm1);
-    mbar_init(q_full, 1);
-#pragma unroll
-    for (int s = 0; s < DSTAGES; ++s) {
-      mbar_init(&full[s], full_count);
-      mbar_init(&empty[s], 4 * nlive);
-    }
-    fence_barrier_init();
+  __device__ __nv_bfloat16* row(__nv_bfloat16* base, long long ld, int j, int i) const {
+    return base + (row0() + j * ATILE + i) * ld + h() * HD + (threadIdx.x & 3) * 2;
   }
-  __syncthreads();
-}
-__device__ __forceinline__ void release_stage(uint64_t* empty, int s) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[s]);
-}
+};
 
-}  // namespace
+struct DenseFwd : Dense {
+  __nv_bfloat16* out;
+  float* lse;
 
-// ======================================================================== forward
-// grid (ceil(ntiles / 2), H, n_seq); consumer c of CTA x owns query tile 2x + c.  Shared memory: the two Q tiles, then
-// DSTAGES x {K, V}.
-__global__ void __launch_bounds__(DENSE_THREADS, 1)
-dense_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restrict__ out, float* __restrict__ lse,
-                 const DenseDims d) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = smem_raw + (((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw));
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(sm + (2 + 2 * DSTAGES) * DTILE_BYTES);
-  uint64_t* full = q_full + 1;
-  uint64_t* empty = full + DSTAGES;
-  const int h = blockIdx.y, seq = blockIdx.z;
-  const int ntiles = num_tiles(d);
-  const int qt0 = 2 * blockIdx.x;
-  const int nlive = min(2, ntiles - qt0);
-  const int wg = threadIdx.x >> 7;
-  init_ring(q_full, full, empty, 1, nlive, &tm, &tm);
-
-  if (wg == 0) {
-    // ------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(q_full, nlive * DTILE_BYTES);
-      for (int c = 0; c < nlive; ++c) tma_load_3d(sm + c * DTILE_BYTES, &tm, q_full, h * HD, (qt0 + c) * DTILE, seq);
-      for (int kb = 0; kb < ntiles; ++kb) {
-        const int s = kb % DSTAGES;
-        mbar_wait_nocall(&empty[s], ((kb / DSTAGES) & 1) ^ 1);
-        uint8_t* st = sm + (2 + 2 * s) * DTILE_BYTES;
-        mbar_arrive_expect_tx(&full[s], 2 * DTILE_BYTES);
-        tma_load_3d(st, &tm, &full[s], d.C + h * HD, kb * DTILE, seq);
-        tma_load_3d(st + DTILE_BYTES, &tm, &full[s], 2 * d.C + h * HD, kb * DTILE, seq);
-      }
-    }
-    return;
+  __device__ void store_fwd(int qt, int i, int r, const float (&o)[32], float m, float l) const {
+    const float inv = 1.f / l;   // > 0: every query sees at least one key
+    __nv_bfloat16* dst = row(out, d.ld_o, qt, i);
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      *reinterpret_cast<uint32_t*>(dst + k * 8) = pack_bf16(o[4 * k + 2 * r] * inv, o[4 * k + 2 * r + 1] * inv);
+    if ((threadIdx.x & 3) == 0) lse[static_cast<long long>(h()) * d.n_rows + row0() + qt * ATILE + i] = m + logf(l);
   }
-  // -------------------------------------------------------- consumers
-  setmaxnreg_inc<232>();
-  const int c = wg - 1, qt = qt0 + c;
-  if (c >= nlive) return;
-  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int r_lo = wq * 16 + (lane >> 2);
-  const uint32_t sQ = smem_u32(sm) + c * DTILE_BYTES;
-  float o[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  mbar_wait_nocall(q_full, 0);
-#pragma unroll 1
-  for (int kb = 0; kb < ntiles; ++kb) {
-    const int s = kb % DSTAGES;
-    const int klim = live_rows(d, kb);
-    mbar_wait_nocall(&full[s], (kb / DSTAGES) & 1);
-    const uint32_t sK = smem_u32(sm) + (2 + 2 * s) * DTILE_BYTES, sV = sK + DTILE_BYTES;
-    float sc[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
-    wgmma_fence_regs(sc);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_ss<0, 0>(sc, kdesc(sQ + ks * 32), kdesc(sK + ks * 32));
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sc);
-    if (klim < DTILE) {   // the last block of a ragged sequence: keys past the end (zero-filled rows) get no weight
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          if (i * 8 + (lane & 3) * 2 + (e & 1) >= klim) sc[4 * i + e] = -INFINITY;
-    }
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int i = 0; i < 32; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
-    float corr[2], mb[2];
+};
+
+struct DenseBwd : Dense {
+  const float* lse;
+  const float* delta;
+  __nv_bfloat16* dqkv;
+  float q_scale;
+
+  // threads 0-63: lse, 64-127: delta.  Rows past the end: lse = +inf gives P = 0 exactly (their Q and dO are
+  // zero-filled, so every product is finite)
+  __device__ void fill_stats(float* s, int qb) const {
+    const int i = threadIdx.x & 63, which = threadIdx.x >> 6;
+    const float* src = (which == 0 ? lse : delta) + static_cast<long long>(h()) * d.n_rows + row0();
+    const bool valid = i < rows(qb);
+    const float v = valid ? __ldg(src + qb * ATILE + i) : 0.f;
+    s[which * ATILE + i] = which == 0 ? (valid ? v * LOG2E : INFINITY) : v;
+  }
+  // +inf / 0 past the end: P = 0
+  __device__ void row_stats(int qt, int q_lo, float (&lse_r)[2], float (&del_r)[2]) const {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_run[r], mx[r]);
-      corr[r] = (m_new == -INFINITY) ? 1.f : fast_exp2((m_run[r] - m_new) * LOG2E);
-      l_run[r] *= corr[r];
-      m_run[r] = m_new;
-      mb[r] = m_new == -INFINITY ? 0.f : m_new * LOG2E;
+      const int i = q_lo + r * 8;
+      const long long at = static_cast<long long>(h()) * d.n_rows + row0() + qt * ATILE + i;
+      lse_r[r] = i < rows(qt) ? __ldg(lse + at) * LOG2E : INFINITY;
+      del_r[r] = i < rows(qt) ? __ldg(delta + at) : 0.f;
     }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      o[4 * i + 0] *= corr[0]; o[4 * i + 1] *= corr[0];
-      o[4 * i + 2] *= corr[1]; o[4 * i + 3] *= corr[1];
-    }
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const float pv = fast_exp2(fmaf(sc[i], LOG2E, -mb[(i >> 1) & 1]));   // exp2(-inf) = 0 for masked entries
-      sc[i] = pv;
-      l_run[(i >> 1) & 1] += pv;
-    }
-    // P·V with P = hi + lo in bf16
-    uint32_t ph[4][4], pl[4][4];
-    acc_to_afrag(sc, ph);
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        pl[ks][j] = pack_bf16(sc[8 * ks + 2 * j] - bf16_lo(ph[ks][j]), sc[8 * ks + 2 * j + 1] - bf16_hi(ph[ks][j]));
-    wgmma_fence_regs(o);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const uint64_t vd = mndesc(sV + ks * 16 * 128);
-      wgmma_m64n64k16_rs<1>(o, ph[ks], vd);
-      wgmma_m64n64k16_rs<1>(o, pl[ks], vd);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(o);
-    release_stage(empty, s);
   }
+  __device__ void store_kv(int kt, int key, int r, const float (&dk)[32], const float (&dv)[32]) const {
+    __nv_bfloat16* dst = row(dqkv, d.ld_qkv, kt, key);
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
-    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    for (int k = 0; k < 8; ++k) {
+      *reinterpret_cast<uint32_t*>(dst + d.C + k * 8) = pack_bf16(dk[4 * k + 2 * r], dk[4 * k + 2 * r + 1]);
+      *reinterpret_cast<uint32_t*>(dst + 2 * d.C + k * 8) = pack_bf16(dv[4 * k + 2 * r], dv[4 * k + 2 * r + 1]);
+    }
   }
-  const int qrows = live_rows(d, qt);
+  __device__ void store_q(int qt, int q, int r, const float (&dq)[32]) const {
+    __nv_bfloat16* dst = row(dqkv, d.ld_qkv, qt, q);
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int row = r_lo + r * 8;
-    if (row >= qrows) continue;
-    const long long grow = static_cast<long long>(seq) * d.L + qt * DTILE + row;
-    const float inv = 1.f / l_run[r];   // > 0: every query sees at least one key
-    __nv_bfloat16* dst = out + grow * d.ld_o + h * HD + (lane & 3) * 2;
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      *reinterpret_cast<uint32_t*>(dst + i * 8) = pack_bf16(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
-    if ((lane & 3) == 0) lse[static_cast<long long>(h) * d.n_rows + grow] = m_run[r] + logf(l_run[r]);
+    for (int k = 0; k < 8; ++k)
+      *reinterpret_cast<uint32_t*>(dst + k * 8) = pack_bf16(dq[4 * k + 2 * r] * q_scale, dq[4 * k + 2 * r + 1] * q_scale);
   }
-}
+};
+
+}  // namespace
 
 // ============================================================ backward: delta = rowsum(dO * O)
 // Eight threads per (row, head), 8 columns each, summed in a fixed shuffle order.  grid-stride over n_seq * L * H rows.
@@ -244,246 +133,10 @@ dense_delta_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* _
   }
 }
 
-// ============================================================ backward, key-stationary -> dK, dV
-// grid (ceil(ntiles / 2), H, n_seq); consumer c owns key tile 2x + c.  Shared memory: {K, V} of each consumer, then
-// DSTAGES x {Q, dO}, then DSTAGES x {lse * log2(e), delta} of the streamed query block.  A fill completes when the TMA
-// bytes have landed and all 128 producer threads have written the block's lse / delta.
-__global__ void __launch_bounds__(DENSE_THREADS, 1)
-dense_bwd_kv_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ CUtensorMap tdo,
-                    const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
-                    const DenseDims d) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = smem_raw + (((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw));
-  float* s_stat = reinterpret_cast<float*>(sm + (4 + 2 * DSTAGES) * DTILE_BYTES);   // [DSTAGES][2][64]
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(s_stat + DSTAGES * 2 * DTILE);
-  uint64_t* full = q_full + 1;
-  uint64_t* empty = full + DSTAGES;
-  const int h = blockIdx.y, seq = blockIdx.z;
-  const int ntiles = num_tiles(d);
-  const int kt0 = 2 * blockIdx.x;
-  const int nlive = min(2, ntiles - kt0);
-  const int wg = threadIdx.x >> 7;
-  init_ring(q_full, full, empty, 1 + 128, nlive, &tm, &tdo);
-  const long long row0 = static_cast<long long>(seq) * d.L;   // first row of the sequence
-
-  if (wg == 0) {
-    // ------------------------------------ producer: Q / dO by TMA, lse / delta by the whole warpgroup
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(q_full, nlive * 2 * DTILE_BYTES);
-      for (int c = 0; c < nlive; ++c) {
-        tma_load_3d(sm + 2 * c * DTILE_BYTES, &tm, q_full, d.C + h * HD, (kt0 + c) * DTILE, seq);
-        tma_load_3d(sm + (2 * c + 1) * DTILE_BYTES, &tm, q_full, 2 * d.C + h * HD, (kt0 + c) * DTILE, seq);
-      }
-    }
-    const int row = threadIdx.x & 63, which = threadIdx.x >> 6;   // threads 0-63: lse, 64-127: delta
-    const float* src = (which == 0 ? lse : delta) + static_cast<long long>(h) * d.n_rows + row0;
-    for (int qb = 0; qb < ntiles; ++qb) {
-      const int s = qb % DSTAGES;
-      mbar_wait(&empty[s], ((qb / DSTAGES) & 1) ^ 1);
-      if (threadIdx.x == 0) {
-        uint8_t* st = sm + (4 + 2 * s) * DTILE_BYTES;
-        mbar_arrive_expect_tx(&full[s], 2 * DTILE_BYTES);
-        tma_load_3d(st, &tm, &full[s], h * HD, qb * DTILE, seq);
-        tma_load_3d(st + DTILE_BYTES, &tdo, &full[s], h * HD, qb * DTILE, seq);
-      }
-      const bool valid = row < live_rows(d, qb);
-      // rows past the end: lse = +inf gives P = 0 exactly (their Q and dO are zero-filled, so every product is finite)
-      const float v = valid ? src[qb * DTILE + row] : 0.f;
-      s_stat[(s * 2 + which) * DTILE + row] = which == 0 ? (valid ? v * LOG2E : INFINITY) : v;
-      mbar_arrive(&full[s]);
-    }
-    return;
-  }
-  // -------------------------------------------------------- consumers
-  setmaxnreg_inc<232>();
-  const int c = wg - 1, kt = kt0 + c;
-  if (c >= nlive) return;
-  const int krows = live_rows(d, kt);
-  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int k_lo = wq * 16 + (lane >> 2);
-  const uint32_t sK = smem_u32(sm) + 2 * c * DTILE_BYTES, sV = sK + DTILE_BYTES;
-  float dk[32], dv[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) dk[i] = dv[i] = 0.f;
-  mbar_wait_nocall(q_full, 0);
-#pragma unroll 1
-  for (int qb = 0; qb < ntiles; ++qb) {
-    const int s = qb % DSTAGES;
-    mbar_wait_nocall(&full[s], (qb / DSTAGES) & 1);
-    const uint32_t sQ = smem_u32(sm) + (4 + 2 * s) * DTILE_BYTES, sdO = sQ + DTILE_BYTES;
-    const float* s_lse = s_stat + (s * 2) * DTILE;
-    const float* s_delta = s_lse + DTILE;
-    float st[32], dpt[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
-    wgmma_fence_regs(st);
-    wgmma_fence_regs(dpt);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      wgmma_m64n64k16_ss<0, 0>(st, kdesc(sK + ks * 32), kdesc(sQ + ks * 32));
-      wgmma_m64n64k16_ss<0, 0>(dpt, kdesc(sV + ks * 32), kdesc(sdO + ks * 32));
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(st);
-    wgmma_fence_regs(dpt);
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int q = i * 8 + (lane & 3) * 2 + (e & 1);
-        const float p = fast_exp2(fmaf(st[4 * i + e], LOG2E, -s_lse[q]));
-        st[4 * i + e] = p;
-        dpt[4 * i + e] = p * (dpt[4 * i + e] - s_delta[q]);
-      }
-    uint32_t ap[4][4], ad[4][4];
-    acc_to_afrag(st, ap);
-    acc_to_afrag(dpt, ad);
-    wgmma_fence_regs(dv);
-    wgmma_fence_regs(dk);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      wgmma_m64n64k16_rs<1>(dv, ap[ks], mndesc(sdO + ks * 16 * 128));
-      wgmma_m64n64k16_rs<1>(dk, ad[ks], mndesc(sQ + ks * 16 * 128));
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(dv);
-    wgmma_fence_regs(dk);
-    release_stage(empty, s);
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int key = k_lo + r * 8;
-    if (key >= krows) continue;
-    __nv_bfloat16* row = dqkv + (row0 + kt * DTILE + key) * d.ld_qkv + h * HD + (lane & 3) * 2;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      *reinterpret_cast<uint32_t*>(row + d.C + i * 8) = pack_bf16(dk[4 * i + 2 * r], dk[4 * i + 2 * r + 1]);
-      *reinterpret_cast<uint32_t*>(row + 2 * d.C + i * 8) = pack_bf16(dv[4 * i + 2 * r], dv[4 * i + 2 * r + 1]);
-    }
-  }
-}
-
-// ============================================================ backward, query-stationary -> dQ
-// grid (ceil(ntiles / 2), H, n_seq); consumer c owns query tile 2x + c.  Shared memory: {Q, dO} of each consumer, then
-// DSTAGES x {K, V}.
-__global__ void __launch_bounds__(DENSE_THREADS, 1)
-dense_bwd_q_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ CUtensorMap tdo,
-                   const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
-                   const DenseDims d, float q_scale) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = smem_raw + (((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw));
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(sm + (4 + 2 * DSTAGES) * DTILE_BYTES);
-  uint64_t* full = q_full + 1;
-  uint64_t* empty = full + DSTAGES;
-  const int h = blockIdx.y, seq = blockIdx.z;
-  const int ntiles = num_tiles(d);
-  const int qt0 = 2 * blockIdx.x;
-  const int nlive = min(2, ntiles - qt0);
-  const int wg = threadIdx.x >> 7;
-  init_ring(q_full, full, empty, 1, nlive, &tm, &tdo);
-  const long long row0 = static_cast<long long>(seq) * d.L;
-
-  if (wg == 0) {
-    // ------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(q_full, nlive * 2 * DTILE_BYTES);
-      for (int c = 0; c < nlive; ++c) {
-        tma_load_3d(sm + 2 * c * DTILE_BYTES, &tm, q_full, h * HD, (qt0 + c) * DTILE, seq);
-        tma_load_3d(sm + (2 * c + 1) * DTILE_BYTES, &tdo, q_full, h * HD, (qt0 + c) * DTILE, seq);
-      }
-      for (int kb = 0; kb < ntiles; ++kb) {
-        const int s = kb % DSTAGES;
-        mbar_wait_nocall(&empty[s], ((kb / DSTAGES) & 1) ^ 1);
-        uint8_t* st = sm + (4 + 2 * s) * DTILE_BYTES;
-        mbar_arrive_expect_tx(&full[s], 2 * DTILE_BYTES);
-        tma_load_3d(st, &tm, &full[s], d.C + h * HD, kb * DTILE, seq);
-        tma_load_3d(st + DTILE_BYTES, &tm, &full[s], 2 * d.C + h * HD, kb * DTILE, seq);
-      }
-    }
-    return;
-  }
-  // -------------------------------------------------------- consumers
-  setmaxnreg_inc<232>();
-  const int c = wg - 1, qt = qt0 + c;
-  if (c >= nlive) return;
-  const int qrows = live_rows(d, qt);
-  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int q_lo = wq * 16 + (lane >> 2);
-  // lse * log2(e) and delta of this thread's two rows (+inf / 0 past the end: P = 0)
-  float lse_r[2], del_r[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int row = q_lo + r * 8;
-    const long long at = static_cast<long long>(h) * d.n_rows + row0 + qt * DTILE + row;
-    lse_r[r] = row < qrows ? lse[at] * LOG2E : INFINITY;
-    del_r[r] = row < qrows ? delta[at] : 0.f;
-  }
-  const uint32_t sQ = smem_u32(sm) + 2 * c * DTILE_BYTES, sdO = sQ + DTILE_BYTES;
-  float dq[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
-  mbar_wait_nocall(q_full, 0);
-#pragma unroll 1
-  for (int kb = 0; kb < ntiles; ++kb) {
-    const int s = kb % DSTAGES;
-    const int klim = live_rows(d, kb);
-    mbar_wait_nocall(&full[s], (kb / DSTAGES) & 1);
-    const uint32_t sK = smem_u32(sm) + (4 + 2 * s) * DTILE_BYTES, sV = sK + DTILE_BYTES;
-    float sc[32], dp[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) sc[i] = dp[i] = 0.f;
-    wgmma_fence_regs(sc);
-    wgmma_fence_regs(dp);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      wgmma_m64n64k16_ss<0, 0>(sc, kdesc(sQ + ks * 32), kdesc(sK + ks * 32));
-      wgmma_m64n64k16_ss<0, 0>(dp, kdesc(sdO + ks * 32), kdesc(sV + ks * 32));
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sc);
-    wgmma_fence_regs(dp);
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = i * 8 + (lane & 3) * 2 + (e & 1);
-        const float p = key < klim ? fast_exp2(fmaf(sc[4 * i + e], LOG2E, -lse_r[e >> 1])) : 0.f;
-        dp[4 * i + e] = p * (dp[4 * i + e] - del_r[e >> 1]);
-      }
-    uint32_t ad[4][4];
-    acc_to_afrag(dp, ad);
-    wgmma_fence_regs(dq);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs<1>(dq, ad[ks], mndesc(sK + ks * 16 * 128));
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(dq);
-    release_stage(empty, s);
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int q = q_lo + r * 8;
-    if (q >= qrows) continue;
-    __nv_bfloat16* row = dqkv + (row0 + qt * DTILE + q) * d.ld_qkv + h * HD + (lane & 3) * 2;
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      *reinterpret_cast<uint32_t*>(row + i * 8) = pack_bf16(dq[4 * i + 2 * r] * q_scale, dq[4 * i + 2 * r + 1] * q_scale);
-  }
-}
-
 namespace {
-constexpr int DENSE_FWD_SMEM = (2 + 2 * DSTAGES) * DTILE_BYTES + 1024 + 64;
-constexpr int DENSE_BWD_KV_SMEM = (4 + 2 * DSTAGES) * DTILE_BYTES + DSTAGES * 2 * DTILE * 4 + 1024 + 64;
-constexpr int DENSE_BWD_Q_SMEM = (4 + 2 * DSTAGES) * DTILE_BYTES + 1024 + 64;
+constexpr int DENSE_FWD_SMEM = stream_fwd_smem(Dense::STAGES);
+constexpr int DENSE_BWD_KV_SMEM = stream_kv_smem(Dense::STAGES);
+constexpr int DENSE_BWD_Q_SMEM = stream_q_smem(Dense::STAGES);
 
 int to_dims(const XpDenseAttn* a, DenseDims& d, const char* who) {
   if (a == nullptr) return fail(std::string(who) + ": null descriptor");
@@ -507,13 +160,13 @@ int to_dims(const XpDenseAttn* a, DenseDims& d, const char* who) {
 }
 
 dim3 dense_grid(const DenseDims& d) {
-  const int ntiles = (d.L + DTILE - 1) / DTILE;
+  const int ntiles = (d.L + ATILE - 1) / ATILE;
   return dim3((ntiles + 1) / 2, d.H, d.n_seq);
 }
 
 // {columns, seq_len, n_seq} view of a token-major [rows, ld] buffer: box rows past a sequence's end read as zero
 int seq_tmap(CUtensorMap* tm, const void* base, long long ld, const DenseDims& d) {
-  return make_tmap_bf16_3d(tm, base, ld, d.L, d.n_seq, ld, ld * d.L, HD, DTILE);
+  return make_tmap_bf16_3d(tm, base, ld, d.L, d.n_seq, ld, ld * d.L, HD, ATILE);
 }
 }  // namespace
 
@@ -529,11 +182,12 @@ extern "C" int xp_dense_attention_fwd(const void* qkv, void* out, float* lse, co
   if (seq_tmap(&tm, qkv, d.ld_qkv, d)) return -1;
   static bool attr = false;
   if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(dense_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_FWD_SMEM));
+    XP_CHECK_CUDA(
+        cudaFuncSetAttribute(stream_fwd_kernel<DenseFwd>, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_FWD_SMEM));
     attr = true;
   }
-  dense_fwd_kernel<<<dense_grid(d), DENSE_THREADS, DENSE_FWD_SMEM, static_cast<cudaStream_t>(stream)>>>(
-      tm, static_cast<__nv_bfloat16*>(out), lse, d);
+  const DenseFwd p{{d}, static_cast<__nv_bfloat16*>(out), lse};
+  stream_fwd_kernel<<<dense_grid(d), STREAM_THREADS, DENSE_FWD_SMEM, static_cast<cudaStream_t>(stream)>>>(tm, p);
   XP_CHECK_LAUNCH("dense_fwd_kernel");
   return 0;
 }
@@ -548,9 +202,10 @@ extern "C" int xp_dense_attention_bwd(const void* qkv, const void* out, const vo
   if (seq_tmap(&tm, qkv, d.ld_qkv, d) || seq_tmap(&tdo, dout, d.ld_o, d)) return -1;
   static bool attr = false;
   if (!attr) {
-    XP_CHECK_CUDA(
-        cudaFuncSetAttribute(dense_bwd_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_BWD_KV_SMEM));
-    XP_CHECK_CUDA(cudaFuncSetAttribute(dense_bwd_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_BWD_Q_SMEM));
+    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_kv_kernel<DenseBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       DENSE_BWD_KV_SMEM));
+    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_q_kernel<DenseBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       DENSE_BWD_Q_SMEM));
     attr = true;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -559,10 +214,10 @@ extern "C" int xp_dense_attention_bwd(const void* qkv, const void* out, const vo
   dense_delta_kernel<<<blocks, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(out),
                                              static_cast<const __nv_bfloat16*>(dout), delta, d);
   XP_CHECK_LAUNCH("dense_delta_kernel");
-  __nv_bfloat16* dx = static_cast<__nv_bfloat16*>(dqkv);
-  dense_bwd_kv_kernel<<<dense_grid(d), DENSE_THREADS, DENSE_BWD_KV_SMEM, st>>>(tm, tdo, lse, delta, dx, d);
+  const DenseBwd p{{d}, lse, delta, static_cast<__nv_bfloat16*>(dqkv), q_scale};
+  stream_bwd_kv_kernel<<<dense_grid(d), STREAM_THREADS, DENSE_BWD_KV_SMEM, st>>>(tm, tdo, p);
   XP_CHECK_LAUNCH("dense_bwd_kv_kernel");
-  dense_bwd_q_kernel<<<dense_grid(d), DENSE_THREADS, DENSE_BWD_Q_SMEM, st>>>(tm, tdo, lse, delta, dx, d, q_scale);
+  stream_bwd_q_kernel<<<dense_grid(d), STREAM_THREADS, DENSE_BWD_Q_SMEM, st>>>(tm, tdo, p);
   XP_CHECK_LAUNCH("dense_bwd_q_kernel");
   return 0;
 }

@@ -11,16 +11,12 @@
 //
 // Hopper path: one thread stages the operands by TMA (two boxes per matrix: the L frame rows into shared-memory rows
 // [0, L), the M global rows into rows [248, 248 + M), both 1024-byte aligned for the 128B swizzle; the rows between
-// are zero), completion on an mbarrier.  Two warpgroups each own 64-row tiles and run every product on wgmma:
-//   forward   S = Q·Kᵀ (both operands from shared memory), online softmax over 64-key blocks in registers, and
-//             O += P·V with P taken from registers as the A operand (split into bf16 hi + lo, see below);
-//   backward  pass A (key-stationary): Sᵀ = K·Qᵀ and dPᵀ = V·dOᵀ, then dV += Pᵀ·dO and dK += dSᵀ·Q with Pᵀ / dSᵀ in
-//             registers; pass B (query-stationary): S = Q·Kᵀ, dP = dO·Vᵀ, dQ += dS·K.  No operand is transposed in
-//             memory: V, dO, Q and K serve as MN-major B operands where the product contracts over their rows.
+// are zero), completion on an mbarrier.  Two warpgroups each own 64-row tiles and run the per-block steps of
+// attn_wgmma.cuh over the four staged tiles: forward fwd_step; backward pass A (key-stationary) kv_step, pass B
+// (query-stationary) q_step.
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
-#include "ptx.cuh"
-#include "mma_frag.cuh"
+#include "attn_wgmma.cuh"
 #include "vip_attention.h"
 
 namespace xp {
@@ -37,9 +33,6 @@ __device__ __forceinline__ bool row_global(int r) { return r >= GROW; }
 __device__ __forceinline__ int row_seq(int r, const AttnDims& d) { return r >= GROW ? r - GROW : d.M + r; }
 // a 64-row tile holds at least one token (tile 3 always holds the global rows)
 __device__ __forceinline__ bool tile_live(int k, const AttnDims& d) { return k == 3 || 64 * k < d.L; }
-
-__device__ __forceinline__ uint64_t kdesc(uint32_t addr) { return make_smem_desc_sw128(addr, 16, 1024); }     // K-major
-__device__ __forceinline__ uint64_t mndesc(uint32_t addr) { return make_smem_desc_sw128(addr, 8192, 1024); }  // MN-major
 
 // Zero the padding rows of NMAT matrices, then TMA the frame rows and global rows of each; every thread waits.
 template <int NMAT>
@@ -68,17 +61,6 @@ __device__ __forceinline__ void stage_rows(uint8_t* sm, uint64_t* bar, const CUt
   mbar_wait_nocall(bar, 0);
 }
 
-// P (or dS) of a 64 x 64 accumulator as the A fragments of the four k16 steps: k-step ks covers columns [16 ks, 16 ks + 16)
-__device__ __forceinline__ void acc_to_afrag(const float (&x)[32], uint32_t (&a)[4][4]) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = pack_bf16(x[8 * ks + 0], x[8 * ks + 1]);
-    a[ks][1] = pack_bf16(x[8 * ks + 2], x[8 * ks + 3]);
-    a[ks][2] = pack_bf16(x[8 * ks + 4], x[8 * ks + 5]);
-    a[ks][3] = pack_bf16(x[8 * ks + 6], x[8 * ks + 7]);
-  }
-}
-
 // ======================================================================== forward
 // grid (T, H, B).  out: [B*S, C] bf16 (frame rows); lse: [B, H, S] fp32 (frame rows);
 // part: [B, H, T, M, 66] fp32 = {max, sum, unnormalised out[64]} of the global queries over this frame's keys.
@@ -102,7 +84,6 @@ vip_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_consta
   for (int qt = wg; qt < 4; qt += 2) {
     if (!tile_live(qt, d)) continue;
     const int r_lo = qt * 64 + wq * 16 + (lane >> 2);
-    const bool qg[2] = {row_global(r_lo), row_global(r_lo + 8)};
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -110,76 +91,13 @@ vip_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_consta
 #pragma unroll 1
     for (int kb = 0; kb < 4; ++kb) {
       if (!tile_live(kb, d)) continue;
-      float s[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) s[i] = 0.f;
-      wgmma_fence_regs(s);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        wgmma_m64n64k16_ss<0, 0>(s, kdesc(sQ + qt * TILE_BYTES + ks * 32), kdesc(sK + kb * TILE_BYTES + ks * 32));
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(s);
       // masks: padding keys; for global QUERY rows, the global keys count only once (frame 0)
-      float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = kb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
-          const bool dead = !row_valid(key, d) || (mask_gg && qg[e >> 1] && row_global(key));
-          if (dead) s[4 * i + e] = -INFINITY;
-          mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * i + e]);
-        }
-      float corr[2], mb[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float m_new = fmaxf(m_run[r], mx[r]);
-        corr[r] = (m_new == -INFINITY) ? 1.f : fast_exp2((m_run[r] - m_new) * LOG2E);
-        l_run[r] *= corr[r];
-        m_run[r] = m_new;
-        mb[r] = m_new == -INFINITY ? 0.f : m_new * LOG2E;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        o[4 * i + 0] *= corr[0]; o[4 * i + 1] *= corr[0];
-        o[4 * i + 2] *= corr[1]; o[4 * i + 3] *= corr[1];
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const float pv = fast_exp2(fmaf(s[i], LOG2E, -mb[(i >> 1) & 1]));   // exp2(-inf) = 0 for masked entries
-        s[i] = pv;
-        l_run[(i >> 1) & 1] += pv;
-      }
-      // P·V with P split into bf16 hi + lo (P = hi + lo to ~2^-16): rounding P to bf16 is the largest error of the forward,
-      // and it reaches the pooled CLS features through the global-query rows
-      uint32_t ph[4][4], pl[4][4];
-      acc_to_afrag(s, ph);
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          pl[ks][j] = pack_bf16(s[8 * ks + 2 * j] - bf16_lo(ph[ks][j]), s[8 * ks + 2 * j + 1] - bf16_hi(ph[ks][j]));
-      wgmma_fence_regs(o);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const uint64_t vd = mndesc(sV + kb * TILE_BYTES + ks * 16 * 128);
-        wgmma_m64n64k16_rs<1>(o, ph[ks], vd);
-        wgmma_m64n64k16_rs<1>(o, pl[ks], vd);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(o);
+      fwd_step(sQ + qt * TILE_BYTES, sK + kb * TILE_BYTES, sV + kb * TILE_BYTES, o, m_run, l_run, [&](int q, int key) {
+        const int k = kb * 64 + key;
+        return row_valid(k, d) && !(mask_gg && row_global(qt * 64 + q) && row_global(k));
+      });
     }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
-      l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
-    }
+    quad_sum(l_run);
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int row = r_lo + r * 8;
@@ -280,6 +198,10 @@ vip_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_consta
   const uint32_t sQ = smem_u32(sm), sK = sQ + MAT_BYTES, sV = sK + MAT_BYTES, sdO = sV + MAT_BYTES;
   const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const bool mask_gg = (t != 0);
+  // (query row, key row) pairs of the staged rows that enter the softmax
+  const auto pair_live = [&](int q, int key) {
+    return row_valid(q, d) && row_valid(key, d) && !(mask_gg && row_global(q) && row_global(key));
+  };
   float* gp = gpart + ((static_cast<long long>(b) * d.H + h) * d.T + t) * d.M * 3 * HD;
 
   // ------------------------------------------------ pass A: key-stationary -> dK, dV
@@ -292,47 +214,8 @@ vip_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_consta
 #pragma unroll 1
     for (int qb = 0; qb < 4; ++qb) {
       if (!tile_live(qb, d)) continue;
-      float st[32], dpt[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
-      wgmma_fence_regs(st);
-      wgmma_fence_regs(dpt);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        wgmma_m64n64k16_ss<0, 0>(st, kdesc(sK + kt * TILE_BYTES + ks * 32), kdesc(sQ + qb * TILE_BYTES + ks * 32));
-        wgmma_m64n64k16_ss<0, 0>(dpt, kdesc(sV + kt * TILE_BYTES + ks * 32), kdesc(sdO + qb * TILE_BYTES + ks * 32));
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(st);
-      wgmma_fence_regs(dpt);
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int q = qb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
-          const int key = k_lo + (e >> 1) * 8;
-          const bool valid = row_valid(q, d) && row_valid(key, d) && !(mask_gg && row_global(q) && row_global(key));
-          const float p = valid ? fast_exp2(fmaf(st[4 * i + e], LOG2E, -s_lse[q])) : 0.f;
-          st[4 * i + e] = p;
-          dpt[4 * i + e] = p * (dpt[4 * i + e] - s_delta[q]);
-        }
-      uint32_t ap[4][4], ad[4][4];
-      acc_to_afrag(st, ap);
-      acc_to_afrag(dpt, ad);
-      wgmma_fence_regs(dv);
-      wgmma_fence_regs(dk);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        wgmma_m64n64k16_rs<1>(dv, ap[ks], mndesc(sdO + qb * TILE_BYTES + ks * 16 * 128));
-        wgmma_m64n64k16_rs<1>(dk, ad[ks], mndesc(sQ + qb * TILE_BYTES + ks * 16 * 128));
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dv);
-      wgmma_fence_regs(dk);
+      kv_step(sK + kt * TILE_BYTES, sV + kt * TILE_BYTES, sQ + qb * TILE_BYTES, sdO + qb * TILE_BYTES, s_lse + qb * 64,
+              s_delta + qb * 64, dk, dv, [&](int q, int key) { return pair_live(qb * 64 + q, kt * 64 + key); });
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -367,40 +250,8 @@ vip_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_consta
 #pragma unroll 1
     for (int kb = 0; kb < 4; ++kb) {
       if (!tile_live(kb, d)) continue;
-      float s[32], dp[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
-      wgmma_fence_regs(s);
-      wgmma_fence_regs(dp);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        wgmma_m64n64k16_ss<0, 0>(s, kdesc(sQ + qt * TILE_BYTES + ks * 32), kdesc(sK + kb * TILE_BYTES + ks * 32));
-        wgmma_m64n64k16_ss<0, 0>(dp, kdesc(sdO + qt * TILE_BYTES + ks * 32), kdesc(sV + kb * TILE_BYTES + ks * 32));
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(s);
-      wgmma_fence_regs(dp);
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = kb * 64 + i * 8 + (lane & 3) * 2 + (e & 1);
-          const int q = q_lo + (e >> 1) * 8;
-          const bool valid = row_valid(q, d) && row_valid(key, d) && !(mask_gg && row_global(q) && row_global(key));
-          const float p = valid ? fast_exp2(fmaf(s[4 * i + e], LOG2E, -lse_r[e >> 1])) : 0.f;
-          dp[4 * i + e] = p * (dp[4 * i + e] - del_r[e >> 1]);
-        }
-      uint32_t ad[4][4];
-      acc_to_afrag(dp, ad);
-      wgmma_fence_regs(dq);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs<1>(dq, ad[ks], mndesc(sK + kb * TILE_BYTES + ks * 16 * 128));
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dq);
+      q_step(sQ + qt * TILE_BYTES, sdO + qt * TILE_BYTES, sK + kb * TILE_BYTES, sV + kb * TILE_BYTES, lse_r, del_r, dq,
+             [&](int q, int key) { return pair_live(qt * 64 + q, kb * 64 + key); });
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
