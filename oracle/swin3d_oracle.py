@@ -152,6 +152,12 @@ def shift_mask(Dp, Hp, Wp, ws, ss) -> torch.Tensor:
     return m.masked_fill(m != 0, -100.0).masked_fill(m == 0, 0.0)
 
 
+def softmax_av(logits, v):
+    """softmax(logits) @ v: the attention core, kept in one function so that a calibration arm can give it the backward
+    of the attention kernels (tests/test_gpu_encoder_calibration.py)."""
+    return logits.softmax(-1) @ v
+
+
 def window_attention(sd, p: str, xw, heads: int, mask: Optional[torch.Tensor]):
     """WindowAttention3D.forward, :135-164.  xw: [B*nW, N, C]."""
     B_, N, C = xw.shape
@@ -164,8 +170,7 @@ def window_attention(sd, p: str, xw, heads: int, mask: Optional[torch.Tensor]):
     if mask is not None:
         nW = mask.shape[0]
         attn = (attn.view(B_ // nW, nW, heads, N, N) + mask.unsqueeze(1).unsqueeze(0)).view(-1, heads, N, N)
-    attn = attn.softmax(-1)
-    out = (attn @ v).transpose(1, 2).reshape(B_, N, C)
+    out = softmax_av(attn, v).transpose(1, 2).reshape(B_, N, C)
     return F.linear(out, sd[p + "proj.weight"], sd[p + "proj.bias"])
 
 

@@ -100,14 +100,19 @@ def interpolated_tables(sd, cfg: TimeSformerCfg, T: int, H: int, W: int):
     return pos[0], time[0]
 
 
+def softmax_av(logits, v):
+    """softmax(logits) @ v: the attention core, kept in one function so that a calibration arm can give it the backward
+    of the attention kernels (tests/test_gpu_encoder_calibration.py)."""
+    return logits.softmax(dim=-1) @ v
+
+
 def attention(x, w_qkv, b_qkv, w_proj, b_proj, heads: int):
     """timesformer.py:156-173.  x: [G, N, C] (G independent groups)."""
     G, N, C = x.shape
     qkv = F.linear(x, w_qkv, b_qkv).reshape(G, N, 3, heads, C // heads).permute(2, 0, 3, 1, 4)
     q, k, v = qkv[0], qkv[1], qkv[2]
     attn = (q @ k.transpose(-2, -1)) * (C // heads) ** -0.5
-    attn = attn.softmax(dim=-1)
-    out = (attn @ v).transpose(1, 2).reshape(G, N, C)
+    out = softmax_av(attn, v).transpose(1, 2).reshape(G, N, C)
     return F.linear(out, w_proj, b_proj)
 
 

@@ -176,23 +176,13 @@ def test_training_mode_draws_the_references_rng_stream(dev):
 
 def test_released_config_one_sample_against_fp32_oracle_on_gpu(dev):
     """The released VideoEncoder config (6 stages, dims 128..1024, windows up to 32 x 3 x 5), 1 x 32 frames x 96 x 160:
-    bf16 kernels vs the oracle run in fp32 on the same GPU; forward and a few gradients."""
-    cfg = SO.Swin3DCfg()
-    sd = SO.init_state_dict(cfg, seed=4)
-    model = _build(cfg, sd, dev).eval()
-    video = SO.synthetic_video(1, 32, 96, 160, cfg, seed=5).to(dev)
-    sdo = {k: (v.to(dev).requires_grad_(True) if v.is_floating_point() else v.to(dev)) for k, v in sd.items()}
-    ref = SO.swin3d_forward(sdo, video, cfg)
-    w_out = torch.randn_like(ref) / ref[0].numel() ** 0.5
-    (ref * w_out).sum().backward()
-    out, _ = model(video)
-    (out * w_out).sum().backward()
-    print(f"released config: out rel-L2 {_rel(out.detach(), ref.detach()):.2e}")
-    assert _rel(out.detach(), ref.detach()) < 3e-2
-    params = dict(model.named_parameters())
+    the output and every parameter gradient within 1.5 x the bf16 oracle's error of the fp32 oracle, whole and per slice
+    (test_gpu_encoder_calibration.swin3d_case); and the earlier fixed thresholds on top."""
+    from test_gpu_encoder_calibration import swin3d_case
+    (out, _, grads), (ref, _, ref_grads) = swin3d_case(dev, "swin released_1x32x96x160", SO.Swin3DCfg(), 1, 32, 96, 160,
+                                                       weight_seed=4, data_seed=5, branches={"colsum"})
+    assert _rel(out, ref) < 3e-2
     for n in ("layers.2.blocks.5.attn.qkv.weight", "layers.2.blocks.6.attn.relative_position_bias_table",
               "layers.0.blocks.1.mlp.fc1.weight", "layers.4.downsample.reduction.weight", "layers.5.blocks.1.attn.proj.weight",
               "patch_embed.proj.weight"):
-        c = _cos(params[n].grad, sdo[n].grad)
-        print(f"  grad {n}: cos {c:.5f}")
-        assert c > 0.98, (n, c)
+        assert _cos(grads[n], ref_grads[n]) > 0.98, n
