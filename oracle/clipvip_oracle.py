@@ -68,12 +68,20 @@ def quick_gelu(x: Tensor) -> Tensor:
     return x * torch.sigmoid(1.702 * x)
 
 
+# The arithmetic points below (layer_norm, linear, residual_add, the attention cores and the embedding sums) are module-level
+# functions looked up at call time, so that a test can swap in a variant that rounds where a reduced-precision
+# implementation rounds (tests/test_gpu_clipvip_calibration.py).  The defaults are the fp32 / fp64 reference arithmetic.
 def layer_norm(x: Tensor, sd: Dict[str, Tensor], prefix: str, eps: float) -> Tensor:
     return F.layer_norm(x, (x.shape[-1],), sd[prefix + ".weight"], sd[prefix + ".bias"], eps)
 
 
 def linear(x: Tensor, sd: Dict[str, Tensor], prefix: str) -> Tensor:
     return F.linear(x, sd[prefix + ".weight"], sd.get(prefix + ".bias"))
+
+
+def residual_add(x: Tensor, h: Tensor) -> Tensor:
+    """The residual stream plus a block branch (CLIP_ViP.py:452,458)."""
+    return x + h
 
 
 # --------------------------------------------------------------------------- vision
@@ -101,7 +109,9 @@ def vip_embeddings(sd: Dict[str, Tensor], video: Tensor, cfg: ClipVipCfg,
     L = patches.shape[1]
     patches = patches.reshape(B, T, L, -1)
     pos = sd[pre + "position_embedding.weight"]
-    patches = patches + temporal_table(sd, T, pre).unsqueeze(2) + pos[1:].unsqueeze(0).unsqueeze(0)
+    if pre + "temporal_embedding" in sd:    # if_use_temporal_embed = 0 builds no table (CLIP_ViP.py:165-166,183)
+        patches = patches + temporal_table(sd, T, pre).unsqueeze(2)
+    patches = patches + pos[1:].unsqueeze(0).unsqueeze(0)
     cls = (sd[pre + "class_embedding"] + pos[0]).expand(B, 1, -1)
     proxies = (sd[pre + "added_cls"] + pos[0]).unsqueeze(0).expand(B, -1, -1)
     M = 1 + sd[pre + "added_cls"].shape[0]
@@ -127,6 +137,15 @@ def vip_attention(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, size: 
     q = split_heads(linear(x, sd, pre + "q_proj") * d ** -0.5, heads)
     k = split_heads(linear(x, sd, pre + "k_proj"), heads)
     v = split_heads(linear(x, sd, pre + "v_proj"), heads)
+    o = vip_core(q, k, v, size)
+    o = o.transpose(1, 2).reshape(B, S, C)
+    return linear(o, sd, pre + "out_proj")
+
+
+def vip_core(q: Tensor, k: Tensor, v: Tensor, size: Tuple[int, int, int]) -> Tensor:
+    """Both softmaxes of vip_attention: q (already scaled), k, v [B,H,S,d] -> o [B,H,S,d]."""
+    M, T, L = size
+    B, heads, S, d = q.shape
     qf = q[:, :, M:].reshape(B, heads, T, L, d)
     kg = k[:, :, :M].unsqueeze(2).expand(B, heads, T, M, d)
     vg = v[:, :, :M].unsqueeze(2).expand(B, heads, T, M, d)
@@ -134,9 +153,7 @@ def vip_attention(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, size: 
     vf = torch.cat([vg, v[:, :, M:].reshape(B, heads, T, L, d)], dim=3)
     of = torch.softmax(qf @ kf.transpose(-1, -2), dim=-1) @ vf      # [B,H,T,L,d]
     og = torch.softmax(q[:, :, :M] @ k.transpose(-1, -2), dim=-1) @ v  # [B,H,M,d]
-    o = torch.cat([og, of.reshape(B, heads, T * L, d)], dim=2)
-    o = o.transpose(1, 2).reshape(B, S, C)
-    return linear(o, sd, pre + "out_proj")
+    return torch.cat([og, of.reshape(B, heads, T * L, d)], dim=2)
 
 
 def dense_attention(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, add_mask: Optional[Tensor]) -> Tensor:
@@ -146,11 +163,16 @@ def dense_attention(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, add_
     q = split_heads(linear(x, sd, pre + "q_proj") * d ** -0.5, heads)
     k = split_heads(linear(x, sd, pre + "k_proj"), heads)
     v = split_heads(linear(x, sd, pre + "v_proj"), heads)
+    o = dense_core(q, k, v, add_mask)
+    return linear(o.transpose(1, 2).reshape(B, S, C), sd, pre + "out_proj")
+
+
+def dense_core(q: Tensor, k: Tensor, v: Tensor, add_mask: Optional[Tensor]) -> Tensor:
+    """softmax(q k^T + add_mask) v over [B,H,S,d] (q already scaled)."""
     s = q @ k.transpose(-1, -2)
     if add_mask is not None:
         s = s + add_mask
-    o = torch.softmax(s, dim=-1) @ v
-    return linear(o.transpose(1, 2).reshape(B, S, C), sd, pre + "out_proj")
+    return torch.softmax(s, dim=-1) @ v
 
 
 def encoder_layer(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, eps: float,
@@ -161,10 +183,10 @@ def encoder_layer(sd: Dict[str, Tensor], x: Tensor, pre: str, heads: int, eps: f
         h = vip_attention(sd, h, pre + "self_attn.", heads, size)
     else:
         h = dense_attention(sd, h, pre + "self_attn.", heads, add_mask)
-    x = x + h
+    x = residual_add(x, h)
     h = layer_norm(x, sd, pre + "layer_norm2", eps)
     h = linear(quick_gelu(linear(h, sd, pre + "mlp.fc1")), sd, pre + "mlp.fc2")
-    return x + h
+    return residual_add(x, h)
 
 
 def vision_tower(sd: Dict[str, Tensor], video: Tensor, cfg: ClipVipCfg, return_hidden: bool = False):
@@ -189,12 +211,17 @@ def text_additive_mask(attention_mask: Tensor, dtype: torch.dtype) -> Tensor:
     return causal[None, None] + pad
 
 
+def text_embeddings(sd: Dict[str, Tensor], input_ids: Tensor) -> Tensor:
+    """CLIPTextEmbeddings.forward, CLIP_ViP.py:210-227: token rows plus position rows 0..S-1."""
+    pre = "text_model.embeddings."
+    return sd[pre + "token_embedding.weight"][input_ids] + sd[pre + "position_embedding.weight"][:input_ids.shape[1]]
+
+
 def text_tower(sd: Dict[str, Tensor], input_ids: Tensor, attention_mask: Tensor, cfg: ClipVipCfg,
                return_hidden: bool = False):
     """CLIPTextTransformer.forward, CLIP_ViP.py:726-786."""
     B, S = input_ids.shape
-    pre = "text_model.embeddings."
-    x = sd[pre + "token_embedding.weight"][input_ids] + sd[pre + "position_embedding.weight"][:S]
+    x = text_embeddings(sd, input_ids)
     mask = text_additive_mask(attention_mask, x.dtype)
     hidden = [x]
     for i in range(cfg.text.layers):
@@ -214,8 +241,8 @@ def l2_normalize(x: Tensor) -> Tensor:
 def clip_vip_forward(sd: Dict[str, Tensor], video: Tensor, input_ids: Tensor, attention_mask: Tensor,
                      cfg: ClipVipCfg) -> Dict[str, Tensor]:
     """VidCLIP.forward (VidCLIP.py:32-53) -> CLIPModel.forward (CLIP_ViP.py:1089-1172)."""
-    vis = l2_normalize(vision_tower(sd, video, cfg) @ sd["visual_projection.weight"].t())
-    txt = l2_normalize(text_tower(sd, input_ids, attention_mask, cfg) @ sd["text_projection.weight"].t())
+    vis = l2_normalize(linear(vision_tower(sd, video, cfg), sd, "visual_projection"))
+    txt = l2_normalize(linear(text_tower(sd, input_ids, attention_mask, cfg), sd, "text_projection"))
     return {"vis_features": vis, "text_features": txt}
 
 

@@ -52,8 +52,8 @@ def frame_clip_forward(sd: Dict[str, Tensor], video: Tensor, input_ids: Tensor, 
     """VidCLIP.forward with a non-ViP type (VidCLIP.py:54-68): video [B,T,3,H,W] -> vis_features [B, P]; text_features is
     CLIP.py's normalised text_embeds."""
     B, T = video.shape[:2]
-    proj = frame_vision_tower(sd, video.reshape(B * T, *video.shape[2:]), cfg) @ sd["visual_projection.weight"].t()
-    txt = O.l2_normalize(O.text_tower(sd, input_ids, attention_mask, cfg) @ sd["text_projection.weight"].t())
+    proj = O.linear(frame_vision_tower(sd, video.reshape(B * T, *video.shape[2:]), cfg), sd, "visual_projection")
+    txt = O.l2_normalize(O.linear(O.text_tower(sd, input_ids, attention_mask, cfg), sd, "text_projection"))
     return {"vis_features": frame_mean_head(proj, B, T), "text_features": txt}
 
 

@@ -12,6 +12,9 @@ pytestmark = pytest.mark.gpu
 
 bf16, f32 = torch.bfloat16, torch.float32
 CALIBRATION = 1.5        # ours may deviate from the fp32 reference by at most 1.5 x what the reference's own bf16 run deviates
+# The loss and the logit_scale gradient (sum G Z) are each ONE sample of the logits error: the reference's own two bf16
+# runs differ on them by up to 15 x.  They are bounded by the larger of the two reference deviations, with a floor of 2e-3.
+SCALAR_SAMPLES = ("loss", "d vec logit_scale")
 EMB_REL_L2 = 1.2e-2
 
 
@@ -110,11 +113,8 @@ def _errors(gold, vis, txt, loss, grads):
     vec = [(k, _unpack(v)) for k, v in gold["grad_vectors"].items()]
     vec = [(k, g) for k, g in vec if float(g.norm()) > 1e-3 * gold["grad_norms"]["logit_scale"] and "k_proj.bias" not in k
            and k not in _pooled_row_sums(gold)]
-    per_vector = {k: _rel(grads[k], g) for k, g in vec}
-    worst = max(per_vector, key=per_vector.get)
-    e["d vectors (worst)"] = per_vector[worst]
-    print("  worst vectors: " + ", ".join(f"{k} {v:.2e}" for k, v in sorted(per_vector.items(), key=lambda kv: -kv[1])[:6]))
-    e["d vectors (median)"] = sorted(_rel(grads[k], g) for k, g in vec)[len(vec) // 2]
+    for k, g in vec:            # each vector against its own bar (the same vector's error in the reference's bf16 runs)
+        e["d vec " + k] = _rel(grads[k], g)
     return e
 
 
@@ -156,11 +156,12 @@ def test_frame_clip_golden_calibrated_against_reference_bf16(dev, golden_dir, na
     last = meta["vision_layers"] - 1
     low_rank = {f"d vision_model.encoder.layers.{last}.{m}.weight[rows]" for m in ("self_attn.out_proj", "mlp.fc2")}
     for k in ours:
-        if k == "loss":
+        if k in SCALAR_SAMPLES:
             continue
         bar = max(ref["autocast"][k], ref["pure"][k]) if k in low_rank else ref["autocast"][k]
         assert ours[k] <= CALIBRATION * bar + 1e-6, (k, ours[k], ref["autocast"][k], ref["pure"][k])
-    assert ours["loss"] <= max(CALIBRATION * max(ref["pure"]["loss"], ref["autocast"]["loss"]), 2e-3), (ours["loss"], ref)
+    for k in (k for k in SCALAR_SAMPLES if k in ours):
+        assert ours[k] <= max(CALIBRATION * max(ref["pure"][k], ref["autocast"][k]), 2e-3), (k, ours[k], ref)
 
 
 # ------------------------------------------------------------------------------------------ frame-mean head kernel

@@ -127,12 +127,15 @@ def _errors_vs_full_golden(gold, vis, txt, loss, grads):
         e["d " + k] = _rel(got, want)
     vec = [(k, _unpack(e)) for k, e in gold["grad_vectors"].items()]
     vec = [(k, g) for k, g in vec if float(g.norm()) > 1e-3 * gold["grad_norms"]["logit_scale"] and "k_proj.bias" not in k]
-    e["d vectors (worst)"] = max(_rel(grads[k], g) for k, g in vec)
-    e["d vectors (median)"] = sorted(_rel(grads[k], g) for k, g in vec)[len(vec) // 2]
+    for k, g in vec:            # each vector against its own bar (the same vector's error in the reference's bf16 runs)
+        e["d vec " + k] = _rel(grads[k], g)
     return e
 
 
 CALIBRATION = 1.5      # ours may deviate from the fp32 reference by at most 1.5 x what the reference's own bf16 run deviates
+# The loss and the logit_scale gradient (sum G Z) are each ONE sample of the logits error: the reference's own two bf16
+# runs differ on them by up to 15 x.  They are bounded by the larger of the two reference deviations, with a floor of 2e-3.
+SCALAR_SAMPLES = ("loss", "d vec logit_scale")
 
 
 def _full12_case(dev, golden_dir, pad_to):
@@ -184,12 +187,13 @@ def _assert_calibrated(ours, ref):
     import os
     against = "pure" if os.environ.get("XP_RESIDUAL_BF16") == "1" else "autocast"
     for k in ours:
-        if k == "loss":
+        if k in SCALAR_SAMPLES:
             continue
         assert ours[k] <= CALIBRATION * ref[against][k] + 1e-6, (k, ours[k], ref[against][k])
     # the scalar loss is ONE sample of the logits error (the reference's own two bf16 runs differ 18x on it): bounded by the
     # larger of the reference deviations, with a floor of 2e-3
-    assert ours["loss"] <= max(CALIBRATION * max(ref["pure"]["loss"], ref["autocast"]["loss"]), 2e-3), (ours["loss"], ref)
+    for k in (k for k in SCALAR_SAMPLES if k in ours):
+        assert ours[k] <= max(CALIBRATION * max(ref["pure"][k], ref["autocast"][k]), 2e-3), (k, ours[k], ref)
 
 
 def test_full_depth_t12_full_gradients_calibrated_against_reference_bf16(dev, golden_dir):

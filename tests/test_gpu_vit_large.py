@@ -11,6 +11,9 @@ import torch
 pytestmark = pytest.mark.gpu
 
 CALIBRATION = 1.5        # ours may deviate from the fp32 reference by at most 1.5 x what the reference's own bf16 run deviates
+# The loss and the logit_scale gradient (sum G Z) are each ONE sample of the logits error: the reference's own two bf16
+# runs differ on them by up to 15 x.  They are bounded by the larger of the two reference deviations, with a floor of 2e-3.
+SCALAR_SAMPLES = ("loss", "d vec logit_scale")
 EMB_REL_L2 = 1.2e-2
 GRAD_COSINE = 0.97
 
@@ -60,8 +63,8 @@ def _errors(gold, vis, txt, loss, grads):
         e["d " + k] = _rel(grads[k[:-len("[rows]")]][ent["rows"]], _unpack(ent))
     vec = [(k, _unpack(v)) for k, v in gold["grad_vectors"].items()]
     vec = [(k, g) for k, g in vec if float(g.norm()) > 1e-3 * gold["grad_norms"]["logit_scale"] and "k_proj.bias" not in k]
-    e["d vectors (worst)"] = max(_rel(grads[k], g) for k, g in vec)
-    e["d vectors (median)"] = sorted(_rel(grads[k], g) for k, g in vec)[len(vec) // 2]
+    for k, g in vec:            # each vector against its own bar (the same vector's error in the reference's bf16 runs)
+        e["d vec " + k] = _rel(grads[k], g)
     return e
 
 
@@ -101,11 +104,12 @@ def test_vit_l14_golden_calibrated_against_reference_bf16(dev, golden_dir, name)
     last = meta["vision_layers"] - 1
     rank_b = {f"d vision_model.encoder.layers.{last}.{m}.weight[rows]" for m in ("self_attn.out_proj", "mlp.fc2")}
     for k in ours:
-        if k == "loss":
+        if k in SCALAR_SAMPLES:
             continue
         bar = max(ref["autocast"][k], ref["pure"][k]) if k in rank_b else ref["autocast"][k]
         assert ours[k] <= CALIBRATION * bar + 1e-6, (k, ours[k], ref["autocast"][k], ref["pure"][k])
-    assert ours["loss"] <= max(CALIBRATION * max(ref["pure"]["loss"], ref["autocast"]["loss"]), 2e-3), (ours["loss"], ref)
+    for k in (k for k in SCALAR_SAMPLES if k in ours):
+        assert ours[k] <= max(CALIBRATION * max(ref["pure"][k], ref["autocast"][k]), 2e-3), (k, ours[k], ref)
 
 
 # ------------------------------------------------------------------------------------------ checkpointing, streams
