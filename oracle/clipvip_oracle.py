@@ -70,7 +70,7 @@ def quick_gelu(x: Tensor) -> Tensor:
 
 # The arithmetic points below (layer_norm, linear, residual_add, the attention cores and the embedding sums) are module-level
 # functions looked up at call time, so that a test can swap in a variant that rounds where a reduced-precision
-# implementation rounds (tests/test_gpu_clipvip_calibration.py).  The defaults are the fp32 / fp64 reference arithmetic.
+# implementation rounds (tests/clipvip_arm.py).  The defaults are the fp32 / fp64 reference arithmetic.
 def layer_norm(x: Tensor, sd: Dict[str, Tensor], prefix: str, eps: float) -> Tensor:
     return F.layer_norm(x, (x.shape[-1],), sd[prefix + ".weight"], sd[prefix + ".bias"], eps)
 

@@ -19,6 +19,8 @@ from typing import Dict, Optional
 
 import torch
 
+from oracle.embed_ref import ulp_bf16
+
 F64 = torch.float64
 ACT_NONE, ACT_QUICK_GELU, ACT_DQUICK_GELU, ACT_GELU_ERF, ACT_DGELU_ERF = 0, 1, 2, 3, 4     # include/xpretrain_b200.h
 OUT_BF16, OUT_F32, OUT_F32_ATOMIC = 0, 1, 2
@@ -37,12 +39,6 @@ def f32(x: torch.Tensor) -> torch.Tensor:
 def f16_sat(x: torch.Tensor) -> torch.Tensor:
     """cvt.rn.satfinite.f16: nearest even, values beyond fp16's range become +-65504 (NaN stays NaN)."""
     return x.clamp(-FP16_MAX, FP16_MAX).to(torch.float16).to(x.dtype)
-
-
-def ulp_bf16(x: torch.Tensor) -> torch.Tensor:
-    """Spacing of bf16 numbers at |x| (the smallest normal spacing below 2^-126)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126)))
-    return torch.exp2(e - 7)
 
 
 # ------------------------------------------------------------------------------------------ activations

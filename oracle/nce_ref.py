@@ -33,6 +33,8 @@ from typing import Dict, Optional, Sequence
 
 import torch
 
+from oracle.embed_ref import ulp_bf16
+
 F64 = torch.float64
 U = 2.0 ** -24
 EXP_ABS = 2.0 ** -21      # ex2.approx: 2^-22 relative, plus the rounding of its fp32 result
@@ -49,11 +51,6 @@ def bf(x: torch.Tensor) -> torch.Tensor:
 def ftz(x: torch.Tensor) -> torch.Tensor:
     """Flush values below the fp32 normal range to zero, as the kernels' fast-math arithmetic does."""
     return torch.where(x.abs() < TINY, torch.zeros_like(x), x)
-
-
-def ulp_bf16(x: torch.Tensor) -> torch.Tensor:
-    e = torch.floor(torch.log2(x.abs().clamp_min(TINY)))
-    return torch.exp2(e - 7)
 
 
 # ------------------------------------------------------------------------------------------ running error bound

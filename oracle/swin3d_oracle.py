@@ -154,7 +154,7 @@ def shift_mask(Dp, Hp, Wp, ws, ss) -> torch.Tensor:
 
 def softmax_av(logits, v):
     """softmax(logits) @ v: the attention core, kept in one function so that a calibration arm can give it the backward
-    of the attention kernels (tests/test_gpu_encoder_calibration.py)."""
+    of the attention kernels (tests/encoder_cases.py)."""
     return logits.softmax(-1) @ v
 
 

@@ -102,7 +102,7 @@ def interpolated_tables(sd, cfg: TimeSformerCfg, T: int, H: int, W: int):
 
 def softmax_av(logits, v):
     """softmax(logits) @ v: the attention core, kept in one function so that a calibration arm can give it the backward
-    of the attention kernels (tests/test_gpu_encoder_calibration.py)."""
+    of the attention kernels (tests/encoder_cases.py)."""
     return logits.softmax(dim=-1) @ v
 
 

@@ -1,0 +1,232 @@
+"""The calibrated bf16 rule of DESIGN.md §2 and the output checks shared by the kernel contract and calibration tests.
+
+  calibrated   per slice, ||got - ref|| <= FACTOR ||arm - ref|| + FLOOR ||ref|| (+ abs_floor sqrt(count)), where the arm
+               rounds to bf16 exactly where the kernel or module does; calibrated_model_rows applies it to whole tensors
+  within       element by element, |got - exact| <= bound; NaN fails, an exact element passes under a zero bound
+  coverage     Out (2-D, guard rows and pad columns) and Guarded (flat, guard bytes): logical elements start unwritten
+               (NaN, or the dtype's guard pattern for integer dtypes), every other element holds the guard pattern and
+               must keep it
+  same_bits    equality of the bit patterns (tells -0 from +0, compares NaN payloads)
+"""
+import contextlib
+
+import torch
+
+FACTOR = 1.5           # DESIGN.md §2: at most 1.5 x what the rounding of the computation itself costs
+FLOOR = 2.0 ** -16     # x the slice's reference norm: keeps exactly representable slices from dividing by zero
+ABS_FLOOR = 4e-6       # per element, for slices whose exact value is 0 (temporal T = 1: dq = dk = 0) but whose fp32
+                       # residue (dP - delta of O(1) inputs) is not; far below any rounding error of O(1e-3) outputs
+LSE_TOL = 1e-4         # LSE per row: |err| <= LSE_TOL x max(1, |lse|) (fp32 from fp32 scores)
+GUARD_ROWS = 3         # Out: rows past the output
+PAD = 64               # Guarded: bytes before and after the output (keeps it 64-byte aligned)
+
+# the integer view and the guard bit pattern of every dtype an output is guarded in; an integer output starts as its
+# pattern, so it may only be checked for writes where no written value can equal the pattern
+DTYPES = {
+    torch.bfloat16: (torch.int16, 0x3F81),
+    torch.float16: (torch.int16, 0x3C11),
+    torch.float32: (torch.int32, 0x3F810204),
+    torch.int32: (torch.int32, 0x3F810204),
+    torch.int64: (torch.int64, -7777),
+    torch.uint8: (torch.uint8, 0xA5),
+}
+
+
+def bits(t):
+    return t.contiguous().view(DTYPES[t.dtype][0])
+
+
+def same_bits(a, b):
+    return torch.equal(bits(a), bits(b))
+
+
+def _start(t):
+    """Mark the logical elements of an output unwritten: NaN, or the guard pattern for integer dtypes."""
+    if t.dtype.is_floating_point:
+        t.fill_(float("nan"))
+    else:
+        t.fill_(DTYPES[t.dtype][1])
+
+
+def _unwritten(t, finite):
+    """Count of elements still unwritten (for floating dtypes also, with `finite`, those not finite)."""
+    if t.dtype.is_floating_point:
+        return int((~torch.isfinite(t.float()) if finite else torch.isnan(t)).sum())
+    return int((t == DTYPES[t.dtype][1]).sum())
+
+
+class Out:
+    """An output of `rows` x `width` elements (row pitch ld) inside a buffer GUARD_ROWS rows longer: the logical elements
+    start unwritten (or as `init`), every other element holds the guard pattern."""
+
+    def __init__(self, dev, rows, width, dtype, ld=None, init=None):
+        ld = ld or width
+        self.shape = (rows + GUARD_ROWS, ld)
+        self.buf = torch.empty(self.shape, dtype=dtype, device=dev)
+        self.buf.view(DTYPES[dtype][0]).fill_(DTYPES[dtype][1])
+        self.t = self.buf[:rows, :width]
+        if init is None:
+            _start(self.t)
+        else:
+            self.t.copy_(init)
+        self.outside = torch.ones(self.shape, dtype=torch.bool, device=dev)
+        self.outside[:rows, :width] = False
+        self.snap = bits(self.buf).clone()
+
+    def check(self, what):
+        bad = _unwritten(self.t, finite=True)
+        assert bad == 0, f"{what}: {bad} of {self.t.numel()} elements not written (still NaN) or not finite"
+        moved = int((bits(self.buf) != self.snap)[self.outside].sum())
+        assert moved == 0, f"{what}: {moved} elements outside the output (guard rows / pad columns) were overwritten"
+        return self.t.clone()
+
+
+class Guarded:
+    """A tensor of `shape` inside an allocation with PAD bytes of guard pattern before and after it.  Its elements start
+    unwritten or as the given init."""
+
+    def __init__(self, dev, shape, dtype, init=None):
+        n = 1
+        for s in shape:
+            n *= s
+        self.pre = PAD // torch.empty(0, dtype=dtype).element_size()
+        self.n = n
+        self.buf = torch.empty(n + 2 * self.pre, dtype=dtype, device=dev)
+        self.buf.view(DTYPES[dtype][0]).fill_(DTYPES[dtype][1])
+        self.t = self.buf[self.pre:self.pre + n].view(shape)
+        if init is None:
+            _start(self.t)
+        else:
+            self.t.copy_(init)
+        self.snap = bits(self.buf).clone()
+
+    def guards(self, what):
+        iv, sv = bits(self.buf), self.snap
+        moved = int((iv[:self.pre] != sv[:self.pre]).sum() + (iv[self.pre + self.n:] != sv[self.pre + self.n:]).sum())
+        assert moved == 0, f"{what}: {moved} guard elements overwritten"
+
+    def written(self, what):
+        """Guards intact and every element written (inf is a value: an f16 output may overflow)."""
+        self.guards(what)
+        bad = _unwritten(self.t, finite=False)
+        assert bad == 0, f"{what}: {bad} of {self.n} elements not written"
+        return self.t
+
+
+class Report:
+    """The worst value recorded per key, printed under `header` by the owning module's autouse fixture (pytest -s)."""
+
+    def __init__(self, header, width=70, fmt="{:.3g}".format):
+        self.header, self.width, self.fmt, self.worst = header, width, fmt, {}
+
+    def record(self, key, value):
+        self.worst[key] = max(self.worst[key], value) if key in self.worst else value
+
+    def print(self):
+        if self.worst:
+            print("\n" + self.header)
+            for k in sorted(self.worst):
+                print(f"  {k:{self.width}s} {self.fmt(self.worst[k])}")
+
+
+def slice_rule(key, got, ref, arm, ids, label, abs_floor=0.0):
+    """Per slice (ids: slice index of every element; label(i) names slice i):
+    ||got - ref|| <= FACTOR ||arm - ref|| + FLOOR ||ref|| + abs_floor sqrt(count).  A slice with no elements passes.
+    Returns the worst err(got) / err(arm) (with the floor) and the message of the worst violation, or None."""
+    ids = ids.reshape(-1)
+    n = int(ids.max()) + 1
+
+    def norm(x):
+        return torch.zeros(n, dtype=torch.float64, device=x.device).index_add_(0, ids, x.reshape(-1) ** 2).sqrt()
+
+    ref = ref.double()
+    e_k, e_a, nrm = norm(got.double() - ref), norm(arm.double() - ref), norm(ref)
+    count = torch.zeros(n, dtype=torch.float64, device=ids.device).index_add_(0, ids, torch.ones_like(ref.reshape(-1)))
+    floor = FLOOR * nrm + abs_floor * count.sqrt() + (count == 0) + 1e-300
+    ratio = e_k / (FACTOR * e_a + floor)
+    w = int(ratio.argmax())
+    measured = float((e_k / (e_a + floor)).max())
+    if float(ratio[w]) <= 1.0:
+        return measured, None
+    return measured, (f"{key}: worst slice {label(w)}: error {float(e_k[w]):.3e} is "
+                      f"{float(e_k[w] / (e_a[w] + floor[w])):.2f} x the bf16 arm's {float(e_a[w]):.3e} "
+                      f"(slice norm {float(nrm[w]):.3e}; bound {FACTOR} x + {FLOOR:.1e} x norm)")
+
+
+def calibrated(report, key, got, ref, arm, ids, label, abs_floor=0.0):
+    """slice_rule asserted; the worst ratio is recorded under `key` and returned."""
+    measured, bad = slice_rule(key, got, ref, arm, ids, label, abs_floor)
+    report.record(key, measured)
+    assert bad is None, bad
+    return measured
+
+
+def tile_slices(M, N, device):
+    """Slice index [M, N] = (row // 64, col // 128): one consumer's 64 x 128 accumulator block of the GEMM, one
+    warpgroup's half of a fused 128 x 128 InfoNCE tile, one 64 x 128 tile of nce.cu."""
+    nc = (N + 127) // 128
+    ids = (torch.arange(M, device=device)[:, None] // 64) * nc + torch.arange(N, device=device)[None, :] // 128
+    return ids, lambda i: f"(row64={i // nc}, col128={i % nc})"
+
+
+def within(report, key, got, exact, bound):
+    """Every element: |got - exact| <= bound; NaN fails.  Records the worst |err| / bound (0 where err is 0)."""
+    err = (got.double() - exact).abs()
+    bad = ~(err <= bound)
+    ratio = torch.where(err == 0, 0.0, err / bound)
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    report.record(key, worst)
+    if bool(bad.any()):
+        w = int(bad.reshape(-1).nonzero()[0])
+        raise AssertionError(f"{key}: {int(bad.sum())} of {err.numel()} elements outside the bound, the first at flat "
+                             f"index {w}: got {float(got.reshape(-1)[w]):.7e}, exact {float(exact.reshape(-1)[w]):.7e}, "
+                             f"bound {float(bound.reshape(-1)[w]):.3e} (worst ratio {worst:.3g})")
+
+
+def lse_check(report, tag, got, ref):
+    """Per row: |lse - exact| <= LSE_TOL x max(1, |exact|)."""
+    err = (got.double() - ref).abs() / ref.abs().clamp_min(1.0)
+    w = int(err.reshape(-1).argmax())
+    report.record(f"{tag}: lse", float(err.max()))
+    assert float(err.max()) <= LSE_TOL, f"{tag}: lse: worst row (flat index {w}) relative error {float(err.max()):.3e}"
+
+
+def calibrated_model_rows(tag, rows, slices=None):
+    """The calibrated rule on whole tensors and, optionally, on slices of them.
+
+    rows: (name, ours, fp32 oracle, bf16 arm, autocast run or None) per tensor.  Whole tensor: err(ours) <= 1.5 x err(arm)
+    (+1e-7), both relative L2 against the fp32 oracle.  slices: name -> (ids, label) for `slice_rule` (per slice, with its
+    floor of 2^-16 x the slice's norm and ABS_FLOOR).  Returns (violations, worst whole-tensor ratio, worst slice ratio),
+    each ratio a (value, tensor name) pair; the autocast ratio is printed, never asserted."""
+    def rel(a, b):
+        return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
+
+    bad = []
+    worst, worst_ac, worst_sl = (0.0, ""), (0.0, ""), (0.0, "")
+    for name, got, ref, a, c in rows:
+        e, ea = rel(got, ref), rel(a, ref)
+        worst = max(worst, (e / (ea + 1e-7), name))
+        if c is not None:
+            worst_ac = max(worst_ac, (e / (rel(c, ref) + 1e-7), name))
+        if e > FACTOR * ea + 1e-7:
+            bad.append(f"{tag}: {name}: error {e:.3e} vs the bf16 oracle's {ea:.3e}")
+        if slices and name in slices:
+            ratio, msg = slice_rule(f"{tag}: {name}", got, ref, a, *slices[name], ABS_FLOOR)
+            worst_sl = max(worst_sl, (ratio, name))
+            if msg is not None:
+                bad.append(msg)
+    print(f"{tag}: worst err / bf16-oracle err {worst[0]:.3f} ({worst[1]})"
+          + (f", worst slice {worst_sl[0]:.3f} ({worst_sl[1]})" if slices else "")
+          + (f"; worst err / autocast err {worst_ac[0]:.2f} ({worst_ac[1]})" if worst_ac[1] else ""))
+    return bad, worst, worst_sl
+
+
+@contextlib.contextmanager
+def no_tf32():
+    """The fp32 oracle is the truth: no TF32 in its matmuls or convolutions."""
+    saved = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = saved

@@ -1,4 +1,4 @@
-"""The bf16 arm of test_gpu_clipvip_calibration.py on the CPU, and negative controls for the rule it defines.
+"""The bf16 arm of CLIP-ViP (clipvip_arm.py) on the CPU, and negative controls for the rule it defines.
 
 On a tiny CLIP-ViP (width 128, 2 heads of 64, 32 px frames in 8 px patches, T = 3 frames interpolated from a 12-row
 temporal table, M = 4 global rows, Lt = 8 tokens, 2 + 2 layers), one deliberate mistake is planted in the arm and the
@@ -21,8 +21,8 @@ at 1.7 x the arm's error).
 import pytest
 import torch
 
+from clipvip_arm import Bf16Arm, features_objective, oracle_run, rule_violations
 from oracle import clipvip_oracle as O
-from test_gpu_clipvip_calibration import Bf16Arm, features_objective, oracle_run, rule_violations
 
 TINY = O.ClipVipCfg(vision=O.TowerCfg(128, 2, 2, 512), text=O.TowerCfg(128, 2, 2, 512), image_size=32, patch=8,
                     proj_dim=64, vocab=1000, max_text_pos=16, temporal_size=12, add_cls_num=3)

@@ -1,4 +1,4 @@
-"""Negative controls for the calibrated rule of test_gpu_encoder_calibration.py, on the CPU.
+"""Negative controls for the calibrated rule that test_gpu_encoder_calibration.py holds the encoders to, on the CPU.
 
 On a tiny Swin-3D and a tiny divided TimeSformer, the fp32 oracle is run with one deliberate mistake and taken as "ours";
 against the clean fp32 oracle it must break the same rule (whole tensors and slices) that the GPU modules are held to,
@@ -22,10 +22,10 @@ import os
 import pytest
 import torch
 
+from contract_harness import calibrated_model_rows
+from encoder_cases import model_rows, swin_oracle, tsf_oracle
 from oracle import swin3d_oracle as SO
 from oracle import timesformer_oracle as TO
-from test_gpu_encoder_calibration import model_rows, swin_oracle, tsf_oracle
-from test_gpu_timesformer_variants import calibrated_model_rows
 
 SWIN = SO.Swin3DCfg(patch_size=(1, 4, 4), embed_dim=16, depths=(2, 2), num_heads=(2, 4), stages=(0, 1),
                     downsample_stages=(0,), window_size=((2, 3, 3), (2, 3, 3)))

@@ -1,5 +1,6 @@
 """H100: every attention kernel against the float64 references of oracle/attention_ref.py (pinned to the oracles by
-test_attention_reference_cpu.py), with the project's calibrated rule applied slice by slice, plus exact checks.
+test_attention_reference_cpu.py), with the project's calibrated rule (contract_harness.py) applied slice by slice, plus
+exact checks.
 
   calibrated   per slice, err(kernel) <= 1.5 x err(bf16 arm) + a floor of 2^-16 x the slice's reference norm, where the arm
                rounds to bf16 exactly where the kernel does; a 64-row tile, frame, head or window cannot hide in the norm
@@ -11,28 +12,18 @@ test_attention_reference_cpu.py), with the project's calibrated rule applied sli
   repeatable   two calls into fresh buffers give the same bits (no attention kernel uses float atomics)
   locality     inputs a slice does not depend on are perturbed with large finite values; the slice must keep every bit
 """
-import math
-
-import numpy as np
 import pytest
 import torch
 
+from contract_harness import ABS_FLOOR, Out, Report, calibrated, lse_check, same_bits
 from oracle import attention_ref as R
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32 = torch.bfloat16, torch.float32
-FACTOR = 1.5           # DESIGN.md §2: at most 1.5 x what the rounding of the computation itself costs
-FLOOR = 2.0 ** -16     # x the slice's reference norm: keeps exactly representable slices from dividing by zero
-ABS_FLOOR = 4e-6       # per element, for slices whose exact value is 0 (temporal T = 1: dq = dk = 0) but whose fp32
-                       # residue (dP - delta of O(1) inputs) is not; far below any rounding error of O(1e-3) outputs
-LSE_TOL = 1e-4
 PROBS_TOL = 1e-4       # text probabilities are an fp32 output: relative norm per (b, h) against the exact ones
 QS64, QS32 = 64 ** -0.5, 32 ** -0.5
-GUARD_ROWS = 3
-_INT = {bf16: torch.int16, f32: torch.int32}
-_PATTERN = {bf16: 0x3F81, f32: 0x3F810204}
-REPORT = {}
+REPORT = Report("worst slice ratio err(kernel) / err(bf16 arm), LSE and probs: worst relative error")
 
 
 @pytest.fixture(scope="module")
@@ -45,10 +36,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\nworst slice ratio err(kernel) / err(bf16 arm), LSE and probs: worst relative error")
-        for k in sorted(REPORT):
-            print(f"  {k:70s} {REPORT[k]:.3g}")
+    REPORT.print()
 
 
 def _ops():
@@ -58,62 +46,6 @@ def _ops():
 
 def _gen(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def same_bits(a, b):
-    return torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype]))
-
-
-class Out:
-    """An output of `rows` x `width` elements (row pitch ld) inside a buffer GUARD_ROWS rows longer: the logical elements
-    start as NaN, every other element holds a fixed bit pattern."""
-
-    def __init__(self, dev, rows, width, dtype, ld=None):
-        ld = ld or width
-        self.shape = (rows + GUARD_ROWS, ld)
-        self.buf = torch.empty(self.shape, dtype=dtype, device=dev)
-        self.buf.view(_INT[dtype]).fill_(_PATTERN[dtype])
-        self.t = self.buf[:rows, :width]
-        self.t.fill_(float("nan"))
-        self.outside = torch.ones(self.shape, dtype=torch.bool, device=dev)
-        self.outside[:rows, :width] = False
-        self.snap = self.buf.view(_INT[dtype]).clone()
-
-    def check(self, what):
-        bad = int((~torch.isfinite(self.t.float())).sum())
-        assert bad == 0, f"{what}: {bad} of {self.t.numel()} elements not written (still NaN) or not finite"
-        iv = self.buf.view(_INT[self.buf.dtype])
-        moved = int((iv != self.snap)[self.outside].sum())
-        assert moved == 0, f"{what}: {moved} elements outside the output (guard rows / pad columns) were overwritten"
-        return self.t
-
-
-def calibrated(tag, name, got, ref, arm, ids, label):
-    """Per slice (ids: slice index of every element): ||got - ref|| <= FACTOR ||arm - ref|| + FLOOR ||ref||."""
-    ids = ids.reshape(-1)
-    n = int(ids.max()) + 1
-
-    def norm(x):
-        return torch.zeros(n, dtype=torch.float64, device=x.device).index_add_(0, ids, x.reshape(-1) ** 2).sqrt()
-
-    ref = ref.double()
-    e_k, e_a, nrm = norm(got.double() - ref), norm(arm.double() - ref), norm(ref)
-    count = torch.zeros(n, dtype=torch.float64, device=ids.device).index_add_(0, ids, torch.ones_like(ref.reshape(-1)))
-    floor = FLOOR * nrm + ABS_FLOOR * count.sqrt() + (count == 0)     # slices absent from a subset count as 0 / 1
-    ratio = e_k / (FACTOR * e_a + floor)
-    w = int(ratio.argmax())
-    measured = float((e_k / (e_a + floor)).max())
-    REPORT[f"{tag}: {name}"] = max(REPORT.get(f"{tag}: {name}", 0.0), measured)
-    assert float(ratio[w]) <= 1.0, (f"{tag}: {name}: worst slice {label(w)}: error {float(e_k[w]):.3e} is "
-                                    f"{float(e_k[w] / (e_a[w] + floor[w])):.2f} x the bf16 arm's {float(e_a[w]):.3e} "
-                                    f"(slice norm {float(nrm[w]):.3e}; bound {FACTOR} x + {FLOOR:.1e} x norm)")
-
-
-def lse_check(tag, got, ref, label=None):
-    err = (got.double() - ref).abs() / ref.abs().clamp_min(1.0)
-    w = int(err.reshape(-1).argmax())
-    REPORT[f"{tag}: lse"] = max(REPORT.get(f"{tag}: lse", 0.0), float(err.max()))
-    assert float(err.max()) <= LSE_TOL, f"{tag}: lse: worst row (flat index {w}) relative error {float(err.max()):.3e}"
 
 
 # ================================================================================ ViP (staged and streamed)
@@ -201,8 +133,8 @@ def test_vip_attention_calibrated(dev, B, H, T, L, M, regime):
     out, lse = vip_fwd(dev, qkv, B, H, T, L, M)
     out2, lse2 = vip_fwd(dev, qkv, B, H, T, L, M)
     assert same_bits(out, out2) and same_bits(lse, lse2), f"{tag}: forward not bitwise repeatable"
-    calibrated(tag, "out", out, ex["out"], arm["out"], idc, label)
-    lse_check(tag, lse, ex["lse"])
+    calibrated(REPORT, f"{tag}: out", out, ex["out"], arm["out"], idc, label, ABS_FLOOR)
+    lse_check(REPORT, tag, lse, ex["lse"])
 
     # the backward reads the exact forward, rounded as the kernels store it
     out_in, lse_in = ex["out"].to(bf16), ex["lse"].float()
@@ -211,10 +143,11 @@ def test_vip_attention_calibrated(dev, B, H, T, L, M, regime):
     assert same_bits(dqkv, dqkv2), f"{tag}: backward not bitwise repeatable"
     for j, nm in enumerate(("dq", "dk", "dv")):
         cs = slice(j * C, (j + 1) * C)
-        calibrated(tag, nm, dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], idc, label)
+        calibrated(REPORT, f"{tag}: {nm}", dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], idc, label, ABS_FLOOR)
     # the global rows' dq on its own: summed over frames and scaled by q_scale in the combine kernel
     g = (torch.arange(B * (M + T * L), device=dev) % (M + T * L)) < M
-    calibrated(tag, "dq global rows", dqkv[g, :C], ex["dqkv"][g, :C], arm["dqkv"][g, :C], idc[g], label)
+    calibrated(REPORT, f"{tag}: dq global rows", dqkv[g, :C], ex["dqkv"][g, :C], arm["dqkv"][g, :C], idc[g], label,
+               ABS_FLOOR)
 
 
 def _perturb(x, rows, cols, seed, scale):
@@ -336,18 +269,18 @@ def test_text_attention_calibrated(dev, Lt, H):
         out, probs = text_fwd(dev, qkv, mdev, B, H, Lt)
         out2, probs2 = text_fwd(dev, qkv, mdev, B, H, Lt)
         assert same_bits(out, out2) and same_bits(probs, probs2), f"{tag}: forward not bitwise repeatable"
-        calibrated(tag, "out", out, ex["out"], arm["out"], ids, label)
+        calibrated(REPORT, f"{tag}: out", out, ex["out"], arm["out"], ids, label, ABS_FLOOR)
         zero = ex["probs"] == 0
         assert bool((probs[zero] == 0).all()), f"{tag}: probabilities of masked keys are not exactly 0"
         pe = ((probs.double() - ex["probs"]).flatten(2).norm(dim=2) / ex["probs"].flatten(2).norm(dim=2))
-        REPORT[f"{tag}: probs"] = float(pe.max())
+        REPORT.record(f"{tag}: probs", float(pe.max()))
         assert float(pe.max()) <= PROBS_TOL, f"{tag}: probs: worst (b, h) = {divmod(int(pe.argmax()), H)}: {float(pe.max()):.2e}"
         pin = ex["probs"].float()
         dqkv = text_bwd(dev, qkv, dout, pin, B, H, Lt, QS64)
         assert same_bits(dqkv, text_bwd(dev, qkv, dout, pin, B, H, Lt, QS64)), f"{tag}: backward not bitwise repeatable"
         for j, nm in enumerate(("dq", "dk", "dv")):
             cs = slice(j * C, (j + 1) * C)
-            calibrated(tag, nm, dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], ids, label)
+            calibrated(REPORT, f"{tag}: {nm}", dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], ids, label, ABS_FLOOR)
 
 
 def test_text_attention_locality_is_exact(dev):
@@ -495,8 +428,8 @@ def test_seg_attention_calibrated(dev, kind, size, wide):
     out, lse = seg.fwd()
     out2, lse2 = seg.fwd()
     assert same_bits(out, out2) and same_bits(lse, lse2), f"{tag}: forward not bitwise repeatable"
-    calibrated(tag, "out", out, ex["out"], arm["out"], idc, label)
-    lse_check(tag, lse, ex["lse"])
+    calibrated(REPORT, f"{tag}: out", out, ex["out"], arm["out"], idc, label, ABS_FLOOR)
+    lse_check(REPORT, tag, lse, ex["lse"])
 
     out_in, lse_in = ex["out"].to(bf16), ex["lse"].float()
     dqkv, ds = seg.bwd(out_in, lse_in)
@@ -504,11 +437,12 @@ def test_seg_attention_calibrated(dev, kind, size, wide):
     assert same_bits(dqkv, dqkv2) and (ds is None or same_bits(ds, ds2)), f"{tag}: backward not bitwise repeatable"
     for j, nm in enumerate(("dq", "dk", "dv")):
         cs = slice(j * C, (j + 1) * C)
-        calibrated(tag, nm, dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], idc, label)
+        calibrated(REPORT, f"{tag}: {nm}", dqkv[:, cs], ex["dqkv"][:, cs], arm["dqkv"][:, cs], idc, label, ABS_FLOOR)
     if ds is not None:
         n_win, L = seg.rows.shape
         dids = (torch.arange(n_win * seg.H, device=dev)[:, None].expand(-1, L * L)).reshape(n_win, seg.H, L, L)
-        calibrated(tag, "ds_out", ds, ex["ds"], arm["ds"], dids, lambda i: f"(window={i // seg.H}, head={i % seg.H})")
+        calibrated(REPORT, f"{tag}: ds_out", ds, ex["ds"], arm["ds"], dids,
+                   lambda i: f"(window={i // seg.H}, head={i % seg.H})", ABS_FLOOR)
 
 
 @pytest.mark.parametrize("kind", ["temporal", "spatial", "window"])

@@ -15,16 +15,13 @@ test_embed_reference_cpu.py.
 import pytest
 import torch
 
+from contract_harness import Guarded, Report, same_bits, within
 from oracle import embed_ref as E
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32, f16, F64 = torch.bfloat16, torch.float32, torch.float16, torch.float64
-_INT = {bf16: torch.int16, f16: torch.int16, f32: torch.int32, torch.int64: torch.int64, torch.int32: torch.int32,
-        torch.uint8: torch.uint8}
-_PATTERN = {torch.int16: 0x3F81, torch.int32: 0x3F810204, torch.int64: -7777, torch.uint8: 0xA5}
-PAD = 64          # guard bytes before and after every output (keeps the output 64-byte aligned)
-REPORT = {}
+REPORT = Report("embed: worst |err| / bound per kernel", width=40)
 TAPS = {"checked": 0, "drifted": 0, "worst_drift": 0.0}
 
 
@@ -38,10 +35,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\nembed: worst |err| / bound per kernel")
-        for k in sorted(REPORT):
-            print(f"  {k:40s} {REPORT[k]:.3g}")
+    REPORT.print()
     if TAPS["checked"]:
         print(f"embed: {TAPS['checked']} interpolation taps checked; {TAPS['drifted']} moved to a neighbouring index with "
               f"ulp-level weight (largest {TAPS['worst_drift']:.3g})")
@@ -55,50 +49,6 @@ def _ops():
 def _lib():
     from xpretrain_b200 import _lib
     return _lib
-
-
-def same_bits(a, b):
-    return torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype]))
-
-
-def within(key, got, exact, bound):
-    err = (got.to(F64) - exact).abs()
-    ratio = float((err / bound.clamp_min(1e-300)).max()) if err.numel() else 0.0
-    bad = int((err > bound).sum())
-    REPORT[key] = max(REPORT.get(key, 0.0), ratio)
-    assert bad == 0, f"{key}: {bad} of {err.numel()} elements outside the bound (worst ratio {ratio:.3g})"
-
-
-class Guarded:
-    """A tensor of `shape` inside an allocation with PAD bytes of fixed bit pattern before and after it.  Its elements
-    start as NaN (floating dtypes), the given init, or the pattern."""
-
-    def __init__(self, dev, shape, dtype, init=None, nan=True):
-        n = 1
-        for s in shape:
-            n *= s
-        self.pre = PAD // torch.empty(0, dtype=dtype).element_size()
-        self.n = n
-        self.buf = torch.empty(n + 2 * self.pre, dtype=dtype, device=dev)
-        self.buf.view(_INT[dtype]).fill_(_PATTERN[_INT[dtype]])
-        self.t = self.buf[self.pre:self.pre + n].view(shape)
-        if init is not None:
-            self.t.copy_(init)
-        elif nan and dtype.is_floating_point:
-            self.t.fill_(float("nan"))
-        self.snap = self.buf.view(_INT[dtype]).clone()
-
-    def guards(self, what):
-        iv, sv = self.buf.view(_INT[self.buf.dtype]), self.snap
-        moved = int((iv[:self.pre] != sv[:self.pre]).sum() + (iv[self.pre + self.n:] != sv[self.pre + self.n:]).sum())
-        assert moved == 0, f"{what}: {moved} guard elements overwritten"
-
-    def written(self, what):
-        self.guards(what)
-        if self.t.dtype.is_floating_point:
-            bad = int(torch.isnan(self.t).sum())
-            assert bad == 0, f"{what}: {bad} of {self.n} elements not written (still NaN)"
-        return self.t
 
 
 def _launches():
@@ -183,7 +133,7 @@ def test_vip_tables_within_bound_and_global_rows_exact(dev, Tsz, T, M, C):
     if t32 is not None:
         assert same_bits(tab, t32), "non-interpolated table differs from bf16(fp32(temporal + pos))"
     else:
-        within("vip_embed_tables (interpolated)", tab, exact, bound)
+        within(REPORT, "vip_embed_tables (interpolated)", tab, exact, bound)
 
 
 @pytest.mark.parametrize("T", [1, 4, 12, 32])
@@ -235,7 +185,7 @@ def _bwd_case(dev, B, T, L, M, C, Tsz, seed, with_temporal=True, with_cls=True, 
         if not use[k]:
             assert same_bits(got, init[k]), f"d_{k} was not requested but changed"
             continue
-        within(f"vip_embed_bwd d_{k}", got, *ref[k])
+        within(REPORT, f"vip_embed_bwd d_{k}", got, *ref[k])
 
 
 @pytest.mark.parametrize("Tsz,T,M,C", [(12, 12, 4, 768), (12, 5, 8, 512), (12, 32, 4, 1024), (12, 16, 1, 200),
@@ -297,8 +247,8 @@ def test_text_embeddings(dev, B, Lt, C, kind):
     d_tok, d_pos = Guarded(dev, (vocab, C), f32, init=t0), Guarded(dev, (Lt, C), f32, init=p0)
     ops.text_embed_bwd(ids, dx, d_tok.t, d_pos.t, Lt, C, vocab)
     ref = E.text_bwd_ref(ids, dx, t0, p0, Lt)
-    within("text_embed_bwd d_tok", d_tok.written("d_tok"), *ref["tok"])
-    within("text_embed_bwd d_pos", d_pos.written("d_pos"), *ref["pos"])
+    within(REPORT, "text_embed_bwd d_tok", d_tok.written("d_tok"), *ref["tok"])
+    within(REPORT, "text_embed_bwd d_pos", d_pos.written("d_pos"), *ref["pos"])
 
 
 # ============================================================================================== EOS
@@ -465,4 +415,4 @@ def test_vip_embed_bwd_copies_misaligned_gradients(dev, monkeypatch):
     ops.vip_embed_bwd(_misaligned(d_patch, 3), _misaligned(d_glob, 1), d_pos, None, None, None, B, T, L, M, C, 12)
     ref = E.vip_bwd_ref(d_patch, d_glob, {"pos": torch.zeros_like(d_pos), "cls": torch.zeros(C, device=dev)}, B, T, L, M, 12)
     assert len(calls) == 1
-    within("vip_embed_bwd d_pos (misaligned input)", d_pos, *ref["pos"])
+    within(REPORT, "vip_embed_bwd d_pos (misaligned input)", d_pos, *ref["pos"])

@@ -19,17 +19,14 @@ import zlib
 import pytest
 import torch
 
+from contract_harness import Out, Report, calibrated, same_bits, tile_slices, within
 from oracle import gemm_ref as R
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32 = torch.bfloat16, torch.float32
-FACTOR = 1.5           # DESIGN.md §2: at most 1.5 x what the rounding of the computation itself costs
-FLOOR = 2.0 ** -16     # x the slice's reference norm
-GUARD_ROWS = 3
-_INT = {bf16: torch.int16, f32: torch.int32}
-_PATTERN = {bf16: 0x3F81, f32: 0x3F810204}
-REPORT = {}
+REPORT = Report("GEMM: worst slice ratio err(kernel) / err(bf16 arm); element: worst |err| / bound; tail: worst relative "
+                "error", width=78)
 NONE, QG, DQG, GE, DGE = R.ACT_NONE, R.ACT_QUICK_GELU, R.ACT_DQUICK_GELU, R.ACT_GELU_ERF, R.ACT_DGELU_ERF
 ACT_NAME = {NONE: "none", QG: "QuickGELU", DQG: "dQuickGELU", GE: "GELU", DGE: "dGELU"}
 
@@ -44,10 +41,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\nGEMM: worst slice ratio err(kernel) / err(bf16 arm); element: worst |err| / bound; tail: worst relative error")
-        for k in sorted(REPORT):
-            print(f"  {k:78s} {REPORT[k]:.3g}")
+    REPORT.print()
 
 
 def _ops():
@@ -62,82 +56,6 @@ def _lib():
 
 def _gen(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def same_bits(a, b):
-    return torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype]))
-
-
-def _report_max(key, v):
-    REPORT[key] = max(REPORT.get(key, 0.0), float(v))
-
-
-class Out:
-    """An output of `rows` x `width` elements (row pitch ld) inside a buffer GUARD_ROWS rows longer: the logical elements
-    start as NaN (or `init`), every other element holds a fixed bit pattern."""
-
-    def __init__(self, dev, rows, width, dtype, ld=None, init=None):
-        ld = ld or width
-        self.shape = (rows + GUARD_ROWS, ld)
-        self.buf = torch.empty(self.shape, dtype=dtype, device=dev)
-        self.buf.view(_INT[dtype]).fill_(_PATTERN[dtype])
-        self.t = self.buf[:rows, :width]
-        if init is None:
-            self.t.fill_(float("nan"))
-        else:
-            self.t.copy_(init)
-        self.outside = torch.ones(self.shape, dtype=torch.bool, device=dev)
-        self.outside[:rows, :width] = False
-        self.snap = self.buf.view(_INT[dtype]).clone()
-
-    def check(self, what):
-        bad = int((~torch.isfinite(self.t.float())).sum())
-        assert bad == 0, f"{what}: {bad} of {self.t.numel()} elements not written (still NaN) or not finite"
-        iv = self.buf.view(_INT[self.buf.dtype])
-        moved = int((iv != self.snap)[self.outside].sum())
-        assert moved == 0, f"{what}: {moved} elements outside the output (guard rows / pad columns) were overwritten"
-        return self.t.clone()
-
-
-def calibrated(tag, name, got, ref, arm, ids, label):
-    """Per slice (ids: slice index of every element): ||got - ref|| <= FACTOR ||arm - ref|| + FLOOR ||ref||."""
-    ids = ids.reshape(-1)
-    n = int(ids.max()) + 1
-
-    def norm(x):
-        return torch.zeros(n, dtype=torch.float64, device=x.device).index_add_(0, ids, x.reshape(-1) ** 2).sqrt()
-
-    ref = ref.double()
-    e_k, e_a, nrm = norm(got.double() - ref), norm(arm.double() - ref), norm(ref)
-    floor = FLOOR * nrm + 1e-300
-    ratio = e_k / (FACTOR * e_a + floor)
-    w = int(ratio.argmax())
-    _report_max(f"{tag}: {name}", (e_k / (e_a + floor)).max())
-    assert float(ratio[w]) <= 1.0, (f"{tag}: {name}: worst slice {label(w)}: error {float(e_k[w]):.3e} is "
-                                    f"{float(e_k[w] / (e_a[w] + floor[w])):.2f} x the bf16 arm's {float(e_a[w]):.3e} "
-                                    f"(slice norm {float(nrm[w]):.3e}; bound {FACTOR} x + {FLOOR:.1e} x norm)")
-
-
-def element(tag, name, got, exact, bound):
-    err = (got.double() - exact).abs()
-    r = err / bound
-    w = int(r.reshape(-1).argmax())
-    _report_max(f"{tag}: {name} element", r.max())
-    assert float(r.max()) <= 1.0, (f"{tag}: {name}: element {divmod(w, got.shape[1])}: |err| {float(err.reshape(-1)[w]):.3e} "
-                                   f"> bound {float(bound.reshape(-1)[w]):.3e} (exact {float(exact.reshape(-1)[w]):.4e})")
-
-
-def slices(M, N, block_n, dev):
-    """Slice index [M, N] = (row // 64, col // 128): one consumer's 64 x 128 accumulator block under both schedules."""
-    nc = (N + 127) // 128
-    ids = (torch.arange(M, device=dev)[:, None] // 64) * nc + torch.arange(N, device=dev)[None, :] // 128
-
-    def label(i):
-        r64, c128 = divmod(i, nc)
-        if block_n == 128:
-            return f"(m_blk={r64 // 2}, n_blk={c128}, mh={r64 % 2})"
-        return f"(m_blk={r64 // 2}, n_blk={c128 // 2}, cw={r64 % 2}, h={c128 % 2})"
-    return ids, label
 
 
 # ============================================================================================ operands
@@ -232,19 +150,19 @@ def run_gemm(dev, tag, *, M, N, K, block_n, a_layout=0, b_layout=0, lda=None, ld
         return c.check(f"{tag}: C"), (pre.check(f"{tag}: aux (pre-activation)") if pre is not None else None)
 
     got, pre = launch(True)
-    ids, label = slices(M, N, block_n, dev)
+    ids, label = tile_slices(M, N, dev)
     kb = (K + 63) // 64
     K_split = min(K, ((kb + splits - 1) // splits) * 64)
     bound = R.gemm_element_bound(ex, K_split, splits, alpha=alpha, col_scale=col_scale, act=act, aux=aux_in, residual=res,
                                  bias=None if bias_t is None else bias_t[:N], c0=c0, out_mode=out_mode)
-    element(tag, "C", got, ex["exact"], bound)
+    within(REPORT, f"{tag}: C element", got, ex["exact"], bound)
     if out_mode == R.OUT_BF16:
-        calibrated(tag, "C", got, ex["exact"], ref["out"], ids, label)
+        calibrated(REPORT, f"{tag}: C", got, ex["exact"], ref["out"], ids, label)
     if pre is not None:
-        calibrated(tag, "aux", pre, ex["pre"], ref["pre"], ids, label)
+        calibrated(REPORT, f"{tag}: aux", pre, ex["pre"], ref["pre"], ids, label)
         pb = R.gemm_element_bound(ex, K_split, splits, alpha=alpha, col_scale=col_scale, bias=bias_t[:N] if bias else None)
         pb = pb + R.ulp_bf16(ex["pre"].abs() + pb)
-        element(tag, "aux", pre, ex["pre"], pb)
+        within(REPORT, f"{tag}: aux element", pre, ex["pre"], pb)
     # locality: clean padding gives the same bits; repeatability across calls and grid sizes (non-atomic outputs)
     if out_mode != R.OUT_F32_ATOMIC:
         got2, pre2 = launch(False)
@@ -257,7 +175,7 @@ def run_gemm(dev, tag, *, M, N, K, block_n, a_layout=0, b_layout=0, lda=None, ld
                 assert pre is None or same_bits(pre3, pre), f"{tag}: aux not bit-identical with set_sm_limit({sm})"
     else:
         got2, _ = launch(False)
-        element(tag, "C (clean padding)", got2, ex["exact"], bound)
+        within(REPORT, f"{tag}: C (clean padding) element", got2, ex["exact"], bound)
     return got, pre, ex
 
 
@@ -304,8 +222,8 @@ def test_gemm_wgrad_accumulates_into_grad(dev, C):
         ex = R.gemm_ref(dy.T, x.T, out_mode=R.OUT_F32_ATOMIC, c0=c0)
         kb = (rows + 63) // 64
         K_split = ((kb + splits - 1) // splits) * 64
-        element(f"{tag} splits{splits} bn{bn}", "dW", got, ex["exact"],
-                R.gemm_element_bound(ex, K_split, splits, c0=c0, out_mode=R.OUT_F32_ATOMIC))
+        within(REPORT, f"{tag} splits{splits} bn{bn}: dW element", got, ex["exact"],
+               R.gemm_element_bound(ex, K_split, splits, c0=c0, out_mode=R.OUT_F32_ATOMIC))
 
 
 # ================================================================================================ edges
@@ -377,9 +295,9 @@ def test_gemm_patch_embed_grouped(dev, patch):
         return x0.check(f"patch{patch}").reshape(Bv * T * L, C)
     got = launch(True)
     tag = f"patch-embed K{Kp} ld{ldp}"
-    ids, label = slices(Bv * T * L, C, 256, dev)
-    calibrated(tag, "x0", got, ex["exact"], ref_rows["out"], ids, label)
-    element(tag, "x0", got, ex["exact"], R.gemm_element_bound(ex, Kp, 1, residual=table.repeat(Bv, 1)))
+    ids, label = tile_slices(Bv * T * L, C, dev)
+    calibrated(REPORT, f"{tag}: x0", got, ex["exact"], ref_rows["out"], ids, label)
+    within(REPORT, f"{tag}: x0 element", got, ex["exact"], R.gemm_element_bound(ex, Kp, 1, residual=table.repeat(Bv, 1)))
     assert same_bits(launch(False), got), f"{tag}: NaN pad columns / rows changed the output"
 
 
@@ -400,7 +318,8 @@ def test_gemm_nce_head_launches(dev):
         torch.cuda.synchronize()
         got = out.check("nce dX")
         ex = R.gemm_ref(G[r0:r0 + rows, :N], T.T, alpha=scale, out_mode=R.OUT_F32)
-        element(f"nce dX bn{bn}", "dX", got, ex["exact"], R.gemm_element_bound(ex, N, 1, alpha=scale, out_mode=R.OUT_F32))
+        within(REPORT, f"nce dX bn{bn}: dX element", got, ex["exact"],
+               R.gemm_element_bound(ex, N, 1, alpha=scale, out_mode=R.OUT_F32))
         # d_txt: A = g^T as an MN-major window: column r0.. of g's rows, K = N rows of pitch Np
         Gm = rnd(g, N, Np).to(bf16).to(dev)
         Gm[:, :r0] = float("nan")
@@ -411,8 +330,8 @@ def test_gemm_nce_head_launches(dev):
         torch.cuda.synchronize()
         got = out.check("nce dY")
         ex = R.gemm_ref(Gm[:, r0:r0 + rows].T, T.T, alpha=scale, out_mode=R.OUT_F32)
-        element(f"nce dY a_offset bn{bn}", "dY", got, ex["exact"],
-                R.gemm_element_bound(ex, N, 1, alpha=scale, out_mode=R.OUT_F32))
+        within(REPORT, f"nce dY a_offset bn{bn}: dY element", got, ex["exact"],
+               R.gemm_element_bound(ex, N, 1, alpha=scale, out_mode=R.OUT_F32))
     # projection head: fp32 features of pooled bf16 rows
     run_gemm(dev, "projection OUT_F32", M=5, N=256, K=768, block_n=128, out_mode=R.OUT_F32, seed=3)
 
@@ -472,10 +391,10 @@ def test_gemm_epilogue_sweep_every_bf16_value(dev, act):
                                      f"{float(x[w]):.6e}: got {float(got[w]):.6e}, want {float(want[w]):.6e}")
         tail = (x >= -10) & (x <= -3)
         rel = (err / want.abs().clamp_min(1e-300))[tail]
-        _report_max(f"sweep {ACT_NAME[act]}: worst relative error on x in [-10, -3]", rel.max())
-        _report_max(f"sweep {ACT_NAME[act]}: worst relative error on x in [-5, -3]", rel[x[tail] >= -5].max())
-        _report_max(f"sweep {ACT_NAME[act]}: worst |err| / |x| on x in [-10, -3]", (err / x.abs())[tail].max())
-        _report_max(f"sweep {ACT_NAME[act]}: worst |err| / bound", (err / bound)[big].max())
+        REPORT.record(f"sweep {ACT_NAME[act]}: worst relative error on x in [-10, -3]", float(rel.max()))
+        REPORT.record(f"sweep {ACT_NAME[act]}: worst relative error on x in [-5, -3]", float(rel[x[tail] >= -5].max()))
+        REPORT.record(f"sweep {ACT_NAME[act]}: worst |err| / |x| on x in [-10, -3]", float((err / x.abs())[tail].max()))
+        REPORT.record(f"sweep {ACT_NAME[act]}: worst |err| / bound", float((err / bound)[big].max()))
 
 
 def test_dquick_gelu_at_the_ends_of_bf16_range(dev):
@@ -537,8 +456,9 @@ def test_quick_gelu_realistic_tail_calibrated_against_autocast(dev):
             got = c.check("fc1 realistic")
             ex = R.gemm_ref(A, B, act=QG)
             arm = R.gemm_ref(A, B, act=QG, arm="torch_bf16")
-            ids, label = slices(M, N, bn, dev)
-            calibrated(f"fc1 QuickGELU N(0,{sigma:g}) bn{bn}", "C vs autocast arm", got, ex["exact"], arm["out"], ids, label)
+            ids, label = tile_slices(M, N, dev)
+            calibrated(REPORT, f"fc1 QuickGELU N(0,{sigma:g}) bn{bn}: C vs autocast arm", got, ex["exact"], arm["out"], ids,
+                       label)
             tail = ex["pre"] < -4.0 / 1.702
             rel = ((got.double() - ex["exact"]).abs() / ex["exact"].abs().clamp_min(1e-300))[tail]
-            _report_max(f"fc1 QuickGELU N(0,{sigma:g}): worst relative error where 1.702 x < -4", rel.max())
+            REPORT.record(f"fc1 QuickGELU N(0,{sigma:g}): worst relative error where 1.702 x < -4", float(rel.max()))

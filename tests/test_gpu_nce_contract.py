@@ -21,17 +21,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from contract_harness import Out, Report, calibrated, same_bits, tile_slices, within
 from oracle import nce_ref as R
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32, F64 = torch.bfloat16, torch.float32, torch.float64
-FACTOR = 1.5           # DESIGN.md §2: at most 1.5 x what the rounding of the computation itself costs
-FLOOR = 2.0 ** -16     # x the slice's reference norm
-GUARD_ROWS = 3
-_INT = {bf16: torch.int16, f32: torch.int32}
-_PATTERN = {bf16: 0x3F81, f32: 0x3F810204}
-REPORT = {}
+REPORT = Report("NCE: worst slice ratio err(kernel) / err(bf16 arm); element / scalar: worst |err| / bound")
 LOG_SCALES = (0.0, 2.659, 4.6052)      # s = 1, the CLIP initialisation, the drivers' clamp at 100
 TABLES = ("NCEContrastiveLoss", "VidImgDivideNCELearnableTempLoss", "NCELearnableTempLoss_vs_vc",
           "NCELearnableTempLoss_vs_vc_fc", "NCELearnableTempLoss_vsc", "NCELearnableTempLoss_vsc_fc")
@@ -48,10 +44,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\nNCE: worst slice ratio err(kernel) / err(bf16 arm); element / scalar: worst |err| / bound")
-        for k in sorted(REPORT):
-            print(f"  {k:70s} {REPORT[k]:.3g}")
+    REPORT.print()
 
 
 def _lib():
@@ -69,14 +62,6 @@ def _loss():
     return loss
 
 
-def _report_max(key, v):
-    REPORT[key] = max(REPORT.get(key, 0.0), float(v))
-
-
-def same_bits(a, b):
-    return torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype]))
-
-
 def ceil4(n):
     return (n + 3) // 4 * 4
 
@@ -85,69 +70,21 @@ def ceil8(n):
     return (n + 7) // 8 * 8
 
 
-class Out:
-    """An output of `rows` x `width` elements (row pitch ld) inside a buffer GUARD_ROWS rows longer: the logical elements
-    start as NaN, every other element holds a fixed bit pattern."""
-
-    def __init__(self, dev, rows, width, dtype, ld=None):
-        ld = ld or width
-        self.shape = (rows + GUARD_ROWS, ld)
-        self.buf = torch.empty(self.shape, dtype=dtype, device=dev)
-        self.buf.view(_INT[dtype]).fill_(_PATTERN[dtype])
-        self.t = self.buf[:rows, :width]
-        self.t.fill_(float("nan"))
-        self.outside = torch.ones(self.shape, dtype=torch.bool, device=dev)
-        self.outside[:rows, :width] = False
-        self.snap = self.buf.view(_INT[dtype]).clone()
-
-    def check(self, what):
-        bad = int((~torch.isfinite(self.t.float())).sum())
-        assert bad == 0, f"{what}: {bad} of {self.t.numel()} elements not written (still NaN) or not finite"
-        moved = int((self.buf.view(_INT[self.buf.dtype]) != self.snap)[self.outside].sum())
-        assert moved == 0, f"{what}: {moved} elements outside the output (guard rows / pad columns) were overwritten"
-        return self.t.clone()
-
-
 # ============================================================================================ the rules
-def calibrated(tag, name, got, exact, arm):
-    """Per slice (row // 64, col // 128): ||got - exact|| <= FACTOR ||arm - exact|| + FLOOR ||exact||."""
-    M, N = exact.shape
-    nc = (N + 127) // 128
-    ids = ((torch.arange(M, device=exact.device)[:, None] // 64) * nc
-           + torch.arange(N, device=exact.device)[None, :] // 128).reshape(-1)
-    n = int(ids.max()) + 1
-
-    def norm(x):
-        return torch.zeros(n, dtype=F64, device=x.device).index_add_(0, ids, x.reshape(-1).to(F64) ** 2).sqrt()
-
-    e_k, e_a, nrm = norm(got.to(F64) - exact), norm(arm.to(F64) - exact), norm(exact)
-    floor = FLOOR * nrm + 1e-300
-    ratio = e_k / (FACTOR * e_a + floor)
-    w = int(ratio.argmax())
-    _report_max(f"{tag}: {name}", (e_k / (e_a + floor)).max())
-    assert float(ratio[w]) <= 1.0, (f"{tag}: {name}: worst slice (row64={w // nc}, col128={w % nc}): error "
-                                    f"{float(e_k[w]):.3e} is {float(e_k[w] / (e_a[w] + floor[w])):.2f} x the bf16 arm's "
-                                    f"{float(e_a[w]):.3e} (slice norm {float(nrm[w]):.3e})")
-
-
-def element(tag, name, got, exact, bound):
-    err = (got.to(F64) - exact).abs()
-    r = err / bound
-    w = int(r.reshape(-1).argmax())
-    _report_max(f"{tag}: {name} element", r.max())
-    assert float(r.max()) <= 1.0, (f"{tag}: {name}: element {divmod(w, got.shape[1])}: |err| {float(err.reshape(-1)[w]):.3e}"
-                                   f" > bound {float(bound.reshape(-1)[w]):.3e} (exact {float(exact.reshape(-1)[w]):.4e})")
+def tiled(tag, name, got, exact, arm):
+    """The calibrated rule per (row // 64, col // 128) slice."""
+    calibrated(REPORT, f"{tag}: {name}", got, exact, arm, *tile_slices(*exact.shape, exact.device))
 
 
 def scalar(tag, name, got, exact, bound):
     err = abs(float(got) - float(exact))
-    _report_max(f"{tag}: {name}", err / float(bound))
+    REPORT.record(f"{tag}: {name}", err / float(bound))
     assert err <= float(bound), f"{tag}: {name} {float(got):.8g} vs exact {float(exact):.8g}: |err| {err:.3e} > {float(bound):.3e}"
 
 
 def check_sg(tag, got, ref, k=0, name="s dL/dZ"):
-    calibrated(tag, name, got, ref["exact"][k], ref["arm"][k])
-    element(tag, name, got, ref["exact"][k], ref["bound"][k])
+    tiled(tag, name, got, ref["exact"][k], ref["arm"][k])
+    within(REPORT, f"{tag}: {name} element", got, ref["exact"][k], ref["bound"][k])
 
 
 def check_scalars(tag, loss, dscale, ref):
@@ -245,8 +182,8 @@ def check_backward(tag, g, vh, th, V, T, ref, row0=0, nrows=None, scale=1.0):
     ex = R.feature_grads(((0, 1),), ref["exact"], [V, T])
     arm = R.feature_grads(((0, 1),), ref["arm"], [R.bf(V), R.bf(T)])
     rows = slice(row0, row0 + nrows)
-    calibrated(tag, "dV", d_vis, scale * ex[0][rows], scale * arm[0][rows])
-    calibrated(tag, "dT", d_txt, scale * ex[1][rows], scale * arm[1][rows])
+    tiled(tag, "dV", d_vis, scale * ex[0][rows], scale * arm[0][rows])
+    tiled(tag, "dT", d_txt, scale * ex[1][rows], scale * arm[1][rows])
 
 
 FUSED = [  # (world, b, d, kind, log-scale)
@@ -521,8 +458,8 @@ def test_multi_launch_infonce(dev, N, d):
     assert all(same_bits(a.reshape(-1), b.reshape(-1)) for a, b in zip(*grads)), f"{tag} N{N}: module results differ"
     ex = R.feature_grads(((0, 1),), ref["exact"], [Vd, Td])
     arm = R.feature_grads(((0, 1),), ref["arm"], [R.bf(Vd), R.bf(Td)])
-    calibrated(f"{tag} module", "dV", grads[0][1], ex[0], arm[0])
-    calibrated(f"{tag} module", "dT", grads[0][2], ex[1], arm[1])
+    tiled(f"{tag} module", "dV", grads[0][1], ex[0], arm[0])
+    tiled(f"{tag} module", "dT", grads[0][2], ex[1], arm[1])
     check_scalars(f"{tag} module", grads[0][0], grads[0][3], ref)
 
 
@@ -582,7 +519,7 @@ def test_module_api_feature_gradients(dev, name):
     tag = f"module {name}"
     for k, x in enumerate(args):
         if k in ex:
-            calibrated(tag, f"d feature {k}", x.grad, ex[k], arm[k])
+            tiled(tag, f"d feature {k}", x.grad, ex[k], arm[k])
         else:
             assert x.grad is None or float(x.grad.abs().max()) == 0.0, f"{tag}: argument {k} is not read but has a gradient"
     check_scalars(tag, loss.detach(), None if name == "NCEContrastiveLoss" else p.grad, ref)
@@ -606,6 +543,6 @@ def test_gather_nce_loss_single_process(dev, grad_scale):
     ex = R.feature_grads(pairs, ref["exact"], mats)
     arm = R.feature_grads(pairs, ref["arm"], [R.bf(x) for x in mats])
     tag = f"gather_nce_loss grad_scale={grad_scale}"
-    calibrated(tag, "dV", v.grad, sc * ex[0], sc * arm[0])
-    calibrated(tag, "dT", t.grad, sc * ex[1], sc * arm[1])
+    tiled(tag, "dV", v.grad, sc * ex[0], sc * arm[0])
+    tiled(tag, "dT", t.grad, sc * ex[1], sc * arm[1])
     check_scalars(tag, loss.detach(), p.grad, ref)

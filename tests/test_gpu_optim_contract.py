@@ -18,15 +18,16 @@ import numpy as np
 import pytest
 import torch
 
+from contract_harness import DTYPES, Report, bits, within
 from oracle import optim_ref as O
 
 pytestmark = pytest.mark.gpu
 
-F64, bf16, f32 = torch.float64, torch.bfloat16, torch.float32
+bf16, f32 = torch.bfloat16, torch.float32
 GUARD = 16                     # fp32 guard elements on each side of every tensor (64 bytes)
 SIZES = [1, 2, 3, 4, 5, 8191, 8192, 8193, 3 * 8192 + 77]
 BETAS, EPS = (0.9, 0.98), 1e-6
-REPORT = {}
+REPORT = Report("optim: worst |err| / bound", width=40)
 
 
 @pytest.fixture(scope="module")
@@ -39,10 +40,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\noptim: worst |err| / bound")
-        for k in sorted(REPORT):
-            print(f"  {k:40s} {REPORT[k]:.3g}")
+    REPORT.print()
 
 
 def _lib():
@@ -55,16 +53,12 @@ def _adamw():
     return adamw
 
 
-def bits(t):
-    return t.view(torch.int16 if t.dtype == bf16 else torch.int32)
-
-
 class Slot:
     """n elements of `dtype` at element offset `off` past a 64-byte boundary, GUARD pattern elements on each side."""
 
     def __init__(self, dev, n, dtype=f32, off=0, init=None):
         self.buf = torch.empty(n + off + 2 * GUARD, dtype=dtype, device=dev)
-        bits(self.buf).fill_(0x3F81 if dtype == bf16 else 0x3F810204)
+        bits(self.buf).fill_(DTYPES[dtype][1])
         self.lo, self.n = GUARD + off, n
         self.t = self.buf[self.lo:self.lo + n]
         if init is not None:
@@ -133,17 +127,10 @@ class Set:
         return all(r[k].guards_intact() for r in self.rows for k in ("p", "g", "m", "v", "pb") if r[k] is not None)
 
 
-def within(key, got, exact, bound):
-    err = (got.to(F64) - exact).abs()
-    ratio = float((err / bound.clamp_min(1e-300)).max())
-    REPORT[key] = max(REPORT.get(key, 0.0), ratio)
-    assert int((err > bound).sum()) == 0, f"{key}: worst |err| / bound = {ratio:.3g}"
-
-
 def check_norm(s, got):
     norm, rel = O.grad_norm_ref([r["g"].t for r in s.rows])
     err = abs(float(got[0]) - norm)
-    REPORT["grad_norm (relative)"] = max(REPORT.get("grad_norm (relative)", 0.0), err / (rel * norm))
+    REPORT.record("grad_norm (relative)", err / (rel * norm))
     assert err <= rel * norm, f"norm {float(got[0])} vs {norm}: {err / norm:.3g} relative (bound {rel:.3g})"
 
 
@@ -210,7 +197,7 @@ def _check_step(tag, s, before, coef):
     for i, (r, b) in enumerate(zip(s.rows, before)):
         ref = O.adamw_ref(b["p"], b["g"], b["m"], b["v"], coef, BETAS[0], BETAS[1], EPS, r["step_size"], r["decay"])
         for k in ("p", "m", "v"):
-            within(f"adamw {k}", r[k].t, *ref[k])
+            within(REPORT, f"adamw {k}", r[k].t, *ref[k])
         assert float(ref["p"][1].max()) < 1e-2 * r["step_size"]
         if r["pb"] is not None:
             assert torch.equal(bits(r["pb"].t), bits(r["p"].t.to(bf16))), f"{tag}: bf16 target of tensor {i}"

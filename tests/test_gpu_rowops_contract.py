@@ -1,5 +1,5 @@
 """H100: the LayerNorm and small row kernels of rowops.cu against the float64 references of oracle/gemm_ref.py (pinned to
-F.layer_norm and autograd by test_gemm_reference_cpu.py), with the rules of test_gpu_gemm_contract.py.
+F.layer_norm and autograd by test_gemm_reference_cpu.py), with the rules of contract_harness.py.
 
   calibrated   y and dx per logical row: ||got - exact|| <= 1.5 x ||arm - exact|| + 2^-16 x the row's norm, the arm being the
                float64 LayerNorm of the stream value the kernel normalises, rounded once to the output dtype
@@ -13,19 +13,16 @@ F.layer_norm and autograd by test_gemm_reference_cpu.py), with the rules of test
 import pytest
 import torch
 
+from contract_harness import DTYPES, GUARD_ROWS, Report, bits, calibrated, same_bits, within
 from oracle import gemm_ref as R
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32, f16 = torch.bfloat16, torch.float32, torch.float16
-FACTOR, FLOOR = 1.5, 2.0 ** -16
 U = 2.0 ** -24
-GUARD_ROWS = 3
 EPS = 1e-5
-_INT = {bf16: torch.int16, f16: torch.int16, f32: torch.int32}
-_PATTERN = {bf16: 0x3F81, f16: 0x3C11, f32: 0x3F810204}
 DT_NAME = {bf16: "bf16", f32: "fp32", f16: "fp16"}
-REPORT = {}
+REPORT = Report("row kernels: worst row ratio err(kernel) / err(arm); statistics / reductions: worst |err| / bound")
 
 
 @pytest.fixture(scope="module")
@@ -38,10 +35,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    if REPORT:
-        print("\nrow kernels: worst row ratio err(kernel) / err(arm); statistics / reductions: worst |err| / bound")
-        for k in sorted(REPORT):
-            print(f"  {k:70s} {REPORT[k]:.3g}")
+    REPORT.print()
 
 
 def _ops():
@@ -53,17 +47,9 @@ def _gen(seed):
     return torch.Generator().manual_seed(seed)
 
 
-def _report_max(key, v):
-    REPORT[key] = max(REPORT.get(key, 0.0), float(v))
-
-
-def same_bits(a, b):
-    return torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype]))
-
-
 class Rows:
     """A [total, ld] buffer (GUARD_ROWS extra) whose `rows` (indices into the first `total` rows) are the logical output:
-    they start as NaN, every other element holds `fill` (a bit pattern by default) and must keep it."""
+    they start as NaN, every other element holds `fill` (the guard pattern by default) and must keep it."""
 
     def __init__(self, dev, total, C, dtype, rows=None, ld=None, zero=False):
         ld = ld or C
@@ -71,40 +57,27 @@ class Rows:
         if zero:
             self.buf.zero_()
         else:
-            self.buf.view(_INT[dtype]).fill_(_PATTERN[dtype])
+            self.buf.view(DTYPES[dtype][0]).fill_(DTYPES[dtype][1])
         self.rows = torch.arange(total, device=dev) if rows is None else rows
         self.C = C
         self.buf[self.rows, :C] = float("nan")
         self.outside = torch.ones_like(self.buf, dtype=torch.bool)
         self.outside[self.rows, :C] = False
-        self.snap = self.buf.view(_INT[dtype]).clone()
+        self.snap = bits(self.buf).clone()
 
     def check(self, what):
         got = self.buf[self.rows, :self.C]
         bad = int((~torch.isfinite(got.float())).sum())
         assert bad == 0, f"{what}: {bad} of {got.numel()} elements not written (still NaN) or not finite"
-        moved = int((self.buf.view(_INT[self.buf.dtype]) != self.snap)[self.outside].sum())
+        moved = int((bits(self.buf) != self.snap)[self.outside].sum())
         assert moved == 0, f"{what}: {moved} elements outside the output (guard / unmapped rows, pad columns) were overwritten"
         return got
 
 
 def per_row(tag, name, got, exact, arm):
-    e_k = (got.double() - exact).norm(dim=-1)
-    e_a = (arm - exact).norm(dim=-1)
-    floor = FLOOR * exact.norm(dim=-1) + 1e-300
-    ratio = e_k / (FACTOR * e_a + floor)
-    w = int(ratio.argmax())
-    _report_max(f"{tag}: {name}", (e_k / (e_a + floor)).max())
-    assert float(ratio[w]) <= 1.0, (f"{tag}: {name}: row {w}: error {float(e_k[w]):.3e} is "
-                                    f"{float(e_k[w] / (e_a[w] + floor[w])):.2f} x the arm's {float(e_a[w]):.3e}")
-
-
-def bounded(tag, name, got, exact, bound):
-    r = (got.double() - exact).abs() / bound
-    _report_max(f"{tag}: {name}", r.max())
-    w = int(r.reshape(-1).argmax())
-    assert float(r.max()) <= 1.0, (f"{tag}: {name}: element {w}: got {float(got.reshape(-1)[w]):.7e}, exact "
-                                   f"{float(exact.reshape(-1)[w]):.7e}, bound {float(bound.reshape(-1)[w]):.3e}")
+    """The calibrated rule with one slice per logical row."""
+    ids = torch.arange(exact.shape[0], device=exact.device)[:, None].expand(exact.shape)
+    calibrated(REPORT, f"{tag}: {name}", got, exact, arm, ids, lambda i: f"row {i}")
 
 
 def stats_check(tag, mean, rstd, ref, C):
@@ -112,9 +85,9 @@ def stats_check(tag, mean, rstd, ref, C):
     nseq = C / 32 + 16
     s = ref["sum"]
     tol_mean = 2.0 ** -20 * ref["mean"].abs() + nseq * U * s.abs().mean(-1)
-    bounded(tag, "mean", mean, ref["mean"], tol_mean + 1e-300)
+    within(REPORT, f"{tag}: mean", mean, ref["mean"], tol_mean + 1e-300)
     rel = 2.0 ** -20 + nseq * U + (tol_mean / ref["std"]) ** 2
-    bounded(tag, "rstd", rstd, ref["rstd"], rel * ref["rstd"])
+    within(REPORT, f"{tag}: rstd", rstd, ref["rstd"], rel * ref["rstd"])
 
 
 def ln_inputs(dev, rows, C, xdt, seed, with_add):
@@ -181,7 +154,7 @@ def test_layernorm_fwd_bwd_calibrated(dev, C):
         per_row(tag, "dx", got, ex["dx"], R.bf(ex["dx"]))
         nterm = rows + (rows + 7) // 8 + 16
         for nm, t, s0 in (("dgamma", dgam, g0[0]), ("dbeta", dbet, g0[1]), ("dres_colsum", dcol, g0[2])):
-            bounded(tag, nm, t, s0.double() + ex[nm], nterm * U * (ex["abs_" + nm] + s0.double().abs()) + 1e-30)
+            within(REPORT, f"{tag}: {nm}", t, s0.double() + ex[nm], nterm * U * (ex["abs_" + nm] + s0.double().abs()) + 1e-30)
 
 
 def test_layernorm_bwd_without_dres(dev):
@@ -202,8 +175,9 @@ def test_layernorm_bwd_without_dres(dev):
         ex = R.layernorm_bwd_ref(dy, x, gamma, mean, rstd)
         per_row(tag, "dx", dx.check(tag), ex["dx"], R.bf(ex["dx"]))
         nterm = rows + (rows + 7) // 8 + 16
-        bounded(tag, "dgamma", dgam, g0[0].double() + ex["dgamma"], nterm * U * (ex["abs_dgamma"] + g0[0].double().abs()))
-        bounded(tag, "dbeta", dbet, g0[1].double() + ex["dbeta"], nterm * U * (ex["abs_dbeta"] + g0[1].double().abs()))
+        within(REPORT, f"{tag}: dgamma", dgam, g0[0].double() + ex["dgamma"],
+               nterm * U * (ex["abs_dgamma"] + g0[0].double().abs()))
+        within(REPORT, f"{tag}: dbeta", dbet, g0[1].double() + ex["dbeta"], nterm * U * (ex["abs_dbeta"] + g0[1].double().abs()))
 
 
 def test_layernorm_row_statistics(dev):
@@ -231,7 +205,7 @@ def test_layernorm_row_statistics(dev):
         e = gamma.double().abs() * ((tol_mean * ex["rstd"])[:, None] + xh * rel[:, None]) + 4 * U * ex["y"].abs()
         if yd == bf16:
             e = e + R.ulp_bf16(ex["y"].abs() + e)
-        bounded(tag, "y", y, ex["y"], e + 1e-30)
+        within(REPORT, f"{tag}: y", y, ex["y"], e + 1e-30)
 
 
 @pytest.mark.parametrize("xd", [bf16, f32], ids=["x-bf16", "x-fp32"])
@@ -277,7 +251,7 @@ def test_layernorm_row_maps(dev, xd):
         b = R.layernorm_bwd_ref(dy, xr, gamma, st, rs)
         per_row(tag, "dx", dx.check(f"{tag}: dx"), b["dx"], R.bf(b["dx"]))
         nterm = rows + 32
-        bounded(tag, "dgamma", dgam, b["dgamma"], nterm * U * b["abs_dgamma"] + 1e-30)
+        within(REPORT, f"{tag}: dgamma", dgam, b["dgamma"], nterm * U * b["abs_dgamma"] + 1e-30)
 
 
 @pytest.mark.parametrize("C", [1032, 2048, 2056, 4096])
@@ -304,8 +278,8 @@ def test_layernorm_wide(dev, C):
     b = R.layernorm_bwd_ref(dy, x, gamma, m, r)
     per_row(tag, "dx", dx.check(f"{tag}: dx"), b["dx"], R.bf(b["dx"]))
     nterm = rows + 32
-    bounded(tag, "dgamma", dgam, g0[0].double() + b["dgamma"], nterm * U * (b["abs_dgamma"] + g0[0].double().abs()))
-    bounded(tag, "dbeta", dbet, g0[1].double() + b["dbeta"], nterm * U * (b["abs_dbeta"] + g0[1].double().abs()))
+    within(REPORT, f"{tag}: dgamma", dgam, g0[0].double() + b["dgamma"], nterm * U * (b["abs_dgamma"] + g0[0].double().abs()))
+    within(REPORT, f"{tag}: dbeta", dbet, g0[1].double() + b["dbeta"], nterm * U * (b["abs_dbeta"] + g0[1].double().abs()))
 
 
 # ==================================================================================== small row kernels
@@ -343,7 +317,7 @@ def test_colsum_strided_scaled_accumulating(dev):
         torch.cuda.synchronize()
         assert torch.equal(out[C:], c0[C:]), "colsum wrote past C"
         ex, ab = R.colsum_ref(x, -0.5)
-        bounded(f"colsum rows{rows} C{C} ld{ld}", "out", out[:C], c0[:C].double() + ex,
+        within(REPORT, f"colsum rows{rows} C{C} ld{ld}: out", out[:C], c0[:C].double() + ex,
                 (rows + 32) * U * (ab + c0[:C].double().abs()) + 1e-30)
 
 
@@ -372,7 +346,7 @@ def test_cast_bf16_tail(dev, n):
     ops = _ops()
     src = (torch.randn(n, generator=_gen(n)) * 100).to(dev)
     dst = torch.empty(n + 24, dtype=bf16, device=dev)
-    dst.view(torch.int16).fill_(_PATTERN[bf16])
+    dst.view(torch.int16).fill_(DTYPES[bf16][1])
     dst[:n] = float("nan")
     snap = dst.view(torch.int16).clone()
     ops.cast_bf16(src, dst)
@@ -393,8 +367,8 @@ def test_l2norm_fwd_bwd_elementwise(dev, C):
     ref = R.l2norm_ref(x)
     k = (C / 32 + 16) * U
     yk, ik = y.check("l2norm y"), inv.check("l2norm inv_norm")[:, 0]
-    bounded(f"l2norm C{C}", "y", yk, ref["y"], k * ref["y"].abs() + 1e-30)
-    bounded(f"l2norm C{C}", "inv_norm", ik, ref["inv_norm"], k * ref["inv_norm"])
+    within(REPORT, f"l2norm C{C}: y", yk, ref["y"], k * ref["y"].abs() + 1e-30)
+    within(REPORT, f"l2norm C{C}: inv_norm", ik, ref["inv_norm"], k * ref["inv_norm"])
     dy = torch.randn(rows, C, generator=g).to(dev)
     dx = Rows(dev, rows, C, bf16)
     ops.l2norm_bwd(dy, yk.contiguous(), ik.contiguous(), dx.buf[:rows], scale=0.5)
@@ -402,4 +376,4 @@ def test_l2norm_fwd_bwd_elementwise(dev, C):
     ex = R.l2norm_bwd_ref(dy, yk, ik, scale=0.5)
     yd, dyd = yk.double(), dy.double()
     e = 0.5 * ik.double()[:, None] * (yd.abs() * k * (dyd * yd).abs().sum(-1, keepdim=True) + 4 * U * (dyd.abs() + ex.abs()))
-    bounded(f"l2norm bwd C{C}", "dx", dx.check("l2norm dx"), ex, e + R.ulp_bf16(ex.abs() + e))
+    within(REPORT, f"l2norm bwd C{C}: dx", dx.check("l2norm dx"), ex, e + R.ulp_bf16(ex.abs() + e))

@@ -4,6 +4,7 @@ import os
 import pytest
 import torch
 
+from encoder_cases import swin3d_case
 from oracle import swin3d_oracle as SO
 
 pytestmark = pytest.mark.gpu
@@ -177,8 +178,7 @@ def test_training_mode_draws_the_references_rng_stream(dev):
 def test_released_config_one_sample_against_fp32_oracle_on_gpu(dev):
     """The released VideoEncoder config (6 stages, dims 128..1024, windows up to 32 x 3 x 5), 1 x 32 frames x 96 x 160:
     the output and every parameter gradient within 1.5 x the bf16 oracle's error of the fp32 oracle, whole and per slice
-    (test_gpu_encoder_calibration.swin3d_case); and the earlier fixed thresholds on top."""
-    from test_gpu_encoder_calibration import swin3d_case
+    (encoder_cases.swin3d_case); and the earlier fixed thresholds on top."""
     (out, _, grads), (ref, _, ref_grads) = swin3d_case(dev, "swin released_1x32x96x160", SO.Swin3DCfg(), 1, 32, 96, 160,
                                                        weight_seed=4, data_seed=5, branches={"colsum"})
     assert _rel(out, ref) < 3e-2

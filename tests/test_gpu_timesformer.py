@@ -5,6 +5,7 @@ import os
 import pytest
 import torch
 
+from encoder_cases import timesformer_case
 from oracle import timesformer_oracle as TO
 
 pytestmark = pytest.mark.gpu
@@ -158,8 +159,7 @@ def test_module_matches_reference_golden(dev, golden_dir, name):
 def test_full_width_block_against_fp32_oracle_on_gpu(dev):
     """dim 1024 / 16 heads / native 10x16 grid, 7 frames (the reference shape), depth 2: the output, dx and every
     parameter gradient within 1.5 x the bf16 oracle's error of the fp32 oracle, whole and per slice
-    (test_gpu_encoder_calibration.timesformer_case); and the earlier fixed thresholds on top."""
-    from test_gpu_encoder_calibration import timesformer_case
+    (encoder_cases.timesformer_case); and the earlier fixed thresholds on top."""
     (out, dx, grads), (ref, ref_dx, ref_grads) = timesformer_case(dev, "tsf full_width_7x10x16", TO.TimeSformerCfg(depth=2),
                                                                    2, 7, 10, 16, weight_seed=3, data_seed=4)
     assert _rel(out, ref) < 1.5e-2

@@ -16,18 +16,17 @@ import os
 import pytest
 import torch
 
+from contract_harness import ABS_FLOOR, Out, Report, calibrated, calibrated_model_rows, lse_check, same_bits
 from oracle import timesformer_oracle as TO
 from oracle import timesformer_variants_oracle as V
 from oracle.dense_attention_ref import dense_ref
-import test_gpu_attention_contract as AC
-from test_gpu_attention_contract import Out, calibrated, lse_check, same_bits
 
 pytestmark = pytest.mark.gpu
 
 bf16, f32 = torch.bfloat16, torch.float32
-FACTOR = 1.5
 QS64 = 0.125
 GOLDENS = ["timesformer_joint_interp_b2", "timesformer_joint_native_train", "timesformer_space_only_t1"]
+REPORT = Report("dense attention: worst slice ratio err(kernel) / err(bf16 arm), LSE: worst relative error")
 
 
 @pytest.fixture(scope="module")
@@ -35,6 +34,12 @@ def dev():
     if not torch.cuda.is_available():
         pytest.skip("needs an H100")
     return torch.device("cuda", 0)
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield
+    REPORT.print()
 
 
 def _ops():
@@ -68,35 +73,6 @@ def _oracle_run(sd, x, w_out, cfg, kind, masks, mode):
         out = V.timesformer_forward(sdo, xo, cfg, kind, drop_masks=m).float()
     (out * w_out).sum().backward()
     return out.detach(), xo.grad, {n: p.grad for n, p in sdo.items() if p.grad is not None}
-
-
-def calibrated_model_rows(tag, rows, slices=None):
-    """The calibrated rule on whole tensors and, optionally, on slices of them.
-
-    rows: (name, ours, fp32 oracle, bf16 arm, autocast run or None) per tensor.  Whole tensor: err(ours) <= 1.5 x err(arm)
-    (+1e-7), both relative L2 against the fp32 oracle.  slices: name -> (ids, label) for test_gpu_attention_contract's
-    `calibrated` (per slice, with its floor of 2^-16 x the slice's norm).  Returns (violations, worst whole-tensor ratio,
-    worst slice ratio), each ratio a (value, tensor name) pair; the autocast ratio is printed, never asserted."""
-    bad = []
-    worst, worst_ac, worst_sl = (0.0, ""), (0.0, ""), (0.0, "")
-    for name, got, ref, a, c in rows:
-        e, ea = _rel(got, ref), _rel(a, ref)
-        worst = max(worst, (e / (ea + 1e-7), name))
-        if c is not None:
-            worst_ac = max(worst_ac, (e / (_rel(c, ref) + 1e-7), name))
-        if e > FACTOR * ea + 1e-7:
-            bad.append(f"{tag}: {name}: error {e:.3e} vs the bf16 oracle's {ea:.3e}")
-        if slices and name in slices:
-            ids, label = slices[name]
-            try:
-                calibrated(tag, name, got, ref, a, ids, label)
-            except AssertionError as err:
-                bad.append(str(err))
-            worst_sl = max(worst_sl, (AC.REPORT[f"{tag}: {name}"], name))
-    print(f"{tag}: worst err / bf16-oracle err {worst[0]:.3f} ({worst[1]})"
-          + (f", worst slice {worst_sl[0]:.3f} ({worst_sl[1]})" if slices else "")
-          + (f"; worst err / autocast err {worst_ac[0]:.2f} ({worst_ac[1]})" if worst_ac[1] else ""))
-    return bad, worst, worst_sl
 
 
 def _calibrated_model_check(tag, model, x, w_out, cfg, kind, sd, masks):
@@ -240,8 +216,8 @@ def test_dense_attention_calibrated(dev, n_seq, L, H, extra, pad):
     out, lse = dense_fwd(dev, qkv, n_seq, L, H, ld_out)
     out2, lse2 = dense_fwd(dev, qkv, n_seq, L, H, ld_out)
     assert same_bits(out, out2) and same_bits(lse, lse2), f"{tag}: forward not bitwise repeatable"
-    calibrated(tag, "out", out, ex["out"][:n], arm["out"][:n], idc, label)
-    lse_check(tag, lse, ex["lse"][:, :n])
+    calibrated(REPORT, f"{tag}: out", out, ex["out"][:n], arm["out"][:n], idc, label, ABS_FLOOR)
+    lse_check(REPORT, tag, lse, ex["lse"][:, :n])
     # the backward reads the exact forward, rounded as the kernel stores it
     out_in, lse_in = ex["out"][:n].to(bf16), ex["lse"][:, :n].float()
     dqkv = dense_bwd(dev, qkv, out_in, dout, lse_in, n_seq, L, H)
@@ -249,7 +225,7 @@ def test_dense_attention_calibrated(dev, n_seq, L, H, extra, pad):
     assert same_bits(dqkv, dqkv2), f"{tag}: backward not bitwise repeatable"
     for j, nm in enumerate(("dq", "dk", "dv")):
         cs = slice(j * C, (j + 1) * C)
-        calibrated(tag, nm, dqkv[:, cs], ex["dqkv"][:n, cs], arm["dqkv"][:n, cs], idc, label)
+        calibrated(REPORT, f"{tag}: {nm}", dqkv[:, cs], ex["dqkv"][:n, cs], arm["dqkv"][:n, cs], idc, label, ABS_FLOOR)
 
 
 @pytest.mark.parametrize("L", [63, 65, 392])

@@ -13,8 +13,8 @@ The B*T grid limit (65535 runs, 65536 refused before any launch) is tested in te
 import pytest
 import torch
 
+from contract_harness import Guarded, same_bits
 from oracle import embed_ref as E
-from test_gpu_embed_contract import Guarded, same_bits
 
 pytestmark = pytest.mark.gpu
 
