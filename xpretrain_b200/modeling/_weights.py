@@ -6,6 +6,9 @@ including the ones autograd's version counter does not see: `p.data.addcdiv_` in
 the next forward.  A cache keyed on `p._version` breaks that contract (VERDICT r1 / ADVICE r1), so there is no cache
 validity test at all: the cast is 6 B per parameter (~0.15 ms for the 150 M parameters of CLIP-ViP) and simply runs.
 Only the device-side pointer table is cached, keyed on the data pointers.
+
+Two layouts of the copies use this: CLIP-ViP's `_WeightPack` (q/k/v fused per layer, modeling/clip_vip.py) and the
+named-weight cache below (one copy per GEMM weight, `model._cache[name]`) of TimeSformer and Swin-3D.
 """
 from __future__ import annotations
 
@@ -51,3 +54,23 @@ class WeightMirror:
         tab = self._table
         check(lib().xp_cast_table(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks,
                                   torch.cuda.current_stream().cuda_stream), "xp_cast_table")
+
+
+def refresh_weights(model) -> None:
+    """Re-cast every GEMM weight (parameters with >= 2 dims that `weight` serves) of `model` into `model._cache` with ONE
+    launch on every forward."""
+    cache = model._cache
+    named = [(n, p) for n, p in model.named_parameters() if p.dim() >= 2 and n.endswith("weight")]
+    dev = named[0][1].device
+    if cache.get("__device__") != dev:
+        cache.clear()
+        cache["__device__"] = dev
+        cache["__mirror__"] = WeightMirror()
+        for n, p in named:
+            cache[n] = torch.empty(p.shape, dtype=bf16, device=dev)
+    cache["__mirror__"].refresh([(p, cache[n]) for n, p in named])
+
+
+def weight(model, name: str) -> torch.Tensor:
+    """bf16 compute copy of the GEMM weight `name` (refreshed for the whole model at the start of every forward)."""
+    return model._cache[name]

@@ -28,6 +28,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib, ops
+from ._blocks import alloc_flat
 from ._weights import WeightMirror
 
 bf16, f32 = torch.bfloat16, torch.float32
@@ -317,7 +318,7 @@ def _pack(model: CLIPModel, which: str) -> _WeightPack:
     return model._packs[which]
 
 
-def _small_bf16(model: CLIPModel, name: str, p: torch.Tensor) -> torch.Tensor:
+def _small_bf16(model: CLIPModel, name: str) -> torch.Tensor:
     return model._packs["small:" + name]
 
 
@@ -473,19 +474,6 @@ def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch
     return dxin
 
 
-def _alloc_flat(shapes: Dict[str, tuple], grads: Dict[str, torch.Tensor], dev) -> torch.Tensor:
-    """One zeroed fp32 buffer holding all gradients of a group as 16-byte aligned views: the data-parallel
-    all-reduce of the group is then a single collective on `flat` (no packing copies)."""
-    offs, total = {}, 0
-    for n, shp in shapes.items():
-        offs[n] = total
-        total += (int(torch.Size(shp).numel()) + 3) // 4 * 4
-    flat = torch.zeros(total, dtype=f32, device=dev)
-    for n, shp in shapes.items():
-        grads[n] = flat[offs[n]:offs[n] + torch.Size(shp).numel()].view(shp)
-    return flat
-
-
 def _alloc_layer_grads(layer, prefix: str, grads: Dict[str, torch.Tensor], dev) -> torch.Tensor:
     C_ = layer.self_attn.q_proj.weight.shape[0]
     shapes = {prefix + "self_attn.qkv.weight": (3 * C_, C_), prefix + "self_attn.qkv.bias": (3 * C_,)}
@@ -493,7 +481,7 @@ def _alloc_layer_grads(layer, prefix: str, grads: Dict[str, torch.Tensor], dev) 
         if ".q_proj." in n or ".k_proj." in n or ".v_proj." in n:
             continue
         shapes[prefix + n] = tuple(p.shape)
-    return _alloc_flat(shapes, grads, dev)
+    return alloc_flat(shapes, grads, dev)
 
 
 def _grads_ready(model, grads: Dict[str, torch.Tensor], key: str) -> None:
@@ -514,7 +502,7 @@ def _finish_layer_grads(prefix: str, grads: Dict[str, torch.Tensor], C_: int):
         grads[prefix + f"self_attn.{n}.bias"] = b[j * C_:(j + 1) * C_]
 
 
-# ------------------------------------------------------------------------------ vision tower
+# ------------------------------------------------------------------------------ encoder stack
 def _block_saved(sv, i: int):
     """Block i's saved tensors for its backward, released from `sv`.  A checkpointed tower kept only the block's input:
     rebuild the rest now by rerunning the block's forward kernels from it, on the stream and under the SM limit of the backward."""
@@ -522,6 +510,72 @@ def _block_saved(sv, i: int):
     return s if sv.recompute is None else sv.recompute(i, s)
 
 
+def _encoder_fwd(model: CLIPModel, tower: str, pool_ln: str, pk: _WeightPack, x_in: list, rows: int, B: int, attn_fwd,
+                 pool_rows, wproj, save: bool, ckpt: bool, stream_dt, timer=None):
+    """A tower's encoder layers, then its pooled LayerNorm (`pool_ln`) of the B rows picked by the row map `pool_rows()`
+    returns after the layers, and the projection `wproj`.  x_in: a list holding the only reference to the embedded rows, so
+    that layer 0 releases them unless it saves them.  ckpt (with save): keep each block's input only; `recompute` rebuilds
+    the rest per block in the backward.  timer: a list receiving ("fwd", start, end) CUDA events around each block.
+    Returns (proj fp32 [B, projection_dim], saved): saved (None without `save`) holds what _encoder_bwd reads."""
+    eps = model.config.layer_norm_eps
+    tw = getattr(model, tower)
+    layers = tw.encoder.layers
+    x = x_in.pop()
+    layer_saved = []
+    pend = None
+    for i, layer in enumerate(layers):
+        if timer is not None:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
+        if timer is not None:
+            e1.record()
+            timer.append(("fwd", e0, e1))
+        layer_saved.append(sv)
+    rmap = pool_rows()
+    pooled, meanp, rstdp, post_in = _pooled_ln(x, pend, rmap, getattr(tw, pool_ln), B, pk.C, eps)
+    proj = torch.empty(B, model.config.projection_dim, dtype=f32, device=x.device)
+    ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
+    if not save:
+        return proj, None
+    recompute = None
+    if ckpt:
+        def recompute(i, xin):
+            return _layer_fwd(xin, None, layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
+    return proj, SimpleNamespace(B=B, rows=rows, layers=layer_saved, x_last=(x, pend), pool_map=rmap, post_in=post_in,
+                                 pooled=pooled, meanp=meanp, rstdp=rstdp, recompute=recompute)
+
+
+def _encoder_bwd(model: CLIPModel, tower: str, pool_ln: str, proj: str, pk: _WeightPack, sv, dproj_bf16, grads, wproj,
+                 attn_bwd, aux=None, timer=None):
+    """Backward of _encoder_fwd from dproj_bf16 [B, proj] (the gradient of the un-normalised projection output): the
+    projection, the pooled LayerNorm, then the layers in reverse, each handing its finished gradient group to
+    `_grads_ready`.  aux: the stream of the layers' bias column sums (_colsum); timer: ("bwd", start, end) events per block.
+    Returns the gradient of the embedded rows [rows, C] bf16."""
+    tw = getattr(model, tower)
+    C_, B, rows = pk.C, sv.B, sv.rows
+    dev = dproj_bf16.device
+    ops.linear_wgrad(dproj_bf16, sv.pooled, grads[proj + ".weight"])
+    dpooled = torch.empty(B, C_, dtype=bf16, device=dev)
+    ops.linear_dgrad(dproj_bf16, wproj, dpooled)
+    dx = torch.zeros(rows, C_, dtype=bf16, device=dev)  # only the pooled rows receive gradient from the head
+    ln = f"{tower}.{pool_ln}."
+    ops.layernorm_bwd(dpooled, ops.rowmap(C_), sv.post_in[0], sv.post_in[1], getattr(tw, pool_ln).weight, sv.meanp, sv.rstdp,
+                      None, None, dx, sv.pool_map, grads[ln + "weight"], grads[ln + "bias"], B, C_)
+    for i in reversed(range(len(tw.encoder.layers))):
+        prefix = f"{tower}.encoder.layers.{i}."
+        if timer is not None:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        dx = _layer_bwd(dx, _block_saved(sv, i), tw.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows, aux)
+        if timer is not None:
+            e1.record()
+            timer.append(("bwd", e0, e1))
+        _grads_ready(model, grads, prefix)
+    return dx
+
+
+# ------------------------------------------------------------------------------ vision tower
 def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = False):
     """ckpt (with save): keep each block's input only (gradient checkpointing); the backward rebuilds the rest per block.
     The per-frame model folds the frames into the batch (CLIP.py sees [B*T, 3, H, W]): B*T sequences of one frame and one
@@ -559,7 +613,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     added = None if cfg.per_frame else emb.added_cls       # M = 1: the kernel reads no added_cls row
     ops.vip_embed_tables(emb.position_embedding.weight, temporal, emb.class_embedding, added, table, x0, B, T, L,
                          M, C_, cfg.temporal_size)
-    wp = _small_bf16(model, "patch", emb.patch_embedding.weight).view(C_, Kp)
+    wp = _small_bf16(model, "patch").view(C_, Kp)
     if ldp != Kp:   # e.g. p = 14: the GEMM's B operand needs the same 16-byte row pitch as the patch matrix
         wpad = model._packs.get("pad:patch")
         if wpad is None or wpad.shape != (C_, ldp) or wpad.device != dev:
@@ -569,7 +623,6 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     # conv-as-GEMM; epilogue adds the periodic [T*L, C] position+temporal table and writes past the M global rows
     ops.gemm(patches, wp, x0, M=B * T * L, N=C_, K=Kp, lda=ldp, ldb=ldp, ldc=C_, residual=table, ldr=C_, r_group=T * L,
              r_group_stride=0, c_group=T * L, c_group_stride=S * C_, c_offset=M * C_)
-    plain = ops.rowmap(C_)
     # pre_layrnorm (CLIP_ViP.py:881) in two launches so that its statistics are stored compactly per half
     # (patch rows / global rows), the layout its backward and the embedding backward consume
     pmap = ops.rowmap(C_, group=T * L, group_stride=S * C_)
@@ -582,6 +635,8 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     ops.layernorm_fwd(x0, pmap, x, pmap, ln0.weight, ln0.bias, mean0p, rstd0p, B * T * L, C_, eps, x_off=M * C_,
                       y_off=M * C_)
     ops.layernorm_fwd(x0, gmap, x, gmap, ln0.weight, ln0.bias, mean0g, rstd0g, B * M, C_, eps)
+    x_in = [x]
+    del x
 
     ws = ops.vip_attention_workspace(B, H, T, M, dev)
 
@@ -590,33 +645,13 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
         ops.vip_attention_fwd(qkv, out, lse, ws, B, H, T, L, M, C_)
         return lse
 
-    layer_saved = []
-    pend = None
-    timer = getattr(model, "block_timer", None)   # bench.py: CUDA events around each ViP block (metric 2 of BASELINE.json)
-    for i, layer in enumerate(vm.encoder.layers):
-        if timer is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
-        if timer is not None:
-            e1.record()
-            timer.append(("fwd", e0, e1))
-        layer_saved.append(sv)
     # pooled = post_layernorm(last_hidden[:, 0])  (CLIP_ViP.py:891-893): CLS rows picked by the row map
-    cls_map = ops.rowmap(C_, group=1, group_stride=S * C_)
-    pooled, meanp, rstdp, post_in = _pooled_ln(x, pend, cls_map, vm.post_layernorm, B, C_, eps)
-    wproj = _small_bf16(model, "vproj", model.visual_projection.weight)
-    proj = torch.empty(B, cfg.projection_dim, dtype=f32, device=dev)
-    ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
-    saved = None
-    if save:
-        recompute = None
-        if ckpt:
-            def recompute(i, xin):
-                return _layer_fwd(xin, None, vm.encoder.layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
-        saved = SimpleNamespace(B=B, T=T, S=S, rows=rows, patches=patches, x0=x0, stats0=(mean0p, rstd0p, mean0g, rstd0g),
-                                layers=layer_saved, x_last=(x, pend), post_in=post_in, pooled=pooled, meanp=meanp, rstdp=rstdp,
-                                ws=ws, recompute=recompute)
+    proj, saved = _encoder_fwd(model, "vision_model", "post_layernorm", pk, x_in, rows, B, attn_fwd,
+                               lambda: ops.rowmap(C_, group=1, group_stride=S * C_), _small_bf16(model, "vproj"), save,
+                               ckpt, stream_dt, timer=getattr(model, "block_timer", None))  # bench.py: metric 2 of BASELINE.json
+    if saved is not None:
+        saved.T, saved.S, saved.patches, saved.x0, saved.ws = T, S, patches, x0, ws
+        saved.stats0 = (mean0p, rstd0p, mean0g, rstd0g)
     return proj, saved
 
 
@@ -626,34 +661,17 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
     vm = model.vision_model
     C_, L, M = cfg.vision.hidden_size, cfg.num_patches, cfg.num_global_tokens
     H = cfg.vision.num_attention_heads
-    B, T, S, rows = sv.B, sv.T, sv.S, sv.rows
+    B, T, S = sv.B, sv.T, sv.S
     dev = dproj_bf16.device
     pk = _pack(model, "vision")
     plain = ops.rowmap(C_)
-    wproj = _small_bf16(model, "vproj", model.visual_projection.weight)
-    ops.linear_wgrad(dproj_bf16, sv.pooled, grads["visual_projection.weight"])
-    dpooled = torch.empty(B, C_, dtype=bf16, device=dev)
-    ops.linear_dgrad(dproj_bf16, wproj, dpooled)
-    dx = torch.zeros(rows, C_, dtype=bf16, device=dev)  # only the CLS rows receive gradient from the head
-    cls_map = ops.rowmap(C_, group=1, group_stride=S * C_)
-    ops.layernorm_bwd(dpooled, plain, sv.post_in[0], sv.post_in[1], vm.post_layernorm.weight, sv.meanp, sv.rstdp, None, None,
-                      dx, cls_map, grads["vision_model.post_layernorm.weight"], grads["vision_model.post_layernorm.bias"], B, C_)
 
     def attn_bwd(qkv, a, da, lse, dqkv):
         ops.vip_attention_bwd(qkv, a, da, lse, dqkv, sv.ws, B, H, T, L, M, C_, pk.q_scale)
 
-    timer = getattr(model, "block_timer", None)
-    aux = _aux_stream(model, dev)
-    for i in reversed(range(len(vm.encoder.layers))):
-        prefix = f"vision_model.encoder.layers.{i}."
-        if timer is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        dx = _layer_bwd(dx, _block_saved(sv, i), vm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows, aux)
-        if timer is not None:
-            e1.record()
-            timer.append(("bwd", e0, e1))
-        _grads_ready(model, grads, prefix)
+    dx = _encoder_bwd(model, "vision_model", "post_layernorm", "visual_projection", pk, sv, dproj_bf16, grads,
+                      _small_bf16(model, "vproj"), attn_bwd, aux=_overlap_stream(model, dev, "overlap_colsum"),
+                      timer=getattr(model, "block_timer", None))
     # pre_layrnorm backward, written as two compact halves: patch rows [B, T*L, C] and global rows [B, M, C]
     d_patch = torch.empty(B * T * L, C_, dtype=bf16, device=dev)
     d_glob = torch.empty(B * M, C_, dtype=bf16, device=dev)
@@ -682,20 +700,18 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
 def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor], save: bool,
               ckpt: bool = False):
     cfg = model.config
-    tm = model.text_model
     B, Lt = input_ids.shape
     C_, H = cfg.text.hidden_size, cfg.text.num_attention_heads
     rows = B * Lt
     dev = input_ids.device
-    pk = _pack(model, "text")
-    eps = cfg.layer_norm_eps
+    te = model.text_model.embeddings
     if Lt > cfg.max_position_embeddings:      # the reference fails in position_ids[:, :seq_length] + embedding add (CLIP_ViP.py:217-225)
         raise ValueError(f"text length {Lt} exceeds max_position_embeddings {cfg.max_position_embeddings}")
     ids = input_ids.contiguous().to(torch.int64)
     mask = attention_mask.contiguous().to(torch.int64) if attention_mask is not None else None
     x = torch.empty(rows, C_, dtype=bf16, device=dev)
     err = torch.zeros(1, dtype=torch.int32, device=dev)
-    ops.text_embed_fwd(ids, tm.embeddings.token_embedding.weight, tm.embeddings.position_embedding.weight, x, Lt, err)
+    ops.text_embed_fwd(ids, te.token_embedding.weight, te.position_embedding.weight, x, Lt, err)
     if getattr(model, "validate_ids", False) and int(err.item()) != 0:   # opt-in: costs a device sync per forward
         raise IndexError("text_input_ids contains a token id outside [0, vocab_size) (nn.Embedding would raise, CLIP_ViP.py:222)")
 
@@ -704,58 +720,37 @@ def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optiona
         ops.text_attention_fwd(qkv, mask, out, probs, B, H, Lt, C_)
         return probs
 
-    layer_saved = []
-    pend = None
     stream_dt = _stream_dtype(model) if _residual_fp32(model) else None
     if stream_dt is not None:
         x = x.to(stream_dt)          # [B*Lt, 512]: the token + position embeddings enter the stream in its storage type
-    for i, layer in enumerate(tm.encoder.layers):
-        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
-        layer_saved.append(sv)
-    # final_layer_norm is per-row, so it is applied to the pooled EOS row only (first argmax of the ids, :776)
-    eos = torch.empty(B, dtype=torch.int64, device=dev)
-    ops.eos_offsets(ids, eos, None, C_)
-    plain = ops.rowmap(C_)
-    emap = ops.rowmap(C_, offsets=eos)
-    pooled, meanp, rstdp, post_in = _pooled_ln(x, pend, emap, tm.final_layer_norm, B, C_, eps)
-    wproj = _small_bf16(model, "tproj", model.text_projection.weight)
-    proj = torch.empty(B, cfg.projection_dim, dtype=f32, device=dev)
-    ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
-    saved = None
-    if save:
-        recompute = None
-        if ckpt:
-            def recompute(i, xin):
-                return _layer_fwd(xin, None, tm.encoder.layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
-        saved = SimpleNamespace(B=B, Lt=Lt, rows=rows, ids=ids, layers=layer_saved, x_last=(x, pend), post_in=post_in, eos=eos,
-                                pooled=pooled, meanp=meanp, rstdp=rstdp, err=err, recompute=recompute)
+    x_in = [x]
+    del x
+    eos = None
+
+    def eos_rows():     # final_layer_norm is per-row, so it is applied to the pooled EOS row only (first argmax of the ids, :776)
+        nonlocal eos
+        eos = torch.empty(B, dtype=torch.int64, device=dev)
+        ops.eos_offsets(ids, eos, None, C_)
+        return ops.rowmap(C_, offsets=eos)
+
+    proj, saved = _encoder_fwd(model, "text_model", "final_layer_norm", _pack(model, "text"), x_in, rows, B, attn_fwd,
+                               eos_rows, _small_bf16(model, "tproj"), save, ckpt, stream_dt)
+    if saved is not None:
+        saved.Lt, saved.ids, saved.eos, saved.err = Lt, ids, eos, err
     return proj, saved
 
 
 def _text_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, torch.Tensor]):
     cfg = model.config
-    tm = model.text_model
     C_, H = cfg.text.hidden_size, cfg.text.num_attention_heads
-    B, Lt, rows = sv.B, sv.Lt, sv.rows
-    dev = dproj_bf16.device
+    B, Lt = sv.B, sv.Lt
     pk = _pack(model, "text")
-    plain = ops.rowmap(C_)
-    wproj = _small_bf16(model, "tproj", model.text_projection.weight)
-    ops.linear_wgrad(dproj_bf16, sv.pooled, grads["text_projection.weight"])
-    dpooled = torch.empty(B, C_, dtype=bf16, device=dev)
-    ops.linear_dgrad(dproj_bf16, wproj, dpooled)
-    dx = torch.zeros(rows, C_, dtype=bf16, device=dev)
-    emap = ops.rowmap(C_, offsets=sv.eos)
-    ops.layernorm_bwd(dpooled, plain, sv.post_in[0], sv.post_in[1], tm.final_layer_norm.weight, sv.meanp, sv.rstdp, None, None,
-                      dx, emap, grads["text_model.final_layer_norm.weight"], grads["text_model.final_layer_norm.bias"], B, C_)
 
     def attn_bwd(qkv, a, da, probs, dqkv):
         ops.text_attention_bwd(qkv, da, probs, dqkv, B, H, Lt, C_, pk.q_scale)
 
-    for i in reversed(range(len(tm.encoder.layers))):
-        prefix = f"text_model.encoder.layers.{i}."
-        dx = _layer_bwd(dx, _block_saved(sv, i), tm.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows)
-        _grads_ready(model, grads, prefix)
+    dx = _encoder_bwd(model, "text_model", "final_layer_norm", "text_projection", pk, sv, dproj_bf16, grads,
+                      _small_bf16(model, "tproj"), attn_bwd)
     ops.text_embed_bwd(sv.ids, dx, grads["text_model.embeddings.token_embedding.weight"],
                        grads["text_model.embeddings.position_embedding.weight"], Lt, C_, cfg.vocab_size)
 
@@ -807,7 +802,7 @@ class _ClipVipFunction(torch.autograd.Function):
             return feat
 
         none = torch.empty(0, device=dev)
-        side = _side_stream(model, dev) if (video is not None and input_ids is not None) else None
+        side = _overlap_stream(model, dev, "overlap_text_tower") if (video is not None and input_ids is not None) else None
         ctx.side = side
         if side is None:
             vis = run_tower("vis") if video is not None else none
@@ -878,7 +873,7 @@ def _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, nam
         grads["__flat__" + pre] = _alloc_layer_grads(layer, pre, grads, dev)
     rest = {n: tuple(named[n].shape) for n in names if n.startswith(tower + ".") and ".encoder.layers." not in n}
     rest[proj_name] = tuple(named[proj_name].shape)
-    grads["__flat__" + tower] = _alloc_flat(rest, grads, dev)
+    grads["__flat__" + tower] = alloc_flat(rest, grads, dev)
     pool = getattr(sv, "pool", None)
     if pool is not None:        # frame-mean head: d(video feature) [B, P] -> d(frame projections) [B*T, P]
         proj, pool_t = pool
@@ -897,25 +892,16 @@ def _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, nam
         _finish_layer_grads(f"{tower}.encoder.layers.{i}.", grads, C_)
 
 
-def _side_stream(model: CLIPModel, dev):
-    """Side stream for the text tower (None when `model.overlap_text_tower` is False or XP_NO_OVERLAP=1)."""
+def _overlap_stream(model: CLIPModel, dev, option: str):
+    """The model's stream for one overlap, created once per device: `option` "overlap_text_tower" runs the text tower on it
+    under the vision tower, "overlap_colsum" the HBM-bound bias column sums of the vision backward under its GEMMs.  None
+    when `model.<option>` is False or XP_NO_OVERLAP=1."""
     import os
-    if not getattr(model, "overlap_text_tower", True) or os.environ.get("XP_NO_OVERLAP") == "1":
+    if not getattr(model, option, True) or os.environ.get("XP_NO_OVERLAP") == "1":
         return None
-    st = model._packs.get("side_stream")
+    st = model._packs.get(option)
     if st is None or st.device != dev:
-        st = model._packs["side_stream"] = torch.cuda.Stream(device=dev)
-    return st
-
-
-def _aux_stream(model: CLIPModel, dev):
-    """Stream for the HBM-bound bias column sums of the vision backward (None: XP_NO_OVERLAP=1 / model.overlap_colsum False)."""
-    import os
-    if not getattr(model, "overlap_colsum", True) or os.environ.get("XP_NO_OVERLAP") == "1":
-        return None
-    st = model._packs.get("aux_stream")
-    if st is None or st.device != dev:
-        st = model._packs["aux_stream"] = torch.cuda.Stream(device=dev)
+        st = model._packs[option] = torch.cuda.Stream(device=dev)
     return st
 
 

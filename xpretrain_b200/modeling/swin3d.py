@@ -26,15 +26,15 @@ from __future__ import annotations
 
 from functools import reduce
 from operator import mul
-from typing import Dict, List
+from typing import Dict, List, NamedTuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib, ops
-from .clip_vip import _alloc_flat
-from .timesformer import _linear_bwd, _w, refresh_weights
+from ._blocks import alloc_flat, drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd, residual_linear
+from ._weights import refresh_weights, weight
 
 bf16, f32 = torch.bfloat16, torch.float32
 HEAD_DIM = 32
@@ -250,18 +250,21 @@ def _merge_index(model: SwinTransformer3D, B: int, D: int, H: int, W: int, devic
     return ent
 
 
-def _ln_any(x, ln: nn.LayerNorm, rows: int, C_: int, eps: float, out=None):
-    mean = torch.empty(rows, dtype=f32, device=x.device)
-    rstd = torch.empty_like(mean)
-    y = torch.empty(rows, C_, dtype=bf16, device=x.device) if out is None else out
-    ops.layernorm_any_fwd(x, y, ln.weight, ln.bias, mean, rstd, rows, C_, eps)
-    return y, mean, rstd
-
-
 # --------------------------------------------------------------------------------------------- blocks
+class _WindowSaved(NamedTuple):
+    x: torch.Tensor          # LayerNorm-1 input [n_real, C]
+    mean: torch.Tensor
+    rstd: torch.Tensor
+    h: torch.Tensor          # LayerNorm-1 output + the zero rows of the padded window positions [n_real + n_pad, C]
+    qkv: torch.Tensor
+    a: torch.Tensor          # attention output, real + padded rows
+    lse: torch.Tensor
+    bias: torch.Tensor       # relative-position bias (+ shift mask) slab [nW, heads, L, L]
+
+
 def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, save: bool, scales, B: int):
     """SwinTransformerBlock3D.forward :248-268 on tokens x [n_real, C]."""
-    C_, I = x.shape[1], blk.mlp.fc1.weight.shape[0]
+    C_ = x.shape[1]
     dev = x.device
     n_real, n_pad, L = geo["n_real"], geo["n_pad"], geo["L"]
     n_ext = n_real + n_pad
@@ -270,9 +273,9 @@ def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, sa
     h = torch.empty(n_ext, C_, dtype=bf16, device=dev)
     if n_pad:
         h[n_real:].zero_()
-    _, mean1, rstd1 = _ln_any(x, blk.norm1, n_real, C_, model.eps, out=h)
+    _, mean1, rstd1 = layernorm(x, blk.norm1, wide=True, out=h)
     qkv = torch.empty(n_ext, 3 * C_, dtype=bf16, device=dev)
-    ops.linear_fwd(h, _w(model, p + "attn.qkv.weight", blk.attn.qkv.weight), blk.attn.qkv.bias, qkv, scale_cols=C_,
+    ops.linear_fwd(h, weight(model, p + "attn.qkv.weight"), blk.attn.qkv.bias, qkv, scale_cols=C_,
                    col_scale=HEAD_DIM ** -0.5)                            # q * scale (:145), bias included
     # relative-position bias (+ shift mask) slab [nW, heads, L, L]
     tab = blk.attn.relative_position_bias_table.detach()
@@ -286,67 +289,30 @@ def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, sa
     desc = ops.window_desc(n_ext, heads, HEAD_DIM, 3 * C_, C_, idx, bias)
     ops.seg_attention_fwd(qkv, a, lse, desc)
     # proj on the real rows (the crop of :242-243), residual + drop_path (:260)
-    x1 = _residual(model, p + "attn.proj", blk.attn.proj, a[:n_real], x, s_a, n_real, C_)
-    h2, mean2, rstd2 = _ln_any(x1, blk.norm2, n_real, C_, model.eps)
-    pre = torch.empty(n_real, I, dtype=bf16, device=dev) if save else None
-    f1 = torch.empty(n_real, I, dtype=bf16, device=dev)
-    ops.linear_fwd(h2, _w(model, p + "mlp.fc1.weight", blk.mlp.fc1.weight), blk.mlp.fc1.bias, f1, act=_lib.ACT_GELU_ERF,
-                   aux=pre, ld_aux=I)
-    out = _residual(model, p + "mlp.fc2", blk.mlp.fc2, f1, x1, s_m, n_real, C_)
-    saved = (x, mean1, rstd1, h, qkv, a, lse, bias, x1, mean2, rstd2, h2, pre, f1) if save else None
-    return out, saved
-
-
-def _residual(model, name: str, lin: nn.Linear, a, residual, scale, rows: int, C_: int):
-    out = torch.empty(rows, C_, dtype=bf16, device=a.device)
-    if scale is None:
-        ops.linear_fwd(a, _w(model, name + ".weight", lin.weight), lin.bias, out, residual=residual, ldr=C_)
-    else:
-        tmp = torch.empty(rows, C_, dtype=bf16, device=a.device)
-        ops.linear_fwd(a, _w(model, name + ".weight", lin.weight), lin.bias, tmp)
-        ops.rowscale(tmp, scale, out, residual=residual)
-    return out
+    x1 = residual_linear(model, p + "attn.proj", blk.attn.proj, a[:n_real], x, s_a)
+    out, mlp = mlp_fwd(model, p, blk, x1, save, s_m, wide=True)
+    return out, ((_WindowSaved(x, mean1, rstd1, h, qkv, a, lse, bias), mlp) if save else None)
 
 
 def _block_bwd(model, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads: int, grads, scales):
-    (x, mean1, rstd1, h, qkv, a, lse, bias, x1, mean2, rstd2, h2, pre, f1) = saved
-    C_, I = x.shape[1], blk.mlp.fc1.weight.shape[0]
+    win, mlp = saved
+    C_ = dx.shape[1]
     dev = dx.device
     n_real, n_pad, L = geo["n_real"], geo["n_pad"], geo["L"]
     n_ext = n_real + n_pad
     s_a, s_m = scales if scales is not None else (None, None)
-
-    def dropped(dy, s):
-        if s is None:
-            return dy
-        o = torch.empty_like(dy)
-        ops.rowscale(dy, s, o)
-        return o
-
-    def ln_bwd(dy, x_in, ln, name, mean, rstd, dres):
-        o = torch.empty(n_real, C_, dtype=bf16, device=dev)
-        ops.layernorm_any_bwd(dy, x_in, ln.weight, mean, rstd, dres, o, grads[name + ".weight"], grads[name + ".bias"], n_real, C_)
-        return o
-
-    # ---- out = x1 + drop_path(fc2(gelu(fc1(LN(x1)))))
-    dpre = _linear_bwd(model, p + "mlp.fc2", blk.mlp.fc2, dropped(dx, s_m), f1, grads, act=_lib.ACT_DGELU_ERF, aux=pre, ld_aux=I)
-    dh2 = _linear_bwd(model, p + "mlp.fc1", blk.mlp.fc1, dpre, h2, grads)
-    del dpre
-    dx1 = ln_bwd(dh2, x1, blk.norm2, p + "norm2", mean2, rstd2, dx)
+    dx1 = mlp_bwd(model, p, blk, dx, mlp, grads, s_m, wide=True)
     # ---- x1 = x + drop_path(proj(window_attention(LN(x))))
-    dy = dropped(dx1, s_a)
-    ops.linear_wgrad(dy, a[:n_real], grads[p + "attn.proj.weight"])
-    ops.colsum(dy, grads[p + "attn.proj.bias"])
     da = torch.empty(n_ext, C_, dtype=bf16, device=dev)
     if n_pad:
         da[n_real:].zero_()                                               # outputs at padded positions are cropped away
-    ops.linear_dgrad(dy, _w(model, p + "attn.proj.weight", blk.attn.proj.weight), da[:n_real])
+    linear_bwd(model, p + "attn.proj", drop_scale(dx1, s_a), win.a[:n_real], grads, out=da[:n_real])
     idx = geo["idx"][1 if shifted else 0]
     ds = torch.empty(idx.shape[0], heads, L, L, dtype=bf16, device=dev)
     dqkv = torch.empty(n_ext, 3 * C_, dtype=bf16, device=dev)
     delta = torch.empty(heads, n_ext, dtype=f32, device=dev)
-    desc = ops.window_desc(n_ext, heads, HEAD_DIM, 3 * C_, C_, idx, bias, ds_out=ds)
-    ops.seg_attention_bwd(qkv, a, da, lse, delta, dqkv, desc, HEAD_DIM ** -0.5)
+    desc = ops.window_desc(n_ext, heads, HEAD_DIM, 3 * C_, C_, idx, win.bias, ds_out=ds)
+    ops.seg_attention_bwd(win.qkv, win.a, da, win.lse, delta, dqkv, desc, HEAD_DIM ** -0.5)
     # relative-position bias table: sum dL/dlogits over all windows, scatter through the fixed index (:149)
     if (heads * L * L) % 8 == 0:
         dbias = torch.zeros(heads * L * L, dtype=f32, device=dev)
@@ -357,11 +323,8 @@ def _block_bwd(model, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads:
     grads[p + "attn.relative_position_bias_table"].index_add_(0, ridx, dbias.view(heads, L * L).t())
     del ds
     # qkv Linear over real + padded rows (padded inputs are zero: they only reach the bias)
-    ops.linear_wgrad(dqkv, h, grads[p + "attn.qkv.weight"])
-    ops.colsum(dqkv, grads[p + "attn.qkv.bias"])
-    dh = torch.empty(n_ext, C_, dtype=bf16, device=dev)
-    ops.linear_dgrad(dqkv, _w(model, p + "attn.qkv.weight", blk.attn.qkv.weight), dh)
-    return ln_bwd(dh[:n_real], x, blk.norm1, p + "norm1", mean1, rstd1, dx1)
+    dh = linear_bwd(model, p + "attn.qkv", dqkv, win.h, grads)
+    return layernorm_bwd(dh[:n_real], win.x, blk.norm1, win.mean, win.rstd, dx1, grads, p + "norm1", wide=True)
 
 
 # ------------------------------------------------------------------------------------------- function
@@ -385,12 +348,12 @@ class _Swin3DFunction(torch.autograd.Function):
         if ph != pw:
             raise NotImplementedError("square spatial patches only")
         ops.vip_patchify(frames, patches, ph)
-        w0 = _w(model, "patch_embed.proj.weight", model.patch_embed.proj.weight).view(C0, K0)
+        w0 = weight(model, "patch_embed.proj.weight").view(C0, K0)
         tok = torch.empty(rows, C0, dtype=bf16, device=dev)
         ops.linear_fwd(patches, w0, model.patch_embed.proj.bias, tok)
         pe_saved = None
         if model.patch_embed.norm is not None:
-            tok_n, pm, pr = _ln_any(tok, model.patch_embed.norm, rows, C0, model.eps)
+            tok_n, pm, pr = layernorm(tok, model.patch_embed.norm, wide=True)
             pe_saved = (tok, pm, pr)
             tok = tok_n
         # ---- layers
@@ -416,16 +379,15 @@ class _Swin3DFunction(torch.autograd.Function):
                 n_out = B * D * H2 * W2
                 cat = torch.empty(n_out, 4 * C_, dtype=bf16, device=dev)
                 ops.gather_rows(tok, midx, cat, C_)
-                catn, mm, mr = _ln_any(cat, layer.downsample.norm, n_out, 4 * C_, model.eps)
+                catn, mm, mr = layernorm(cat, layer.downsample.norm, wide=True)
                 red = torch.empty(n_out, 2 * C_, dtype=bf16, device=dev)
-                ops.linear_fwd(catn, _w(model, f"layers.{i}.downsample.reduction.weight", layer.downsample.reduction.weight),
-                               None, red)
+                ops.linear_fwd(catn, weight(model, f"layers.{i}.downsample.reduction.weight"), None, red)
                 merge_saved = (cat, mm, mr, catn, midx, rows, C_)
                 tok, H, W, rows = red, H2, W2, n_out
             layer_saved.append((blocks_saved, merge_saved))
             geos.append(geo)
         Cl = tok.shape[1]
-        outn, fm, fr = _ln_any(tok, model.norm, rows, Cl, model.eps)
+        outn, fm, fr = layernorm(tok, model.norm, wide=True)
         out = outn.view(B, D, H, W, Cl).to(video.dtype)
         if save:
             ctx.model, ctx.names, ctx.geos = model, names, geos
@@ -441,11 +403,9 @@ class _Swin3DFunction(torch.autograd.Function):
         dev = d_out.device
         named = dict(model.named_parameters())
         grads: Dict[str, torch.Tensor] = {}
-        _alloc_flat({n: tuple(named[n].shape) for n in names}, grads, dev)
-        rows = B * D * H * W
-        dy = d_out.reshape(rows, Cl).to(bf16).contiguous()
-        dtok = torch.empty(rows, Cl, dtype=bf16, device=dev)
-        ops.layernorm_any_bwd(dy, tok_last, model.norm.weight, fm, fr, None, dtok, grads["norm.weight"], grads["norm.bias"], rows, Cl)
+        alloc_flat({n: tuple(named[n].shape) for n in names}, grads, dev)
+        dy = d_out.reshape(B * D * H * W, Cl).to(bf16).contiguous()
+        dtok = layernorm_bwd(dy, tok_last, model.norm, fm, fr, None, grads, "norm", wide=True)
         for i in reversed(range(model.num_layers)):
             layer = model.layers[i]
             blocks_saved, merge_saved = layer_saved[i]
@@ -455,10 +415,8 @@ class _Swin3DFunction(torch.autograd.Function):
                 name = f"layers.{i}.downsample."
                 ops.linear_wgrad(dtok, catn, grads[name + "reduction.weight"])
                 dcatn = torch.empty(n_out, 4 * C_, dtype=bf16, device=dev)
-                ops.linear_dgrad(dtok, _w(model, name + "reduction.weight", layer.downsample.reduction.weight), dcatn)
-                dcat = torch.empty(n_out, 4 * C_, dtype=bf16, device=dev)
-                ops.layernorm_any_bwd(dcatn, cat, layer.downsample.norm.weight, mm, mr, None, dcat, grads[name + "norm.weight"],
-                                      grads[name + "norm.bias"], n_out, 4 * C_)
+                ops.linear_dgrad(dtok, weight(model, name + "reduction.weight"), dcatn)
+                dcat = layernorm_bwd(dcatn, cat, layer.downsample.norm, mm, mr, None, grads, name + "norm", wide=True)
                 dtok = torch.empty(rows_in, C_, dtype=bf16, device=dev)
                 ops.scatter_rows(dcat, midx, dtok, C_)                    # every input row occurs exactly once
             heads = model.num_heads[i]
@@ -469,13 +427,9 @@ class _Swin3DFunction(torch.autograd.Function):
                 blocks_saved[j] = None
         # ---- PatchEmbed3D
         C0 = model.embed_dim
-        rows0 = patches.shape[0]
         if pe_saved is not None:
             tok0, pm, pr = pe_saved
-            d0 = torch.empty(rows0, C0, dtype=bf16, device=dev)
-            ops.layernorm_any_bwd(dtok, tok0, model.patch_embed.norm.weight, pm, pr, None, d0, grads["patch_embed.norm.weight"],
-                                  grads["patch_embed.norm.bias"], rows0, C0)
-            dtok = d0
+            dtok = layernorm_bwd(dtok, tok0, model.patch_embed.norm, pm, pr, None, grads, "patch_embed.norm", wide=True)
         ops.linear_wgrad(dtok, patches, grads["patch_embed.proj.weight"].view(C0, -1))
         ops.colsum(dtok, grads["patch_embed.proj.bias"])
         ctx.saved = None

@@ -30,14 +30,16 @@ There is no CPU path.
 from __future__ import annotations
 
 import math
-from typing import Dict, List
+from typing import Dict, List, NamedTuple, Optional
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib, ops
-from .clip_vip import _alloc_flat
+from ._blocks import (MlpSaved, alloc_flat, drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd,
+                      residual_linear)
+from ._weights import refresh_weights, weight
 
 bf16, f32 = torch.bfloat16, torch.float32
 ATTENTION_TYPES = ('divided_space_time', 'space_only', 'joint_space_time')
@@ -154,27 +156,6 @@ class TimeSformer(nn.Module):
 
 
 # ----------------------------------------------------------------------------------- helpers
-def _w(model, name: str, p: torch.Tensor) -> torch.Tensor:
-    """bf16 compute copy of a GEMM weight (refreshed for the whole model at the start of every forward)."""
-    return model._cache[name]
-
-
-def refresh_weights(model) -> None:
-    """Re-cast every GEMM weight (parameters with >= 2 dims that `_w` serves) with ONE launch on every forward: in-place
-    `p.data` updates of the reference optimizers do not move `_version`, so no validity test is used (modeling/_weights.py)."""
-    from ._weights import WeightMirror
-    cache = model._cache
-    named = [(n, p) for n, p in model.named_parameters() if p.dim() >= 2 and n.endswith("weight")]
-    dev = named[0][1].device
-    if cache.get("__device__") != dev:
-        cache.clear()
-        cache["__device__"] = dev
-        cache["__mirror__"] = WeightMirror()
-        for n, p in named:
-            cache[n] = torch.empty(p.shape, dtype=bf16, device=dev)
-    cache["__mirror__"].refresh([(p, cache[n]) for n, p in named])
-
-
 def _tables(model: TimeSformer, T: int, H: int, W: int, pos_param=None, time_param=None):
     """pos [H*W, C] / time [T, C] fp32 as the forward adds them: bilinear / linear interpolation of the learned tables
     when the grid or the frame count differs (timesformer.py:487-494, 504-508).  Parameter preprocessing on tiny
@@ -193,29 +174,6 @@ def _tables(model: TimeSformer, T: int, H: int, W: int, pos_param=None, time_par
     return pos[0].float().contiguous(), time[0].float().contiguous()
 
 
-def _ln(x, ln: nn.LayerNorm, rows: int, C_: int, eps: float):
-    plain = ops.rowmap(C_)
-    mean = torch.empty(rows, dtype=f32, device=x.device)
-    rstd = torch.empty_like(mean)
-    y = torch.empty(rows, C_, dtype=bf16, device=x.device)
-    ops.layernorm_fwd(x, plain, y, plain, ln.weight, ln.bias, mean, rstd, rows, C_, eps)
-    return y, mean, rstd
-
-
-def _attn_fwd(model, pre: str, att: _TsfAttention, h, desc, rows: int, C_: int):
-    dev = h.device
-    qkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
-    # (q k^T) * head_dim**-0.5 (timesformer.py:165): 0.125 is a power of two, folding it into q (bias included) is exact
-    ops.linear_fwd(h, _w(model, pre + "qkv.weight", att.qkv.weight), att.qkv.bias, qkv, scale_cols=C_, col_scale=0.125)
-    a = torch.empty(rows, C_, dtype=bf16, device=dev)
-    lse = torch.empty(model.num_heads, rows, dtype=f32, device=dev)
-    if isinstance(desc, _lib.XpDenseAttn):
-        ops.dense_attention_fwd(qkv, a, lse, desc)
-    else:
-        ops.seg_attention_fwd(qkv, a, lse, desc)
-    return qkv, a, lse
-
-
 def _row_scales(masks, B: int, T: int, HW: int):
     """Per-token-row DropPath factors (rows ordered (b, p, t)) from the per-group factors of one block."""
     if masks is None:
@@ -226,167 +184,100 @@ def _row_scales(masks, B: int, T: int, HW: int):
             m_m.repeat_interleave(HW * T).contiguous())
 
 
-def _residual_linear(model, name: str, lin: nn.Linear, a, residual, scale, rows: int, C_: int):
-    """residual + drop_path(lin(a)): fused into the GEMM epilogue when no path is dropped, else GEMM + one row-scale pass."""
-    out = torch.empty(rows, C_, dtype=bf16, device=a.device)
-    if scale is None:
-        ops.linear_fwd(a, _w(model, name + ".weight", lin.weight), lin.bias, out, residual=residual, ldr=C_)
+class _AttnSaved(NamedTuple):
+    x: torch.Tensor          # LayerNorm input
+    mean: torch.Tensor
+    rstd: torch.Tensor
+    h: torch.Tensor          # LayerNorm output, the qkv GEMM's input
+    qkv: torch.Tensor        # fused [rows, 3C], q pre-scaled
+    a: torch.Tensor          # attention output
+    lse: torch.Tensor
+
+
+class _BlockSaved(NamedTuple):
+    temporal: Optional[_AttnSaved]      # divided_space_time only
+    p_t: Optional[torch.Tensor]         # temporal proj output after drop_path: temporal_fc's input
+    attn: _AttnSaved
+    mlp: MlpSaved
+
+
+def _attn_fwd(model: TimeSformer, i: int, half: str, x, desc) -> _AttnSaved:
+    """LayerNorm -> fused qkv GEMM -> attention of block i's temporal (half 'temporal_') or spatial / dense (half '') part.
+    The kernel follows the descriptor: seg attention (temporal, spatial) or dense attention (joint, space-only)."""
+    blk, p = model.blocks[i], f"blocks.{i}.{half}attn."
+    att = getattr(blk, half + "attn")
+    rows, C_ = x.shape
+    dev = x.device
+    h, mean, rstd = layernorm(x, getattr(blk, half + "norm1"))
+    qkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
+    # (q k^T) * head_dim**-0.5 (timesformer.py:165): 0.125 is a power of two, folding it into q (bias included) is exact
+    ops.linear_fwd(h, weight(model, p + "qkv.weight"), att.qkv.bias, qkv, scale_cols=C_, col_scale=0.125)
+    a = torch.empty(rows, C_, dtype=bf16, device=dev)
+    lse = torch.empty(model.num_heads, rows, dtype=f32, device=dev)
+    if isinstance(desc, _lib.XpDenseAttn):
+        ops.dense_attention_fwd(qkv, a, lse, desc)
     else:
-        tmp = torch.empty(rows, C_, dtype=bf16, device=a.device)
-        ops.linear_fwd(a, _w(model, name + ".weight", lin.weight), lin.bias, tmp)
-        ops.rowscale(tmp, scale, out, residual=residual)
-    return out
+        ops.seg_attention_fwd(qkv, a, lse, desc)
+    return _AttnSaved(x, mean, rstd, h, qkv, a, lse)
 
 
-def _block_fwd(model: TimeSformer, i: int, x, descs, rows: int, save: bool, scales=None):
-    """timesformer.py:207-226.  x: [rows, C] bf16 tokens, (h w t) order.  scales: per-row DropPath factors
-    (temporal, spatial, mlp) of this block or None."""
-    blk = model.blocks[i]
-    C_, I = model.embed_dim, blk.mlp.fc1.weight.shape[0]
-    dev, p = x.device, f"blocks.{i}."
-    d_t, d_s = descs
-    s_t, s_s, s_m = scales if scales is not None else (None, None, None)
-    # ---- temporal attention -> proj -> drop_path -> temporal_fc -> residual (:209-214)
-    ln_t, mean_t, rstd_t = _ln(x, blk.temporal_norm1, rows, C_, model.eps)
-    qkv_t, a_t, lse_t = _attn_fwd(model, p + "temporal_attn.", blk.temporal_attn, ln_t, d_t, rows, C_)
-    p_t = torch.empty(rows, C_, dtype=bf16, device=dev)
-    ops.linear_fwd(a_t, _w(model, p + "temporal_attn.proj.weight", blk.temporal_attn.proj.weight),
-                   blk.temporal_attn.proj.bias, p_t)
-    if s_t is not None:
-        ops.rowscale(p_t, s_t, p_t)          # in place: the saved p_t is the dropped one, as temporal_fc consumed it
-    xt = torch.empty(rows, C_, dtype=bf16, device=dev)
-    ops.linear_fwd(p_t, _w(model, p + "temporal_fc.weight", blk.temporal_fc.weight), blk.temporal_fc.bias, xt,
-                   residual=x, ldr=C_)
-    # ---- spatial attention -> proj -> residual (:216-224)
-    ln_s, mean_s, rstd_s = _ln(xt, blk.norm1, rows, C_, model.eps)
-    qkv_s, a_s, lse_s = _attn_fwd(model, p + "attn.", blk.attn, ln_s, d_s, rows, C_)
-    x2 = _residual_linear(model, p + "attn.proj", blk.attn.proj, a_s, xt, s_s, rows, C_)
+def _attn_bwd(model: TimeSformer, i: int, half: str, da, sv: _AttnSaved, desc, grads, dres):
+    """Backward of _attn_fwd from the gradient of the attention output; dres is the gradient carried by the residual path
+    around this part.  Returns the gradient of the part's input."""
+    blk, p = model.blocks[i], f"blocks.{i}.{half}"
+    rows, C_ = da.shape
+    dqkv = torch.empty(rows, 3 * C_, dtype=bf16, device=da.device)
+    delta = torch.empty(model.num_heads, rows, dtype=f32, device=da.device)
+    if isinstance(desc, _lib.XpDenseAttn):
+        ops.dense_attention_bwd(sv.qkv, sv.a, da, sv.lse, delta, dqkv, desc, 0.125)
+    else:
+        ops.seg_attention_bwd(sv.qkv, sv.a, da, sv.lse, delta, dqkv, desc, 0.125)
+    dh = linear_bwd(model, p + "attn.qkv", dqkv, sv.h, grads)
+    return layernorm_bwd(dh, sv.x, getattr(blk, half + "norm1"), sv.mean, sv.rstd, dres, grads, p + "norm1")
+
+
+def _block_fwd(model: TimeSformer, i: int, x, descs, save: bool, scales=None):
+    """timesformer.py:207-226.  x: [rows, C] bf16 tokens, (h w t) order.  descs: (temporal, spatial) attention descriptors
+    of 'divided_space_time', or (None, dense) for 'joint_space_time' / 'space_only' (:202-205), whose blocks have no temporal
+    part.  scales: per-row DropPath factors (temporal, attention, mlp) of this block or None."""
+    blk, p = model.blocks[i], f"blocks.{i}."
+    C_ = model.embed_dim
+    d_t, d_a = descs
+    s_t, s_a, s_m = scales if scales is not None else (None, None, None)
+    temporal = p_t = None
+    if d_t is not None:
+        # ---- temporal attention -> proj -> drop_path -> temporal_fc -> residual (:209-214)
+        temporal = _attn_fwd(model, i, "temporal_", x, d_t)
+        p_t = torch.empty(x.shape[0], C_, dtype=bf16, device=x.device)
+        ops.linear_fwd(temporal.a, weight(model, p + "temporal_attn.proj.weight"), blk.temporal_attn.proj.bias, p_t)
+        if s_t is not None:
+            ops.rowscale(p_t, s_t, p_t)          # in place: the saved p_t is the dropped one, as temporal_fc consumed it
+        xt = torch.empty(x.shape[0], C_, dtype=bf16, device=x.device)
+        ops.linear_fwd(p_t, weight(model, p + "temporal_fc.weight"), blk.temporal_fc.bias, xt, residual=x, ldr=C_)
+        x = xt
+    # ---- spatial / dense attention -> proj -> drop_path -> residual (:216-224, :202-204)
+    attn = _attn_fwd(model, i, "", x, d_a)
+    x2 = residual_linear(model, p + "attn.proj", blk.attn.proj, attn.a, x, s_a)
     # ---- MLP with exact-erf GELU (:225, :132-138)
-    ln_m, mean_m, rstd_m = _ln(x2, blk.norm2, rows, C_, model.eps)
-    pre = torch.empty(rows, I, dtype=bf16, device=dev) if save else None
-    f1 = torch.empty(rows, I, dtype=bf16, device=dev)
-    ops.linear_fwd(ln_m, _w(model, p + "mlp.fc1.weight", blk.mlp.fc1.weight), blk.mlp.fc1.bias, f1,
-                   act=_lib.ACT_GELU_ERF, aux=pre, ld_aux=I)
-    out = _residual_linear(model, p + "mlp.fc2", blk.mlp.fc2, f1, x2, s_m, rows, C_)
-    saved = (x, mean_t, rstd_t, ln_t, qkv_t, a_t, lse_t, p_t, xt, mean_s, rstd_s, ln_s, qkv_s, a_s, lse_s, x2, mean_m,
-             rstd_m, ln_m, pre, f1) if save else None
-    return out, saved
+    out, mlp = mlp_fwd(model, p, blk, x2, save, s_m)
+    return out, (_BlockSaved(temporal, p_t, attn, mlp) if save else None)
 
 
-def _dense_block_fwd(model: TimeSformer, i: int, x, desc, rows: int, save: bool, scales=None):
-    """timesformer.py:202-205 ('joint_space_time' / 'space_only'): x + drop_path(attn(norm1(x))), then the MLP.  The
-    attention is dense within each sequence of `desc`; scales: per-row DropPath factors (attention, mlp) or None."""
-    blk = model.blocks[i]
-    C_, I = model.embed_dim, blk.mlp.fc1.weight.shape[0]
-    dev, p = x.device, f"blocks.{i}."
-    s_a, s_m = scales if scales is not None else (None, None)
-    ln_a, mean_a, rstd_a = _ln(x, blk.norm1, rows, C_, model.eps)
-    qkv, a, lse = _attn_fwd(model, p + "attn.", blk.attn, ln_a, desc, rows, C_)
-    x2 = _residual_linear(model, p + "attn.proj", blk.attn.proj, a, x, s_a, rows, C_)
-    ln_m, mean_m, rstd_m = _ln(x2, blk.norm2, rows, C_, model.eps)
-    pre = torch.empty(rows, I, dtype=bf16, device=dev) if save else None
-    f1 = torch.empty(rows, I, dtype=bf16, device=dev)
-    ops.linear_fwd(ln_m, _w(model, p + "mlp.fc1.weight", blk.mlp.fc1.weight), blk.mlp.fc1.bias, f1,
-                   act=_lib.ACT_GELU_ERF, aux=pre, ld_aux=I)
-    out = _residual_linear(model, p + "mlp.fc2", blk.mlp.fc2, f1, x2, s_m, rows, C_)
-    saved = (x, mean_a, rstd_a, ln_a, qkv, a, lse, x2, mean_m, rstd_m, ln_m, pre, f1) if save else None
-    return out, saved
-
-
-def _linear_bwd(model, name: str, lin: nn.Linear, dy, x_in, grads, need_dx: bool = True, **dgrad_kw):
-    """dW += dy^T x_in, db += colsum(dy), returns dx = dy W (bf16)."""
-    ops.linear_wgrad(dy, x_in, grads[name + ".weight"])
-    ops.colsum(dy, grads[name + ".bias"])
-    if not need_dx:
-        return None
-    dx = torch.empty(dy.shape[0], lin.weight.shape[1], dtype=bf16, device=dy.device)
-    ops.linear_dgrad(dy, _w(model, name + ".weight", lin.weight), dx, **dgrad_kw)
-    return dx
-
-
-def _block_bwd(model: TimeSformer, i: int, dx, saved, descs, grads, rows: int, scales=None):
-    (x, mean_t, rstd_t, ln_t, qkv_t, a_t, lse_t, p_t, xt, mean_s, rstd_s, ln_s, qkv_s, a_s, lse_s, x2, mean_m, rstd_m,
-     ln_m, pre, f1) = saved
-    blk = model.blocks[i]
-    C_, I = model.embed_dim, blk.mlp.fc1.weight.shape[0]
-    dev, p = dx.device, f"blocks.{i}."
-    d_t, d_s = descs
-    plain = ops.rowmap(C_)
-    delta = torch.empty(model.num_heads, rows, dtype=f32, device=dev)
-
-    def ln_bwd(dy, x_in, ln, name, mean, rstd, dres):
-        out = torch.empty(rows, C_, dtype=bf16, device=dev)
-        ops.layernorm_bwd(dy, plain, x_in, plain, ln.weight, mean, rstd, dres, plain, out, plain,
-                          grads[name + ".weight"], grads[name + ".bias"], rows, C_)
-        return out
-
-    def attn_bwd(pre_name, att, qkv, a, da, lse, h_in, desc):
-        dqkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
-        ops.seg_attention_bwd(qkv, a, da, lse, delta, dqkv, desc, 0.125)
-        return _linear_bwd(model, pre_name + "qkv", att.qkv, dqkv, h_in, grads)
-
-    s_t, s_s, s_m = scales if scales is not None else (None, None, None)
-
-    def dropped(dy, s):     # gradient entering a drop_path'ed branch: the same per-row factor (one extra pass when active)
-        if s is None:
-            return dy
-        out = torch.empty_like(dy)
-        ops.rowscale(dy, s, out)
-        return out
-
-    # ---- out = x2 + drop_path(fc2(gelu(fc1(LN(x2)))))
-    dpre = _linear_bwd(model, p + "mlp.fc2", blk.mlp.fc2, dropped(dx, s_m), f1, grads, act=_lib.ACT_DGELU_ERF, aux=pre,
-                       ld_aux=I)
-    dln_m = _linear_bwd(model, p + "mlp.fc1", blk.mlp.fc1, dpre, ln_m, grads)
-    del dpre
-    dx2 = ln_bwd(dln_m, x2, blk.norm2, p + "norm2", mean_m, rstd_m, dx)
-    # ---- x2 = xt + drop_path(proj(attn_s(LN(xt))))
-    da_s = _linear_bwd(model, p + "attn.proj", blk.attn.proj, dropped(dx2, s_s), a_s, grads)
-    dln_s = attn_bwd(p + "attn.", blk.attn, qkv_s, a_s, da_s, lse_s, ln_s, d_s)
-    dxt = ln_bwd(dln_s, xt, blk.norm1, p + "norm1", mean_s, rstd_s, dx2)
+def _block_bwd(model: TimeSformer, i: int, dx, saved: _BlockSaved, descs, grads, scales=None):
+    blk, p = model.blocks[i], f"blocks.{i}."
+    s_t, s_a, s_m = scales if scales is not None else (None, None, None)
+    dx2 = mlp_bwd(model, p, blk, dx, saved.mlp, grads, s_m)
+    # ---- x2 = xt + drop_path(proj(attn(LN(xt))))
+    da = linear_bwd(model, p + "attn.proj", drop_scale(dx2, s_a), saved.attn.a, grads)
+    dxt = _attn_bwd(model, i, "", da, saved.attn, descs[1], grads, dx2)
+    if saved.temporal is None:
+        return dxt
     # ---- xt = x + temporal_fc(drop_path(proj_t(attn_t(LN(x)))))   (the saved p_t is already the dropped one)
-    dp_t = _linear_bwd(model, p + "temporal_fc", blk.temporal_fc, dxt, p_t, grads)
+    dp_t = linear_bwd(model, p + "temporal_fc", dxt, saved.p_t, grads)
     if s_t is not None:
         ops.rowscale(dp_t, s_t, dp_t)
-    da_t = _linear_bwd(model, p + "temporal_attn.proj", blk.temporal_attn.proj, dp_t, a_t, grads)
-    dln_t = attn_bwd(p + "temporal_attn.", blk.temporal_attn, qkv_t, a_t, da_t, lse_t, ln_t, d_t)
-    return ln_bwd(dln_t, x, blk.temporal_norm1, p + "temporal_norm1", mean_t, rstd_t, dxt)
-
-
-def _dense_block_bwd(model: TimeSformer, i: int, dx, saved, desc, grads, rows: int, scales=None):
-    x, mean_a, rstd_a, ln_a, qkv, a, lse, x2, mean_m, rstd_m, ln_m, pre, f1 = saved
-    blk = model.blocks[i]
-    C_, I = model.embed_dim, blk.mlp.fc1.weight.shape[0]
-    dev, p = dx.device, f"blocks.{i}."
-    plain = ops.rowmap(C_)
-    s_a, s_m = scales if scales is not None else (None, None)
-
-    def ln_bwd(dy, x_in, ln, name, mean, rstd, dres):
-        out = torch.empty(rows, C_, dtype=bf16, device=dev)
-        ops.layernorm_bwd(dy, plain, x_in, plain, ln.weight, mean, rstd, dres, plain, out, plain,
-                          grads[name + ".weight"], grads[name + ".bias"], rows, C_)
-        return out
-
-    def dropped(dy, s):
-        if s is None:
-            return dy
-        out = torch.empty_like(dy)
-        ops.rowscale(dy, s, out)
-        return out
-
-    # ---- out = x2 + drop_path(fc2(gelu(fc1(LN(x2)))))
-    dpre = _linear_bwd(model, p + "mlp.fc2", blk.mlp.fc2, dropped(dx, s_m), f1, grads, act=_lib.ACT_DGELU_ERF, aux=pre,
-                       ld_aux=I)
-    dln_m = _linear_bwd(model, p + "mlp.fc1", blk.mlp.fc1, dpre, ln_m, grads)
-    del dpre
-    dx2 = ln_bwd(dln_m, x2, blk.norm2, p + "norm2", mean_m, rstd_m, dx)
-    # ---- x2 = x + drop_path(proj(attn(LN(x))))
-    da = _linear_bwd(model, p + "attn.proj", blk.attn.proj, dropped(dx2, s_a), a, grads)
-    dqkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
-    delta = torch.empty(model.num_heads, rows, dtype=f32, device=dev)
-    ops.dense_attention_bwd(qkv, a, da, lse, delta, dqkv, desc, 0.125)
-    dln_a = _linear_bwd(model, p + "attn.qkv", blk.attn.qkv, dqkv, ln_a, grads)
-    return ln_bwd(dln_a, x, blk.norm1, p + "norm1", mean_a, rstd_a, dx2)
+    da_t = linear_bwd(model, p + "temporal_attn.proj", dp_t, saved.temporal.a, grads)
+    return _attn_bwd(model, i, "temporal_", da_t, saved.temporal, descs[0], grads, dxt)
 
 
 class _TimeSformerFunction(torch.autograd.Function):
@@ -406,17 +297,15 @@ class _TimeSformerFunction(torch.autograd.Function):
             descs = (ops.temporal_desc(rows, T, model.num_heads, 3 * C_, C_),
                      ops.spatial_desc(B, T, HW, model.num_heads, 3 * C_, C_))
             scales = [_row_scales(None if masks is None else masks[i], B, T, HW) for i in range(model.depth)]
-            block_fwd = _block_fwd
         else:
             # one sequence per clip ('b (h w t) m', joint) or per frame ('(b t) (h w) m', space_only at T = 1)
             seq_len = HW * T if model.attention_type == 'joint_space_time' else HW
-            descs = ops.dense_desc(rows, model.num_heads, 3 * C_, C_, n_seq=rows // seq_len, seq_len=seq_len)
+            descs = (None, ops.dense_desc(rows, model.num_heads, 3 * C_, C_, n_seq=rows // seq_len, seq_len=seq_len))
             scales = [None if masks is None or masks[i] is None else
-                      tuple(m.repeat_interleave(seq_len).contiguous() for m in masks[i]) for i in range(model.depth)]
-            block_fwd = _dense_block_fwd
+                      (None,) + tuple(m.repeat_interleave(seq_len).contiguous() for m in masks[i]) for i in range(model.depth)]
         saved = []
         for i in range(model.depth):
-            tok, sv = block_fwd(model, i, tok, descs, rows, save, scales[i])
+            tok, sv = _block_fwd(model, i, tok, descs, save, scales[i])
             saved.append(sv)
         out = torch.empty(B, T, C_, H, W, dtype=x.dtype, device=x.device)   # timesformer.py:523 (values; contiguous)
         ops.tsf_untokenize(tok, out, B, T, C_, HW)
@@ -437,9 +326,8 @@ class _TimeSformerFunction(torch.autograd.Function):
         grads: Dict[str, torch.Tensor] = {}
         for i in reversed(range(model.depth)):
             shapes = {n: tuple(p.shape) for n, p in model.blocks[i].named_parameters(prefix=f"blocks.{i}")}
-            _alloc_flat(shapes, grads, dev)
-            block_bwd = _block_bwd if model.attention_type == 'divided_space_time' else _dense_block_bwd
-            dtok = block_bwd(model, i, dtok, saved[i], descs, grads, rows, ctx.scales[i])
+            alloc_flat(shapes, grads, dev)
+            dtok = _block_bwd(model, i, dtok, saved[i], descs, grads, ctx.scales[i])
             saved[i] = None
         dx = None
         if ctx.needs_input_grad[3]:
