@@ -17,7 +17,139 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(handle, name), f"{name} declared in include/xpretrain_b200.h but not exported"
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    assert handle.xp_version() == 1
+    assert handle.xp_version() == _lib.ABI_VERSION
+
+
+_C_KINDS = {"int": "int32_t", "int32_t": "int32_t", "uint32_t": "uint32_t", "int64_t": "int64_t", "float": "float",
+            "void": "void"}
+
+
+def _c_kind(decl: str) -> str:
+    """pointer / int32_t / uint32_t / int64_t / float / void of a C return type or parameter declaration."""
+    if "*" in decl:
+        return "pointer"
+    words = [w for w in re.findall(r"\w+", decl) if w != "const"]
+    return _C_KINDS.get(words[0], words[0])
+
+
+def _py_kind(t) -> str:
+    import ctypes as C
+    if t is None:
+        return "void"
+    if t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer):
+        return "pointer"
+    return {C.c_int32: "int32_t", C.c_uint32: "uint32_t", C.c_int64: "int64_t", C.c_float: "float"}.get(t, t.__name__)
+
+
+def _header_declarations():
+    """({struct: [(field, kind)]}, {function: (return kind, [argument kinds])}, [enum names]) of the header, comments and
+    preprocessor lines stripped.  An array field has the kind of its elements."""
+    src = open(os.path.join(ROOT, "include", "xpretrain_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", " ", src, flags=re.S)
+    src = "\n".join(line for line in src.splitlines() if not line.lstrip().startswith("#"))
+    structs = {}
+    for name, body in re.findall(r"typedef\s+struct\s+(\w+)\s*\{(.*?)\}\s*\1\s*;", src, flags=re.S):
+        structs[name] = [(re.findall(r"\w+", part)[-1], "pointer" if "*" in part else _c_kind(decl))
+                         for decl in body.split(";") if decl.strip()
+                         for part in re.sub(r"\[[^\]]*\]", "", decl).split(",")]
+    protos = {}
+    for chunk in src.split(";"):
+        m = re.search(r"\b(xp_\w+)\s*\(([^)]*)\)\s*$", chunk)
+        if m:
+            ret = re.split(r"[{}]", chunk[:m.start()])[-1]
+            args = [a for a in m.group(2).split(",") if a.strip() not in ("", "void")]
+            protos[m.group(1)] = (_c_kind(ret), [_c_kind(a) for a in args])
+    enums = re.findall(r"\b(XP_(?:ACT|OUT|DTYPE)_\w+)\s*=", src)
+    return structs, protos, enums
+
+
+def test_declarations_match_the_header(tmp_path):
+    """The hand-written ctypes declarations of _lib.py against include/xpretrain_b200.h, compiled by the host C compiler:
+    every struct (the ctypes ones and the XpOptTensor numpy row) with the header's field names and kinds in order, its
+    sizeof and each field's offset and size; the XP_ACT_* / XP_OUT_* / XP_DTYPE_* values and XP_ABI_VERSION; and for every
+    prototype the return kind and each argument's kind (pointer / int32_t / uint32_t / int64_t / float).  A mismatch here hands a kernel
+    wrong pointers or strides on the GPU.  Needs neither the built library nor a GPU; a missing C compiler is a failure
+    (nvcc needs one to build this project)."""
+    import ctypes as C
+    import itertools
+    import shutil
+    import subprocess
+    from xpretrain_b200 import _lib
+
+    structs, protos, enums = _header_declarations()
+    assert len(structs) >= 8 and len(protos) >= 50 and enums, "the header parse found too little"
+    bad = []
+
+    # the Python layouts: name -> (sizeof, {field: (offset, size)}, [(field, kind)] in order)
+    layouts = {}
+    for name, obj in vars(_lib).items():
+        if isinstance(obj, type) and issubclass(obj, C.Structure) and obj is not C.Structure:
+            layouts[name] = (C.sizeof(obj), {f: (getattr(obj, f).offset, getattr(obj, f).size) for f, _ in obj._fields_},
+                             [(f, _py_kind(t._type_ if issubclass(t, C.Array) else t)) for f, t in obj._fields_])
+    dt = _lib.XpOptTensor        # the numpy row keeps pointers as u8
+    np_kinds = {"u8": "pointer", "i8": "int64_t", "i4": "int32_t", "f4": "float"}
+    layouts["XpOptTensor"] = (dt.itemsize, {f: (dt.fields[f][1], dt.fields[f][0].itemsize) for f in dt.names},
+                              [(f, np_kinds.get(dt.fields[f][0].base.str[1:], dt.fields[f][0].str)) for f in dt.names])
+    if set(layouts) != set(structs):
+        bad.append(f"structs declared on one side only: Python {sorted(set(layouts) - set(structs))}, "
+                   f"header {sorted(set(structs) - set(layouts))}")
+    py_consts = {n: getattr(_lib, n) for n in dir(_lib) if re.match(r"(ACT|OUT|DTYPE)_[A-Z0-9_]+$", n)}
+    if {"XP_" + n for n in py_consts} != set(enums):
+        bad.append(f"enum constants on one side only: {sorted({'XP_' + n for n in py_consts} ^ set(enums))}")
+    py_consts["ABI_VERSION"] = _lib.ABI_VERSION
+
+    # the C side: sizeof / offsetof / field sizes / enum values, printed by a program compiled against the header
+    lines = []
+    for s in sorted(set(layouts) & set(structs)):
+        lines.append(f'printf("sizeof {s} %zu\\n", sizeof({s}));')
+        for f in sorted(set(layouts[s][1]) & {f for f, _ in structs[s]}):
+            lines.append(f'printf("field {s} {f} %zu %zu\\n", offsetof({s}, {f}), sizeof((({s}*)0)->{f}));')
+    for n in sorted(py_consts):
+        if n == "ABI_VERSION" or "XP_" + n in enums:
+            lines.append(f'printf("value {n} %lld\\n", (long long)XP_{n});')
+    prog = tmp_path / "abi_layout.c"
+    prog.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "xpretrain_b200.h"\nint main(void) {\n  '
+                    + "\n  ".join(lines) + "\n  return 0;\n}\n")
+    cc = shutil.which(os.environ.get("CC", "cc"))
+    assert cc, "no host C compiler (`cc`) found: nvcc needs one to build this project, and this test needs it too"
+    exe = tmp_path / "abi_layout"
+    r = subprocess.run([cc, "-std=c99", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)],
+                       capture_output=True, text=True)
+    assert r.returncode == 0, f"compiling the layout probe against the header failed:\n{r.stderr}"
+    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split("\n")
+
+    c_size, c_field, c_value = {}, {}, {}
+    for line in filter(None, out):
+        kind, *rest = line.split()
+        if kind == "sizeof":
+            c_size[rest[0]] = int(rest[1])
+        elif kind == "field":
+            c_field[rest[0], rest[1]] = (int(rest[2]), int(rest[3]))
+        else:
+            c_value[rest[0]] = int(rest[1])
+    for s in sorted(set(layouts) & set(structs)):
+        size, fields, order = layouts[s]
+        for i, (py, h) in enumerate(itertools.zip_longest(order, structs[s])):
+            if py != h:
+                bad.append(f"{s} field {i}: (name, kind) {py} in Python, {h} in the header")
+        if size != c_size[s]:
+            bad.append(f"{s}: sizeof {size} in Python, {c_size[s]} in the header")
+        for f in sorted(set(fields) & {f for f, _ in structs[s]}):
+            if fields[f] != c_field[s, f]:
+                bad.append(f"{s}.{f}: (offset, size) {fields[f]} in Python, {c_field[s, f]} in the header")
+    for n, v in sorted(py_consts.items()):
+        if n in c_value and c_value[n] != v:
+            bad.append(f"XP_{n}: {v} in Python, {c_value[n]} in the header")
+
+    # prototypes: the kind of the return value and of every argument
+    if set(protos) != set(_lib.SIGNATURES):
+        bad.append(f"functions declared on one side only: {sorted(set(protos) ^ set(_lib.SIGNATURES))}")
+    for fn in sorted(set(protos) & set(_lib.SIGNATURES)):
+        res, args = _lib.SIGNATURES[fn]
+        py = (_py_kind(res), [_py_kind(a) for a in args])
+        if py != protos[fn]:
+            bad.append(f"{fn}: (return, arguments) {py} in Python, {protos[fn]} in the header")
+    assert not bad, "the Python declarations disagree with include/xpretrain_b200.h:\n  " + "\n  ".join(bad)
 
 
 def test_no_cpu_fallback():

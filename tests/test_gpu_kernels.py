@@ -428,7 +428,7 @@ def test_fused_gather_nce_kernel_rank_major_rows_and_unfused_path(dev, world, b,
     read through the pointer table in rank-major order (hvd.allgather's concat order, run_pretrain.py:344-345).  Checked
     against the reference-class golden (world 4 x 8), the oracle, and the unfused multi-launch path on the same rows."""
     from oracle import clipvip_oracle as O
-    from xpretrain_b200 import _lib
+    from xpretrain_b200 import ops
     from xpretrain_b200.optimization import loss as XL
     d, N = 512, world * b
     if (world, b) == (4, 8):
@@ -451,15 +451,11 @@ def test_fused_gather_nce_kernel_rank_major_rows_and_unfused_path(dev, world, b,
     gmat = torch.zeros(N, Np, dtype=bf16, device=dev)
     vh, th = torch.empty(N, d, dtype=bf16, device=dev), torch.empty(N, d, dtype=bf16, device=dev)
     loss, dscale = torch.empty(1, device=dev), torch.empty(1, device=dev)
-    ws = torch.zeros(int(_lib.lib().xp_nce_gather_workspace_bytes(N)) // 4, device=dev)
+    ws = ops.nce_gather_workspace(N, dev)
     tdev = temp.reshape(1).to(dev)
-    a = _lib.XpNceGather()
-    a.logit_scale, a.g_scaled, a.vis_hi, a.txt_hi = tdev.data_ptr(), gmat.data_ptr(), vh.data_ptr(), th.data_ptr()
-    a.loss, a.d_logit_scale, a.workspace, a.peer_bufs = loss.data_ptr(), dscale.data_ptr(), ws.data_ptr(), ptrs.data_ptr()
-    a.rank, a.world, a.b, a.d, a.mode, a.epoch, a.ld_g = 0, world, b, d, 1, 0, Np
-    import ctypes
     for _ in range(2):           # twice: the kernel must leave its barrier counters reset
-        _lib.check(_lib.lib().xp_nce_gather_fused(ctypes.byref(a), torch.cuda.current_stream().cuda_stream), "xp_nce_gather_fused")
+        ops.nce_gather_fused(None, None, ptrs, tdev, gmat, vh, th, loss, dscale, ws, rank=0, world=world, b=b, d=d, epoch=0,
+                             mode=1)
     torch.cuda.synchronize()
     s = float(temp.exp())
     P = torch.softmax(s * V @ T.t(), 1) + torch.softmax(s * V @ T.t(), 0) - 2 * torch.eye(N)

@@ -133,8 +133,7 @@ def scale_ls(dev, ls):
 def fused_ws(dev, N):
     """The fused kernel's workspace and the float offset of its three counters (nce_fused.cu:410-414)."""
     nt = (N + 127) // 128
-    ws = torch.zeros(int(_lib().lib().xp_nce_gather_workspace_bytes(N)) // 4, dtype=f32, device=dev)
-    return ws, 4 * nt * nt * 128 + 2 * nt * nt
+    return _ops().nce_gather_workspace(N, dev), 4 * nt * nt * 128 + 2 * nt * nt
 
 
 def poison_ws(ws, off):
@@ -148,21 +147,14 @@ def counters(ws, off):
 
 def launch_fused(dev, *, world, b, d, peers, ls, ws, off, ld_g, mode=1, rank=0, epoch=0, vis_local=None, txt_local=None):
     """One xp_nce_gather_fused call into NaN-filled outputs; returns (loss, dscale, g [N, N], vis_hi, txt_hi)."""
-    lib = _lib()
     N = world * b
     assert counters(ws, off) == [0, 0, 0], "the counters must be zero before a launch"
     g, vh, th = Out(dev, N, N, bf16, ld_g), Out(dev, N, d, bf16), Out(dev, N, d, bf16)
     loss = torch.full((1,), float("nan"), device=dev)
     dscale = torch.full((1,), float("nan"), device=dev)
-    a = lib.XpNceGather()
-    a.vis_local = vis_local.data_ptr() if vis_local is not None else None
-    a.txt_local = txt_local.data_ptr() if txt_local is not None else None
-    a.peer_bufs, a.logit_scale = peers.data_ptr(), ls.data_ptr()
-    a.g_scaled, a.vis_hi, a.txt_hi = g.buf.data_ptr(), vh.buf.data_ptr(), th.buf.data_ptr()
-    a.loss, a.d_logit_scale, a.workspace = loss.data_ptr(), dscale.data_ptr(), ws.data_ptr()
-    a.rank, a.world, a.b, a.d, a.epoch, a.mode, a.ld_g = rank, world, b, d, epoch, mode, ld_g
-    lib.check(lib.lib().xp_nce_gather_fused(ctypes.byref(a), torch.cuda.current_stream().cuda_stream),
-              "xp_nce_gather_fused")
+    assert g.buf.stride(0) == ld_g
+    _ops().nce_gather_fused(vis_local, txt_local, peers, ls, g.buf, vh.buf, th.buf, loss, dscale, ws, rank=rank, world=world,
+                            b=b, d=d, epoch=epoch, mode=mode)
     torch.cuda.synchronize()
     assert counters(ws, off) == [0, 0, 0], "the fused kernel left its counters non-zero"
     return (loss.clone(), dscale.clone(), g.check("fused g_scaled"), vh.check("fused vis_hi"), th.check("fused txt_hi"))
@@ -235,11 +227,10 @@ def test_fused_kernel_exchange_mode0_simulated_on_one_gpu(dev, world, b):
     slot of every buffer hold NaN, so a missing or misplaced publish and a wrong-slot read show.  Epochs 1-3 with fresh
     rows, each as every rank: the outputs are bit-identical on every rank and to mode 1 on the same rows, the kernel
     publishes rank r's rows, and rank r's backward rows match `world` x the global gradient."""
-    lib = _lib()
     d = 256
     N = world * b
     tag = f"mode0 w{world} b{b}"
-    nbytes = int(lib.lib().xp_nce_gather_exchange_bytes(b, d, world))
+    nbytes = _ops().nce_gather_exchange_bytes(b, d, world)
     slot = 2 * b * d                                       # floats per slot: [vis b x d | txt b x d]
     bufs = [torch.zeros(nbytes // 4, dtype=f32, device=dev) for _ in range(world)]
     table = torch.tensor([x.data_ptr() for x in bufs], dtype=torch.int64, device=dev)

@@ -48,9 +48,9 @@ def _lib():
     return _lib
 
 
-def _adamw():
-    from xpretrain_b200.optimization import adamw
-    return adamw
+def _ops():
+    from xpretrain_b200 import ops
+    return ops
 
 
 class Slot:
@@ -87,38 +87,30 @@ class Set:
             r["step_size"] = O.f32(O.step_size_of(3e-4 * (1 + i % 2), BETAS, 1))
             r["decay"] = 0.0 if i % 4 == 1 else O.f32(3e-4 * 0.05)          # decay 0: the no-decay groups
             self.rows.append(r)
-        self.tab = _adamw()._Table(list(sizes), dev)
+        self.tab = _ops().OptTable(list(sizes), dev)
         self.fill()
 
     def fill(self, step_sizes=None):
         rows = self.tab.begin()
         for k in ("p", "g", "m", "v"):
             rows[k] = [r[k].t.data_ptr() for r in self.rows]
-        rows["pb"] = [r["pb"].t.data_ptr() if r["pb"] is not None else 0 for r in self.rows]
+        rows["p_bf16"] = [r["pb"].t.data_ptr() if r["pb"] is not None else 0 for r in self.rows]
         rows["step_size"] = [r["step_size"] for r in self.rows]
         rows["decay"] = [r["decay"] for r in self.rows]
         self.tab.upload()
 
     def args(self):
-        return self.tab.dev.data_ptr(), self.tab.block_map.data_ptr(), self.tab.n_blocks
+        return self.tab.launch_args
 
-    def norm(self, max_norm, stream=None):
-        lib = _lib().lib()
-        t, bm, nb = self.args()
-        _lib().check(lib.xp_opt_grad_norm(t, bm, nb, self.tab.partial.data_ptr(), float(max_norm), self.tab.norm.data_ptr(),
-                                          torch.cuda.current_stream().cuda_stream), "xp_opt_grad_norm")
+    def norm(self, max_norm):
+        _ops().opt_grad_norm(self.tab, max_norm)
         return self.tab.norm.clone()
 
     def scale(self):
-        t, bm, nb = self.args()
-        _lib().check(_lib().lib().xp_opt_scale_grads(t, bm, nb, self.tab.norm.data_ptr(),
-                                                     torch.cuda.current_stream().cuda_stream), "xp_opt_scale_grads")
+        _ops().opt_scale_grads(self.tab)
 
     def step(self, with_norm=True):
-        t, bm, nb = self.args()
-        _lib().check(_lib().lib().xp_opt_adamw_step(t, bm, nb, self.tab.norm.data_ptr() if with_norm else None,
-                                                    BETAS[0], BETAS[1], EPS, torch.cuda.current_stream().cuda_stream),
-                     "xp_opt_adamw_step")
+        _ops().opt_adamw_step(self.tab, BETAS[0], BETAS[1], EPS, clip=with_norm)
 
     def snapshot(self):
         return [{k: r[k].t.clone() for k in ("p", "g", "m", "v")} for r in self.rows]
@@ -253,18 +245,17 @@ def test_model_sized_table(dev):
 
 
 def test_cast_table_is_exact(dev):
-    adamw = _adamw()
+    ops = _ops()
     sizes = [1, 5, 8192, 8193, 3 * 8192 + 77]
     src = [torch.randn(n, device=dev) * 100 for n in sizes]
     dst = [Slot(dev, n, bf16 if i % 2 == 0 else f32, off=i % 3) for i, n in enumerate(sizes)]
-    tab = adamw._Table(sizes, dev)
+    tab = ops.OptTable(sizes, dev)
     rows = tab.begin()
     rows["g"] = [x.data_ptr() for x in src]
-    rows["pb"] = [d.t.data_ptr() if d.t.dtype == bf16 else 0 for d in dst]
+    rows["p_bf16"] = [d.t.data_ptr() if d.t.dtype == bf16 else 0 for d in dst]
     rows["p"] = [d.t.data_ptr() if d.t.dtype == f32 else 0 for d in dst]
     tab.upload()
-    _lib().check(_lib().lib().xp_cast_table(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks,
-                                            torch.cuda.current_stream().cuda_stream), "xp_cast_table")
+    ops.cast_table(tab)
     for x, d in zip(src, dst):
         assert torch.equal(bits(d.t), bits(x.to(d.t.dtype))) and d.guards_intact()
 

@@ -3,11 +3,16 @@
 There is deliberately no fallback: if `libxpretrain_b200.so` is missing, or a call is made without an
 H100 (sm_90a), the error is raised to the caller.  Build with `python -c "import __graft_entry__ as g; g.build()"`
 (or `make`) — the library is kept in-tree under xpretrain_b200/lib/.
+
+The declarations below are a hand-written copy of the header, held to it by tests/test_boundary_cpu.py; `ops.py` is
+their only caller.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+
+import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libxpretrain_b200.so")
@@ -60,6 +65,11 @@ class XpNceTerms(C.Structure):
                 ("loss", c_void_p), ("d_logit_scale", c_void_p), ("workspace", c_void_p)]
 
 
+# XpOptTensor as a numpy row type, filled column by column; `pb` (the column's earlier name) is a title: an alias
+XpOptTensor = np.dtype([("p", "<u8"), ("g", "<u8"), ("m", "<u8"), ("v", "<u8"), (("pb", "p_bf16"), "<u8"), ("n", "<i8"),
+                        ("step_size", "<f4"), ("decay", "<f4"), ("reserved", "<i4", (2,))])
+
+ABI_VERSION = 1
 ACT_NONE, ACT_QUICK_GELU, ACT_DQUICK_GELU, ACT_GELU_ERF, ACT_DGELU_ERF = 0, 1, 2, 3, 4
 OUT_BF16, OUT_F32, OUT_F32_ATOMIC = 0, 1, 2
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2

@@ -16,8 +16,7 @@ from typing import List, Tuple
 
 import torch
 
-from .. import _lib
-from .._lib import check, lib
+from .. import _lib, ops
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -32,28 +31,24 @@ class WeightMirror:
     def refresh(self, items: List[Tuple[torch.Tensor, torch.Tensor]]) -> None:
         """items: (fp32 source, destination) pairs; destinations are contiguous bf16 (cast) or fp32 (copy) views.  Per call the
         host only compares the sources' data pointers with the cached table (~0.1 ms for the 300 tensors of CLIP-ViP)."""
-        from ..optimization.adamw import _Table
         # a non-contiguous parameter (e.g. a channels_last conv weight) is gathered into a temporary on every refresh: its data
         # pointer changes, so the table is rebuilt each time — slow but correct; contiguous parameters take the cached path
         srcs = [s.detach() if s.is_contiguous() else s.detach().contiguous() for s, _ in items]
         src_key = tuple(s.data_ptr() for s in srcs)
         if src_key != self._key or len(items) != self._n:
             for s, (_, d) in zip(srcs, items):
-                if s.dtype != f32 or not s.is_cuda:
-                    raise _lib.XpError("xpretrain_b200: parameters must be fp32 CUDA tensors (there is no CPU path)")
+                if s.dtype != f32:
+                    raise _lib.XpError("xpretrain_b200: parameters must be fp32")
                 assert d.is_contiguous() and d.numel() == s.numel() and d.dtype in (bf16, f32)
-            dev = items[0][1].device
-            tab = _Table([s.numel() for s in srcs], dev)
+            g_ptrs = ops.ptrs(srcs)                         # CUDA tensors only: there is no CPU path
+            tab = ops.OptTable([s.numel() for s in srcs], items[0][1].device)
             rows = tab.begin()
-            rows["g"] = [s.data_ptr() for s in srcs]
-            rows["pb"] = [d.data_ptr() if d.dtype == bf16 else 0 for _, d in items]
-            rows["p"] = [d.data_ptr() if d.dtype == f32 else 0 for _, d in items]
+            rows["g"], rows["p"] = g_ptrs, [d.data_ptr() if d.dtype == f32 else 0 for _, d in items]
+            rows["p_bf16"] = [d.data_ptr() if d.dtype == bf16 else 0 for _, d in items]
             tab.upload()
             self._table, self._key, self._n = tab, src_key, len(items)
         self._keep = srcs          # temporaries of non-contiguous sources must outlive the launch
-        tab = self._table
-        check(lib().xp_cast_table(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks,
-                                  torch.cuda.current_stream().cuda_stream), "xp_cast_table")
+        ops.cast_table(self._table)
 
 
 def refresh_weights(model) -> None:

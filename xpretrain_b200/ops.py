@@ -1,9 +1,10 @@
 """Tensor-level wrappers over the C ABI.  PyTorch supplies device memory and the current stream only;
-every computation below runs in the hand-written sm_90a kernels of libxpretrain_b200.so."""
+every computation below runs in the hand-written sm_90a kernels of libxpretrain_b200.so.
+This is the only module that calls the library; `_lib.py` declares it."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import Iterable, List, Optional
 
 import torch
 
@@ -11,10 +12,7 @@ from . import _lib
 from ._lib import XpDenseAttn, XpGemm, XpRowMap, XpSegAttn, check, lib
 
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
+_DT = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_F16}
 
 
 def _p(t: Optional[torch.Tensor]):
@@ -23,6 +21,27 @@ def _p(t: Optional[torch.Tensor]):
     if not t.is_cuda:
         raise _lib.XpError("xpretrain_b200 kernels need CUDA tensors (there is no CPU path)")
     return t.data_ptr()
+
+
+def _call(name: str, *args) -> None:
+    """lib().<name>(*args, the current CUDA stream); XpError with the library's message on a nonzero return."""
+    check(getattr(lib(), name)(*args, torch.cuda.current_stream().cuda_stream), name)
+
+
+def _workspace(what: str, nbytes: int, device, workspace: Optional[torch.Tensor] = None, zero: bool = False):
+    """fp32 scratch of the queried nbytes for `what`: the caller's buffer, checked, or a new (zeroed) one."""
+    if nbytes < 0:
+        raise _lib.XpError(f"{what}: invalid sizes (the workspace query returned {nbytes})")
+    if workspace is None:
+        return (torch.zeros if zero else torch.empty)((nbytes + 3) // 4, dtype=f32, device=device)
+    if workspace.numel() * 4 < nbytes:
+        raise _lib.XpError(f"{what}: the workspace needs {nbytes} bytes")
+    return workspace
+
+
+def ptrs(tensors: Iterable[Optional[torch.Tensor]]) -> List[int]:
+    """Device pointers of CUDA tensors (0 for None), for the pointer columns of an OptTable."""
+    return [0 if t is None else _p(t) for t in tensors]
 
 
 def launch_count() -> int:
@@ -58,13 +77,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     g.c_group, g.c_group_stride, g.r_group, g.r_group_stride = c_group, c_group_stride, r_group, r_group_stride
     g.block_n, g.max_ctas = block_n, _sm_limit
     if _gemm_timer is None:
-        check(lib().xp_gemm(C.byref(g), _stream()), "xp_gemm")
-    else:  # bench.py's roofline leg: CUDA events on the launching stream around this launch
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        check(lib().xp_gemm(C.byref(g), _stream()), "xp_gemm")
-        e1.record()
-        _gemm_timer.append((2.0 * M * N * K, e0, e1))
+        return _call("xp_gemm", C.byref(g))
+    # bench.py's roofline leg: CUDA events on the launching stream around this launch
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    _call("xp_gemm", C.byref(g))
+    e1.record()
+    _gemm_timer.append((2.0 * M * N * K, e0, e1))
 
 
 _gemm_timer = None
@@ -128,45 +147,38 @@ def linear_wgrad(dy: torch.Tensor, x: torch.Tensor, dw: torch.Tensor, alpha: flo
 
 # ------------------------------------------------------------------------------------ row kernels
 def rowmap(ld: int, group: int = 0, group_stride: int = 0, offsets: Optional[torch.Tensor] = None) -> XpRowMap:
-    m = XpRowMap()
-    m.group, m.group_stride, m.ld, m.offsets = group, group_stride, ld, _p(offsets)
-    return m
+    return XpRowMap(group=group, group_stride=group_stride, ld=ld, offsets=_p(offsets))
 
 
 def layernorm_fwd(x, xmap, y, ymap, gamma, beta, mean, rstd, rows: int, C_: int, eps: float, x_off=0, y_off=0,
                   add=None, addmap=None, add_off=0, sum_out=None, summap=None):
     """y = LayerNorm(x (+ add)); offsets in ELEMENTS of the respective tensor.  x / y may be bf16 or fp32 (the fp32 residual
     stream); `add` is the bf16 branch output folded in before the normalisation, `sum_out` (fp32) receives x + add."""
-    dt = {torch.bfloat16: _lib.DTYPE_BF16, torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16}
     assert add is None or add.dtype == bf16
     assert sum_out is None or sum_out.dtype == (torch.float16 if x.dtype == torch.float16 else f32)
-    check(lib().xp_layernorm_add_fwd(_p(x) + x_off * x.element_size(), C.byref(xmap), dt[x.dtype],
-                                     (_p(add) + add_off * 2) if add is not None else None,
-                                     C.byref(addmap) if addmap is not None else None, _p(sum_out),
-                                     C.byref(summap) if summap is not None else None, _p(y) + y_off * y.element_size(),
-                                     C.byref(ymap), dt[y.dtype], _p(gamma), _p(beta), _p(mean), _p(rstd), rows, C_, eps,
-                                     _stream()), "xp_layernorm_add_fwd")
+    _call("xp_layernorm_add_fwd", _p(x) + x_off * x.element_size(), C.byref(xmap), _DT[x.dtype],
+          (_p(add) + add_off * 2) if add is not None else None, C.byref(addmap) if addmap is not None else None,
+          _p(sum_out), C.byref(summap) if summap is not None else None, _p(y) + y_off * y.element_size(), C.byref(ymap),
+          _DT[y.dtype], _p(gamma), _p(beta), _p(mean), _p(rstd), rows, C_, eps)
 
 
 def layernorm_bwd(dy, dymap, x, xmap, gamma, mean, rstd, dres, drmap, dx, dxmap, dgamma, dbeta, rows: int, C_: int,
                   dy_off=0, x_off=0, dres_off=0, dx_off=0, dres_colsum=None):
     """x: the saved LayerNorm input, bf16, fp32 or fp16; dy / dres / dx bf16.  Offsets in elements."""
-    dt = {torch.bfloat16: _lib.DTYPE_BF16, torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16}
-    check(lib().xp_layernorm_bwd(_p(dy) + dy_off * 2, C.byref(dymap), _p(x) + x_off * x.element_size(), C.byref(xmap),
-                                 dt[x.dtype], _p(gamma), _p(mean), _p(rstd),
-                                 (_p(dres) + dres_off * 2) if dres is not None else None,
-                                 C.byref(drmap) if drmap is not None else None, _p(dx) + dx_off * 2, C.byref(dxmap),
-                                 _p(dgamma), _p(dbeta), _p(dres_colsum), rows, C_, _stream()), "xp_layernorm_bwd")
+    _call("xp_layernorm_bwd", _p(dy) + dy_off * 2, C.byref(dymap), _p(x) + x_off * x.element_size(), C.byref(xmap),
+          _DT[x.dtype], _p(gamma), _p(mean), _p(rstd), (_p(dres) + dres_off * 2) if dres is not None else None,
+          C.byref(drmap) if drmap is not None else None, _p(dx) + dx_off * 2, C.byref(dxmap), _p(dgamma), _p(dbeta),
+          _p(dres_colsum), rows, C_)
 
 
 def l2norm_fwd(x, y, inv_norm):
     rows, C_ = x.shape
-    check(lib().xp_l2norm_fwd(_p(x), _p(y), _p(inv_norm), rows, C_, _stream()), "xp_l2norm_fwd")
+    _call("xp_l2norm_fwd", _p(x), _p(y), _p(inv_norm), rows, C_)
 
 
 def l2norm_bwd(dy, y, inv_norm, dx_bf16, scale: float = 1.0):
     rows, C_ = y.shape
-    check(lib().xp_l2norm_bwd(_p(dy), _p(y), _p(inv_norm), _p(dx_bf16), rows, C_, scale, _stream()), "xp_l2norm_bwd")
+    _call("xp_l2norm_bwd", _p(dy), _p(y), _p(inv_norm), _p(dx_bf16), rows, C_, scale)
 
 
 def frame_pool_fwd(proj, feat, inv_frame, inv_video, T: int):
@@ -176,8 +188,7 @@ def frame_pool_fwd(proj, feat, inv_frame, inv_video, T: int):
     B = feat.shape[0]
     assert proj.dtype == f32 and feat.dtype == f32 and proj.is_contiguous() and feat.is_contiguous()
     assert rows == B * T and feat.shape[1] == P and inv_frame.numel() == rows and inv_video.numel() == B
-    check(lib().xp_frame_pool_fwd(_p(proj), _p(feat), _p(inv_frame), _p(inv_video), B, T, P, _stream()),
-          "xp_frame_pool_fwd")
+    _call("xp_frame_pool_fwd", _p(proj), _p(feat), _p(inv_frame), _p(inv_video), B, T, P)
 
 
 def frame_pool_bwd(dfeat, feat, proj, inv_frame, inv_video, dproj_bf16, T: int, scale: float = 1.0):
@@ -185,34 +196,30 @@ def frame_pool_bwd(dfeat, feat, proj, inv_frame, inv_video, dproj_bf16, T: int, 
     B, P = feat.shape
     assert dfeat.dtype == f32 and dfeat.is_contiguous() and dfeat.shape == feat.shape
     assert dproj_bf16.dtype == bf16 and dproj_bf16.is_contiguous() and dproj_bf16.shape == (B * T, P)
-    check(lib().xp_frame_pool_bwd(_p(dfeat), _p(feat), _p(proj), _p(inv_frame), _p(inv_video), _p(dproj_bf16), B, T, P,
-                                  scale, _stream()), "xp_frame_pool_bwd")
+    _call("xp_frame_pool_bwd", _p(dfeat), _p(feat), _p(proj), _p(inv_frame), _p(inv_video), _p(dproj_bf16), B, T, P, scale)
 
 
 def colsum(x: torch.Tensor, out: torch.Tensor, scale: float = 1.0):
     rows, C_ = x.shape
-    check(lib().xp_colsum_bf16(_p(x), x.stride(0), _p(out), rows, C_, scale, _stream()), "xp_colsum_bf16")
+    _call("xp_colsum_bf16", _p(x), x.stride(0), _p(out), rows, C_, scale)
 
 
 def cast_bf16(src: torch.Tensor, dst: torch.Tensor, dst_offset: int = 0):
     assert src.dtype == f32 and dst.dtype == bf16 and src.is_contiguous()
-    check(lib().xp_cast_f32_bf16(_p(src), _p(dst) + dst_offset * 2, src.numel(), _stream()), "xp_cast_f32_bf16")
+    _call("xp_cast_f32_bf16", _p(src), _p(dst) + dst_offset * 2, src.numel())
 
 
 # ------------------------------------------------------------------------------------- embeddings
-_DT = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_F16}
-
-
 def patch_pitch(patch: int) -> int:
     """Row pitch (elements) of the bf16 patch matrix: 3*p*p rounded up to a multiple of 8, so that rows are 16-byte aligned
     for TMA; the pad columns are zero.  Equal to 3*p*p for p = 16 and 32; 592 for p = 14."""
     return (3 * patch * patch + 7) // 8 * 8
 
 
-def _aligned_input(x: torch.Tensor, nbytes: int = 16) -> torch.Tensor:
-    """x contiguous with an nbytes-aligned data pointer: the embedding kernels read their inputs in vectors, and a contiguous
-    view (e.g. `video[:, 1:]` of a one-frame-longer buffer, or an offset slice of a flat buffer) need not start aligned.
-    A misaligned input is copied; the kernel computes the same bits from the copy."""
+def aligned_input(x: torch.Tensor, nbytes: int = 16) -> torch.Tensor:
+    """x contiguous with an nbytes-aligned data pointer: the embedding and fused-NCE kernels read their inputs in vectors,
+    and a contiguous view (e.g. `video[:, 1:]` of a one-frame-longer buffer, or an offset slice of a flat buffer) need not
+    start aligned.  A misaligned input is copied; the kernel computes the same bits from the copy."""
     x = x.contiguous()
     return x if x.data_ptr() % nbytes == 0 else x.clone()
 
@@ -226,10 +233,9 @@ def _aligned_output(x: torch.Tensor, nbytes: int, what: str) -> None:
 
 def vip_patchify(video: torch.Tensor, patches: torch.Tensor, patch: int):
     _aligned_output(patches, 16, "vip_patchify")
-    video = _aligned_input(video)
+    video = aligned_input(video)
     frames = video.numel() // (3 * video.shape[-2] * video.shape[-1])
-    check(lib().xp_vip_patchify(_p(video), _DT[video.dtype], _p(patches), frames, video.shape[-2], video.shape[-1], patch,
-                                _stream()), "xp_vip_patchify")
+    _call("xp_vip_patchify", _p(video), _DT[video.dtype], _p(patches), frames, video.shape[-2], video.shape[-1], patch)
 
 
 CLIP_MEAN, CLIP_STD = (0.48145466, 0.4578275, 0.40821073), (0.26862954, 0.26130258, 0.27577711)   # dataloader.py:213-214
@@ -239,74 +245,66 @@ def vip_patchify_u8(frames_hwc: torch.Tensor, patches: torch.Tensor, patch: int,
     """frames_hwc uint8 [..., H, W, 3] -> normalised bf16 patch matrix (the reference's /255 + Normalize fused in)."""
     assert frames_hwc.dtype == torch.uint8 and frames_hwc.is_contiguous() and frames_hwc.shape[-1] == 3
     _aligned_output(patches, 16, "vip_patchify_u8")
-    frames_hwc = _aligned_input(frames_hwc, 8)
+    frames_hwc = aligned_input(frames_hwc, 8)
     H, W = frames_hwc.shape[-3], frames_hwc.shape[-2]
     n = frames_hwc.numel() // (3 * H * W)
     m3, s3 = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
-    check(lib().xp_vip_patchify_u8(_p(frames_hwc), _p(patches), n, H, W, patch, m3, s3, _stream()), "xp_vip_patchify_u8")
+    _call("xp_vip_patchify_u8", _p(frames_hwc), _p(patches), n, H, W, patch, m3, s3)
 
 
 def vip_embed_tables(pos, temporal, cls, added, table, x, B, T, L, M, C_, temporal_size):
-    check(lib().xp_vip_embed_tables(_p(pos), _p(temporal), _p(cls), _p(added), _p(table), _p(x), B, T, L, M, C_,
-                                    temporal_size, _stream()), "xp_vip_embed_tables")
+    _call("xp_vip_embed_tables", _p(pos), _p(temporal), _p(cls), _p(added), _p(table), _p(x), B, T, L, M, C_, temporal_size)
 
 
 def vip_embed_bwd(d_patch, d_global, d_pos, d_temporal, d_cls, d_added, B, T, L, M, C_, temporal_size):
     """Adds (fp32 atomics: not bitwise repeatable) the embedding gradients into d_pos and the optional d_temporal, d_cls,
     d_added (None = not wanted)."""
-    d_patch, d_global = _aligned_input(d_patch), _aligned_input(d_global)
-    check(lib().xp_vip_embed_bwd(_p(d_patch), _p(d_global), _p(d_pos), _p(d_temporal), _p(d_cls), _p(d_added), B, T, L, M,
-                                 C_, temporal_size, _stream()), "xp_vip_embed_bwd")
+    d_patch, d_global = aligned_input(d_patch), aligned_input(d_global)
+    _call("xp_vip_embed_bwd", _p(d_patch), _p(d_global), _p(d_pos), _p(d_temporal), _p(d_cls), _p(d_added), B, T, L, M, C_,
+          temporal_size)
 
 
 def text_embed_fwd(ids, tok, pos, x, Lt, err_flag):
     _aligned_output(x, 8, "text_embed_fwd")
-    tok, pos = _aligned_input(tok), _aligned_input(pos)
+    tok, pos = aligned_input(tok), aligned_input(pos)
     rows = ids.numel()
-    check(lib().xp_text_embed_fwd(_p(ids), _p(tok), _p(pos), _p(x), rows, Lt, tok.shape[1], tok.shape[0], _p(err_flag),
-                                  _stream()), "xp_text_embed_fwd")
+    _call("xp_text_embed_fwd", _p(ids), _p(tok), _p(pos), _p(x), rows, Lt, tok.shape[1], tok.shape[0], _p(err_flag))
 
 
 def text_embed_bwd(ids, dx, d_tok, d_pos, Lt, C_, vocab):
-    check(lib().xp_text_embed_bwd(_p(ids), _p(dx), _p(d_tok), _p(d_pos), ids.numel(), Lt, C_, vocab, _stream()),
-          "xp_text_embed_bwd")
+    _call("xp_text_embed_bwd", _p(ids), _p(dx), _p(d_tok), _p(d_pos), ids.numel(), Lt, C_, vocab)
 
 
 def eos_offsets(ids, offsets, index, C_):
     B, Lt = ids.shape
-    check(lib().xp_eos_offsets(_p(ids), _p(offsets), _p(index), B, Lt, C_, _stream()), "xp_eos_offsets")
+    _call("xp_eos_offsets", _p(ids), _p(offsets), _p(index), B, Lt, C_)
 
 
 # -------------------------------------------------------------------------------------- attention
 def vip_attention_workspace(B, H, T, M, device) -> torch.Tensor:
-    n = int(lib().xp_vip_attention_workspace_bytes(B, H, T, M))
-    return torch.empty(n // 4, dtype=f32, device=device)
+    return _workspace("xp_vip_attention", lib().xp_vip_attention_workspace_bytes(B, H, T, M), device)
 
 
 def vip_attention_fwd(qkv, out, lse, ws, B, H, T, L, M, C_):
-    check(lib().xp_vip_attention_fwd(_p(qkv), _p(out), _p(lse), _p(ws), B, H, T, L, M, C_, _stream()),
-          "xp_vip_attention_fwd")
+    _call("xp_vip_attention_fwd", _p(qkv), _p(out), _p(lse), _p(ws), B, H, T, L, M, C_)
 
 
 def vip_attention_bwd(qkv, out, dout, lse, dqkv, ws, B, H, T, L, M, C_, q_scale):
-    check(lib().xp_vip_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(dqkv), _p(ws), B, H, T, L, M, C_, q_scale,
-                                     _stream()), "xp_vip_attention_bwd")
+    _call("xp_vip_attention_bwd", _p(qkv), _p(out), _p(dout), _p(lse), _p(dqkv), _p(ws), B, H, T, L, M, C_, q_scale)
 
 
 def text_attention_fwd(qkv, mask, out, probs, B, H, Lt, C_):
-    check(lib().xp_text_attention_fwd(_p(qkv), _p(mask), _p(out), _p(probs), B, H, Lt, C_, _stream()),
-          "xp_text_attention_fwd")
+    _call("xp_text_attention_fwd", _p(qkv), _p(mask), _p(out), _p(probs), B, H, Lt, C_)
 
 
 def text_attention_bwd(qkv, dout, probs, dqkv, B, H, Lt, C_, q_scale):
-    check(lib().xp_text_attention_bwd(_p(qkv), _p(dout), _p(probs), _p(dqkv), B, H, Lt, C_, q_scale, _stream()),
-          "xp_text_attention_bwd")
+    _call("xp_text_attention_bwd", _p(qkv), _p(dout), _p(probs), _p(dqkv), B, H, Lt, C_, q_scale)
 
 
 # -------------------------------------------------------------------------------------------- NCE
 def nce_split(x, x3, hi, pattern: int):
     rows, d = x.shape
-    check(lib().xp_nce_split(_p(x), _p(x3), _p(hi), rows, d, pattern, _stream()), "xp_nce_split")
+    _call("xp_nce_split", _p(x), _p(x3), _p(hi), rows, d, pattern)
 
 
 def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logit_scale=None, workspace=None):
@@ -322,14 +320,8 @@ def nce_terms(z, g, terms, loss, *, logit_scale=None, scale: float = 1.0, d_logi
     for t, (axis, members, excl, target) in enumerate(terms):
         a.term[t].axis, a.term[t].members, a.term[t].excl_diag, a.term[t].target = axis, members, excl, target
     a.logit_scale, a.scale, a.loss, a.d_logit_scale = _p(logit_scale), scale, _p(loss), _p(d_logit_scale)
-    nbytes = int(lib().xp_nce_terms_workspace_bytes(C.byref(a)))
-    if nbytes < 0:
-        raise _lib.XpError("xp_nce_terms_workspace_bytes: invalid matrix sizes")
-    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z[0].device) if workspace is None else workspace
-    if ws.numel() * 4 < nbytes:
-        raise _lib.XpError(f"xp_nce_terms: the workspace needs {nbytes} bytes")
-    a.workspace = _p(ws)
-    check(lib().xp_nce_terms(C.byref(a), _stream()), "xp_nce_terms")
+    a.workspace = _p(_workspace("xp_nce_terms", lib().xp_nce_terms_workspace_bytes(C.byref(a)), z[0].device, workspace))
+    _call("xp_nce_terms", C.byref(a))
 
 
 def nce_dsl(z, logit_scale, g, loss, d_logit_scale, workspace=None):
@@ -337,24 +329,36 @@ def nce_dsl(z, logit_scale, g, loss, d_logit_scale, workspace=None):
     workspace: fp32, at least xp_nce_dsl_workspace_bytes(n); allocated here when None."""
     n, ld = z.shape[0], z.stride(0)
     assert z.dtype == f32 and g.dtype == bf16 and g.stride(0) == ld
-    nbytes = int(lib().xp_nce_dsl_workspace_bytes(n))
-    if nbytes < 0:
-        raise _lib.XpError("xp_nce_dsl_workspace_bytes: n must be positive")
-    ws = torch.empty((nbytes + 3) // 4, dtype=f32, device=z.device) if workspace is None else workspace
-    if ws.numel() * 4 < nbytes:
-        raise _lib.XpError(f"xp_nce_dsl: the workspace needs {nbytes} bytes")
-    check(lib().xp_nce_dsl(_p(z), ld, n, _p(logit_scale), _p(g), _p(loss), _p(d_logit_scale), _p(ws), _stream()),
-          "xp_nce_dsl")
+    ws = _workspace("xp_nce_dsl", lib().xp_nce_dsl_workspace_bytes(n), z.device, workspace)
+    _call("xp_nce_dsl", _p(z), ld, n, _p(logit_scale), _p(g), _p(loss), _p(d_logit_scale), _p(ws))
+
+
+def nce_gather_exchange_bytes(b: int, d: int, world: int) -> int:
+    """Size of one rank's exchange buffer of the fused gather + InfoNCE (mode 0)."""
+    return int(lib().xp_nce_gather_exchange_bytes(b, d, world))
+
+
+def nce_gather_workspace(N: int, device) -> torch.Tensor:
+    """Zeroed workspace of the fused gather + InfoNCE for N global rows; every launch leaves its counters zero again."""
+    return _workspace("xp_nce_gather_fused", lib().xp_nce_gather_workspace_bytes(N), device, zero=True)
+
+
+def nce_gather_fused(vis_local, txt_local, peer_bufs, logit_scale, g, vis_hi, txt_hi, loss, d_logit_scale, workspace, *,
+                     rank: int, world: int, b: int, d: int, epoch: int, mode: int):
+    """The fused embedding exchange + InfoNCE over N = world * b rows (xp_nce_gather_fused; modes as in the header);
+    g: bf16 [N, ld_g] receives exp(logit_scale) * dL/dZ.  Every row pointer must be 16-byte aligned."""
+    a = _lib.XpNceGather(vis_local=_p(vis_local), txt_local=_p(txt_local), peer_bufs=_p(peer_bufs),
+                         logit_scale=_p(logit_scale), g_scaled=_p(g), vis_hi=_p(vis_hi), txt_hi=_p(txt_hi), loss=_p(loss),
+                         d_logit_scale=_p(d_logit_scale), workspace=_p(workspace), rank=rank, world=world, b=b, d=d,
+                         epoch=epoch, mode=mode, ld_g=g.stride(0))
+    _call("xp_nce_gather_fused", C.byref(a))
 
 
 # ------------------------------------------------------------- config #4: TimeSformer (HD-VILA)
 def seg_desc(n_rows: int, heads: int, ld_qkv: int, ld_out: int, *, n_seq: int, seq_len: int, seg_len: int, inner: int,
              outer_stride: int, inner_stride: int, tok_stride: int) -> XpSegAttn:
-    d = XpSegAttn()
-    d.n_rows, d.ld_qkv, d.ld_out = n_rows, ld_qkv, ld_out
-    d.outer_stride, d.inner_stride, d.tok_stride = outer_stride, inner_stride, tok_stride
-    d.heads, d.n_seq, d.seq_len, d.seg_len, d.inner, d.reserved = heads, n_seq, seq_len, seg_len, inner, 0
-    return d
+    return XpSegAttn(n_rows=n_rows, ld_qkv=ld_qkv, ld_out=ld_out, outer_stride=outer_stride, inner_stride=inner_stride,
+                     tok_stride=tok_stride, heads=heads, n_seq=n_seq, seq_len=seq_len, seg_len=seg_len, inner=inner)
 
 
 def window_desc(n_rows: int, heads: int, head_dim: int, ld_qkv: int, ld_out: int, row_index: torch.Tensor,
@@ -392,42 +396,36 @@ def spatial_desc(B: int, T: int, HW: int, heads: int, ld_qkv: int, ld_out: int) 
 
 
 def seg_attention_fwd(qkv, out, lse, desc: XpSegAttn):
-    check(lib().xp_seg_attention_fwd(_p(qkv), _p(out), _p(lse), C.byref(desc), _stream()), "xp_seg_attention_fwd")
+    _call("xp_seg_attention_fwd", _p(qkv), _p(out), _p(lse), C.byref(desc))
 
 
 def seg_attention_bwd(qkv, out, dout, lse, delta, dqkv, desc: XpSegAttn, q_scale: float):
-    check(lib().xp_seg_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale,
-                                     _stream()), "xp_seg_attention_bwd")
+    _call("xp_seg_attention_bwd", _p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale)
 
 
 def dense_desc(n_rows: int, heads: int, ld_qkv: int, ld_out: int, *, n_seq: int, seq_len: int) -> XpDenseAttn:
     """n_seq sequences of seq_len consecutive rows, every row attending to every row of its sequence: one clip of H*W*T
     tokens ('joint_space_time', timesformer.py:202-205) or one frame of H*W tokens ('space_only')."""
-    d = XpDenseAttn()
-    d.n_rows, d.ld_qkv, d.ld_out = n_rows, ld_qkv, ld_out
-    d.heads, d.n_seq, d.seq_len, d.reserved = heads, n_seq, seq_len, 0
-    return d
+    return XpDenseAttn(n_rows=n_rows, ld_qkv=ld_qkv, ld_out=ld_out, heads=heads, n_seq=n_seq, seq_len=seq_len)
 
 
 def dense_attention_fwd(qkv, out, lse, desc: XpDenseAttn):
-    check(lib().xp_dense_attention_fwd(_p(qkv), _p(out), _p(lse), C.byref(desc), _stream()), "xp_dense_attention_fwd")
+    _call("xp_dense_attention_fwd", _p(qkv), _p(out), _p(lse), C.byref(desc))
 
 
 def dense_attention_bwd(qkv, out, dout, lse, delta, dqkv, desc: XpDenseAttn, q_scale: float):
-    check(lib().xp_dense_attention_bwd(_p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale,
-                                       _stream()), "xp_dense_attention_bwd")
+    _call("xp_dense_attention_bwd", _p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), C.byref(desc), q_scale)
 
 
 def tsf_embed_fwd(x, pos, time, tokens, B, T, C_, HW):
-    check(lib().xp_tsf_embed_fwd(_p(x), _DT[x.dtype], _p(pos), _p(time), _p(tokens), B, T, C_, HW, _stream()),
-          "xp_tsf_embed_fwd")
+    _call("xp_tsf_embed_fwd", _p(x), _DT[x.dtype], _p(pos), _p(time), _p(tokens), B, T, C_, HW)
 
 
 def rowscale(x, scale, out, residual=None):
     """out = (residual or 0) + scale[:, None] * x  (DropPath on a residual branch); out may alias x."""
     rows, C_ = x.shape
     assert scale.dtype == f32 and scale.numel() == rows and x.is_contiguous() and out.is_contiguous()
-    check(lib().xp_rowscale_bf16(_p(x), _p(scale), _p(residual), _p(out), rows, C_, _stream()), "xp_rowscale_bf16")
+    _call("xp_rowscale_bf16", _p(x), _p(scale), _p(residual), _p(out), rows, C_)
 
 
 def layernorm_any_fwd(x, y, gamma, beta, mean, rstd, rows: int, C_: int, eps: float):
@@ -436,8 +434,7 @@ def layernorm_any_fwd(x, y, gamma, beta, mean, rstd, rows: int, C_: int, eps: fl
         m = rowmap(C_)
         layernorm_fwd(x, m, y, m, gamma, beta, mean, rstd, rows, C_, eps)
     else:
-        check(lib().xp_layernorm_wide_fwd(_p(x), _p(y), _p(gamma), _p(beta), _p(mean), _p(rstd), rows, C_, eps, _stream()),
-              "xp_layernorm_wide_fwd")
+        _call("xp_layernorm_wide_fwd", _p(x), _p(y), _p(gamma), _p(beta), _p(mean), _p(rstd), rows, C_, eps)
 
 
 def layernorm_any_bwd(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta, rows: int, C_: int):
@@ -446,21 +443,87 @@ def layernorm_any_bwd(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta, rows: i
         layernorm_bwd(dy, m, x, m, gamma, mean, rstd, dres, m if dres is not None else None, dx, m, dgamma, dbeta, rows, C_)
     else:
         assert dres is None
-        check(lib().xp_layernorm_wide_bwd(_p(dy), _p(x), _p(gamma), _p(mean), _p(rstd), _p(dx), _p(dgamma), _p(dbeta), rows,
-                                          C_, _stream()), "xp_layernorm_wide_bwd")
+        _call("xp_layernorm_wide_bwd", _p(dy), _p(x), _p(gamma), _p(mean), _p(rstd), _p(dx), _p(dgamma), _p(dbeta), rows,
+              C_)
 
 
 def gather_rows(src, index, out, C_: int):
     """out.view(-1, C)[i] = src[index[i]] (zeros for index < 0); index int32."""
     assert index.dtype == torch.int32 and index.is_contiguous() and out.numel() == index.numel() * C_
-    check(lib().xp_gather_rows_bf16(_p(src), _p(index), _p(out), index.numel(), C_, _stream()), "xp_gather_rows_bf16")
+    _call("xp_gather_rows_bf16", _p(src), _p(index), _p(out), index.numel(), C_)
 
 
 def scatter_rows(inp, index, dst, C_: int):
     """dst[index[i]] = inp.view(-1, C)[i] for index >= 0."""
     assert index.dtype == torch.int32 and index.is_contiguous() and inp.numel() == index.numel() * C_
-    check(lib().xp_scatter_rows_bf16(_p(inp), _p(index), _p(dst), index.numel(), C_, _stream()), "xp_scatter_rows_bf16")
+    _call("xp_scatter_rows_bf16", _p(inp), _p(index), _p(dst), index.numel(), C_)
 
 
 def tsf_untokenize(tokens, x, B, T, C_, HW):
-    check(lib().xp_tsf_untokenize(_p(tokens), _p(x), _DT[x.dtype], B, T, C_, HW, _stream()), "xp_tsf_untokenize")
+    _call("xp_tsf_untokenize", _p(tokens), _p(x), _DT[x.dtype], B, T, C_, HW)
+
+
+# ------------------------------------------------------------------------------------- retrieval
+def sim_f32(a, b, out):
+    """out[Na, Nb] (row pitch out.stride(0)) = a[Na, d] @ b[Nb, d]^T, fp32 FFMA accumulation."""
+    _call("xp_sim_f32", _p(a), _p(b), _p(out), a.shape[0], b.shape[0], a.shape[1], out.stride(0))
+
+
+def dsl_reweight(sim, theta: float, scratch):
+    """sim *= softmax(theta * sim, axis=0) in place; scratch: 2 * cols fp32."""
+    _call("xp_dsl_reweight", _p(sim), sim.shape[0], sim.shape[1], sim.stride(0), float(theta), _p(scratch))
+
+
+def rank_counts(sim, transpose: bool, greater, equal):
+    """greater[i] / equal[i] = entries of row (column) i of the square sim larger than / equal to sim[i, i]."""
+    _call("xp_rank_counts", _p(sim), sim.shape[0], sim.stride(0), 1 if transpose else 0, _p(greater), _p(equal))
+
+
+# ------------------------------------------------------------------------------------- optimizer
+class OptTable:
+    """Device-side XpOptTensor table + block map for a fixed list of tensors (sizes never change; pointers, step sizes
+    and decays are rewritten every step through a pinned staging buffer)."""
+
+    def __init__(self, numels: List[int], device: torch.device):
+        chunk = int(lib().xp_opt_chunk_elems())
+        blocks = [(i, c) for i, n in enumerate(numels) for c in range((n + chunk - 1) // chunk)]
+        self.n_blocks = len(blocks)
+        self.block_map = torch.tensor(blocks, dtype=torch.int32).reshape(-1, 2).to(device)
+        self.host = torch.empty(len(numels) * _lib.XpOptTensor.itemsize, dtype=torch.uint8).pin_memory()
+        self.rows = self.host.numpy().view(_lib.XpOptTensor)
+        self.dev = torch.empty(self.host.shape, dtype=torch.uint8, device=device)
+        self.partial = torch.empty(max(self.n_blocks, 1), dtype=torch.float32, device=device)
+        self.norm = torch.zeros(2, dtype=torch.float32, device=device)
+        self.rows["n"] = numels
+        self.copied = torch.cuda.Event()
+        self.copied.record()
+        self.launch_args = (_p(self.dev), _p(self.block_map), self.n_blocks)     # leading arguments of every launch
+
+    def begin(self):
+        """Wait until the previous asynchronous upload has left the pinned staging buffer before rewriting it."""
+        self.copied.synchronize()
+        return self.rows
+
+    def upload(self):
+        self.dev.copy_(self.host, non_blocking=True)
+        self.copied.record()
+
+
+def opt_grad_norm(tab: OptTable, max_norm: float):
+    """tab.norm = (2-norm over every g of the table, clip coefficient for max_norm)."""
+    _call("xp_opt_grad_norm", *tab.launch_args, _p(tab.partial), float(max_norm), _p(tab.norm))
+
+
+def opt_scale_grads(tab: OptTable):
+    """g *= tab.norm[1] in place for every g of the table."""
+    _call("xp_opt_scale_grads", *tab.launch_args, _p(tab.norm))
+
+
+def opt_adamw_step(tab: OptTable, beta1: float, beta2: float, eps: float, clip: bool):
+    """The fused AdamW update of every row; with clip, g is scaled by the coefficient opt_grad_norm left in tab.norm."""
+    _call("xp_opt_adamw_step", *tab.launch_args, _p(tab.norm) if clip else None, beta1, beta2, eps)
+
+
+def cast_table(tab: OptTable):
+    """Per row: g (fp32 source) -> p_bf16 (bf16 destination) or, if that is null, p (fp32 copy)."""
+    _call("xp_cast_table", *tab.launch_args)

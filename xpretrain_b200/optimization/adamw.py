@@ -15,63 +15,23 @@ There is no CPU path: parameters must be fp32 CUDA tensors.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
-from typing import Dict, Iterable, List, Optional
+from typing import Dict, Iterable, Optional
 
-import numpy as np
 import torch
 from torch.optim import Optimizer
 
-from .. import _lib
-from .._lib import check, lib
-
-_ROW = np.dtype([("p", "<u8"), ("g", "<u8"), ("m", "<u8"), ("v", "<u8"), ("pb", "<u8"), ("n", "<i8"),
-                 ("step_size", "<f4"), ("decay", "<f4"), ("reserved", "<i4", (2,))])
-assert _ROW.itemsize == 64
-
-
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
-
-
-class _Table:
-    """Device-side XpOptTensor table + block map for a fixed list of tensors (sizes never change; pointers, step sizes
-    and decays are rewritten every step through a pinned staging buffer)."""
-
-    def __init__(self, numels: List[int], device: torch.device):
-        chunk = int(lib().xp_opt_chunk_elems())
-        blocks = [(i, c) for i, n in enumerate(numels) for c in range((n + chunk - 1) // chunk)]
-        self.n_blocks = len(blocks)
-        self.n = len(numels)
-        self.block_map = torch.tensor(blocks, dtype=torch.int32).reshape(-1, 2).to(device)
-        self.host = torch.empty(self.n * 64, dtype=torch.uint8).pin_memory()
-        self.rows = self.host.numpy().view(_ROW)
-        self.dev = torch.empty(self.n * 64, dtype=torch.uint8, device=device)
-        self.partial = torch.empty(max(self.n_blocks, 1), dtype=torch.float32, device=device)
-        self.norm = torch.zeros(2, dtype=torch.float32, device=device)
-        self.rows["n"] = numels
-        self.copied = torch.cuda.Event()
-        self.copied.record()
-
-    def begin(self):
-        """Wait until the previous asynchronous upload has left the pinned staging buffer before rewriting it."""
-        self.copied.synchronize()
-        return self.rows
-
-    def upload(self):
-        self.dev.copy_(self.host, non_blocking=True)
-        self.copied.record()
+from .. import ops
+from .._lib import XpError
 
 
 def _check_tensor(t: torch.Tensor, what: str):
-    if not t.is_cuda:
-        raise _lib.XpError(f"xpretrain_b200 optimizer: {what} must be a CUDA tensor (there is no CPU path)")
     if t.dtype != torch.float32 or not t.is_contiguous():
-        raise _lib.XpError(f"xpretrain_b200 optimizer: {what} must be contiguous fp32")
+        raise XpError(f"xpretrain_b200 optimizer: {what} must be contiguous fp32")
 
 
-_clip_tables: Dict[tuple, _Table] = {}
+_Table = ops.OptTable          # the table's earlier name here, kept for code that still builds tables through it
+_clip_tables: Dict[tuple, ops.OptTable] = {}
 
 
 def clip_grad_norm_(parameters: Iterable[torch.Tensor], max_norm: float) -> torch.Tensor:
@@ -86,16 +46,15 @@ def clip_grad_norm_(parameters: Iterable[torch.Tensor], max_norm: float) -> torc
             p.grad = p.grad.contiguous()
         _check_tensor(p.grad, "gradient")
         grads.append(p.grad)
+    g_ptrs = ops.ptrs(grads)                                # CUDA tensors only: refused before any table is built
     key = (tuple(g.numel() for g in grads), grads[0].device)
     tab = _clip_tables.get(key)
     if tab is None:
-        tab = _clip_tables[key] = _Table(list(key[0]), grads[0].device)
-    tab.begin()["g"] = [g.data_ptr() for g in grads]
+        tab = _clip_tables[key] = ops.OptTable(list(key[0]), grads[0].device)
+    tab.begin()["g"] = g_ptrs
     tab.upload()
-    check(lib().xp_opt_grad_norm(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks, tab.partial.data_ptr(),
-                                 float(max_norm), tab.norm.data_ptr(), _stream()), "xp_opt_grad_norm")
-    check(lib().xp_opt_scale_grads(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks, tab.norm.data_ptr(),
-                                   _stream()), "xp_opt_scale_grads")
+    ops.opt_grad_norm(tab, max_norm)
+    ops.opt_scale_grads(tab)
     return tab.norm[0].clone()
 
 
@@ -112,7 +71,7 @@ class AdamW(Optimizer):
         if not 0.0 <= eps:
             raise ValueError("Invalid epsilon value: {} - should be >= 0.0".format(eps))
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias))
-        self._tables: Dict[tuple, _Table] = {}
+        self._tables: Dict[tuple, ops.OptTable] = {}
         self.bf16_targets: Dict[int, torch.Tensor] = {}     # id(param) -> bf16 tensor that receives the updated values
         self.last_grad_norm: Optional[torch.Tensor] = None
 
@@ -139,11 +98,13 @@ class AdamW(Optimizer):
                 if not p.grad.is_contiguous():
                     p.grad = p.grad.contiguous()
                 _check_tensor(p.grad, "gradient")
+            p_ptrs = ops.ptrs(p.data for p, _ in items)     # CUDA tensors only: refused before any state changes
+            g_ptrs = ops.ptrs(p.grad for p, _ in items)
             dev = items[0][0].device
             key = (b1, b2, eps, tuple(p.numel() for p, _ in items), dev)
             tab = self._tables.get(key)
             if tab is None:
-                tab = self._tables[key] = _Table([p.numel() for p, _ in items], dev)
+                tab = self._tables[key] = ops.OptTable([p.numel() for p, _ in items], dev)
             rows = tab.begin()
             sizes, decays = [], []
             for p, group in items:
@@ -160,23 +121,16 @@ class AdamW(Optimizer):
                 sizes.append(step_size)
                 decays.append(group["lr"] * group["weight_decay"] if group["weight_decay"] > 0.0 else 0.0)
             # column-wise fills of the pinned table (one numpy assignment per field, not one tuple per parameter)
-            rows["p"] = [p.data_ptr() for p, _ in items]
-            rows["g"] = [p.grad.data_ptr() for p, _ in items]
+            rows["p"], rows["g"] = p_ptrs, g_ptrs
             rows["m"] = [self.state[p]["exp_avg"].data_ptr() for p, _ in items]
             rows["v"] = [self.state[p]["exp_avg_sq"].data_ptr() for p, _ in items]
-            rows["pb"] = [self.bf16_targets[id(p)].data_ptr() if id(p) in self.bf16_targets else 0 for p, _ in items]
-            rows["step_size"] = sizes
-            rows["decay"] = decays
+            rows["p_bf16"] = [self.bf16_targets[id(p)].data_ptr() if id(p) in self.bf16_targets else 0 for p, _ in items]
+            rows["step_size"], rows["decay"] = sizes, decays
             tab.upload()
-            norm_ptr = None
             if max_grad_norm is not None:
-                check(lib().xp_opt_grad_norm(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks,
-                                             tab.partial.data_ptr(), float(max_grad_norm), tab.norm.data_ptr(), _stream()),
-                      "xp_opt_grad_norm")
-                norm_ptr = tab.norm.data_ptr()
+                ops.opt_grad_norm(tab, max_grad_norm)
                 self.last_grad_norm = tab.norm[0]
-            check(lib().xp_opt_adamw_step(tab.dev.data_ptr(), tab.block_map.data_ptr(), tab.n_blocks, norm_ptr, b1, b2, eps,
-                                          _stream()), "xp_opt_adamw_step")
+            ops.opt_adamw_step(tab, b1, b2, eps, clip=max_grad_norm is not None)
             torch.autograd.graph.increment_version([p for p, _ in items])   # raw-pointer writes: tell autograd / the packs
         return loss
 

@@ -61,7 +61,7 @@ class _Exchange:
     def __init__(self, group, world: int, rank: int, b: int, d: int, dev: torch.device):
         import torch.distributed as dist
         self.world, self.rank, self.epoch = world, rank, 0
-        nbytes = int(_lib.lib().xp_nce_gather_exchange_bytes(b, d, world))
+        nbytes = ops.nce_gather_exchange_bytes(b, d, world)
         self.mode = 0
         try:
             import torch.distributed._symmetric_memory as symm
@@ -79,7 +79,7 @@ class _Exchange:
             self.gathered = torch.empty(world, 2, b, d, dtype=f32, device=dev)
             ptrs = [self.gathered[r, 0].data_ptr() for r in range(world)] + [self.gathered[r, 1].data_ptr() for r in range(world)]
         self.ptrs = torch.tensor(ptrs, dtype=torch.int64, device=dev)
-        self.ws = torch.zeros(int(_lib.lib().xp_nce_gather_workspace_bytes(world * b)) // 4, dtype=f32, device=dev)
+        self.ws = ops.nce_gather_workspace(world * b, dev)
 
     @classmethod
     def get(cls, group, world, rank, b, d, dev):
@@ -93,13 +93,6 @@ class _Exchange:
 _local_ws = {}
 
 
-def _aligned(x: torch.Tensor) -> torch.Tensor:
-    """x contiguous and 16-byte aligned: the fused kernel reads caller rows with 16-byte vector loads, and a contiguous
-    view may start anywhere in its allocation."""
-    x = x.contiguous()
-    return x if x.data_ptr() % 16 == 0 else x.clone()
-
-
 def _nce_forward_fused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor, exchange: "_Exchange" = None, group=None):
     """One launch of csrc/nce_fused.cu.  vis, txt: this rank's [b, d] fp32 rows.  Returns (loss[1], g_scaled[N, Np] bf16,
     vis_hi[N, d], txt_hi[N, d], dscale[1]) for the global batch N = world * b."""
@@ -108,37 +101,29 @@ def _nce_forward_fused(vis: torch.Tensor, txt: torch.Tensor, temp: torch.Tensor,
     world = exchange.world if exchange is not None else 1
     N = world * b
     Np = _pad8(N)
-    vis, txt = _aligned(vis), _aligned(txt)
+    vis, txt = ops.aligned_input(vis), ops.aligned_input(txt)      # the kernel reads rows with 16-byte vector loads
     g = (torch.zeros if Np != N else torch.empty)(N, Np, dtype=bf16, device=dev)
     vh = torch.empty(N, d, dtype=bf16, device=dev)
     th = torch.empty(N, d, dtype=bf16, device=dev)
     loss = torch.empty(1, dtype=f32, device=dev)
     dscale = torch.empty(1, dtype=f32, device=dev)
     scale = temp.detach().reshape(1).to(f32)
-    a = _lib.XpNceGather()
-    a.vis_local, a.txt_local = vis.data_ptr(), txt.data_ptr()
-    a.logit_scale, a.g_scaled, a.vis_hi, a.txt_hi = scale.data_ptr(), g.data_ptr(), vh.data_ptr(), th.data_ptr()
-    a.loss, a.d_logit_scale = loss.data_ptr(), dscale.data_ptr()
-    a.b, a.d, a.ld_g = b, d, Np
-    keep = None
     if exchange is None:                                  # single process: rows are read in place
         key = (N, dev)
         ws = _local_ws.get(key)
         if ws is None:
-            ws = _local_ws[key] = (torch.zeros(int(_lib.lib().xp_nce_gather_workspace_bytes(N)) // 4, dtype=f32, device=dev),
-                                   torch.empty(2, dtype=torch.int64, device=dev))
+            ws = _local_ws[key] = (ops.nce_gather_workspace(N, dev), torch.empty(2, dtype=torch.int64, device=dev))
         keep = torch.tensor([vis.data_ptr(), txt.data_ptr()], dtype=torch.int64).pin_memory()
         ws[1].copy_(keep, non_blocking=True)
-        a.rank, a.world, a.mode, a.epoch = 0, 1, 1, 0
-        a.peer_bufs, a.workspace = ws[1].data_ptr(), ws[0].data_ptr()
+        ops.nce_gather_fused(vis, txt, ws[1], scale, g, vh, th, loss, dscale, ws[0], rank=0, world=1, b=b, d=d, epoch=0,
+                             mode=1)
     else:
         if exchange.mode == 1:
             import torch.distributed as dist
             dist.all_gather_into_tensor(exchange.gathered, torch.stack([vis, txt]), group=group)
         exchange.epoch += 1
-        a.rank, a.world, a.mode, a.epoch = exchange.rank, world, exchange.mode, exchange.epoch
-        a.peer_bufs, a.workspace = exchange.ptrs.data_ptr(), exchange.ws.data_ptr()
-    ops.check(_lib.lib().xp_nce_gather_fused(ops.C.byref(a), ops._stream()), "xp_nce_gather_fused")
+        ops.nce_gather_fused(vis, txt, exchange.ptrs, scale, g, vh, th, loss, dscale, exchange.ws, rank=exchange.rank,
+                             world=world, b=b, d=d, epoch=exchange.epoch, mode=exchange.mode)
     return loss, g, vh, th, dscale
 
 

@@ -13,50 +13,40 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from .. import _lib
-from .._lib import check, lib
+from .. import ops
 
 
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _f32_cuda(t: torch.Tensor, what: str) -> torch.Tensor:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise _lib.XpError(f"xpretrain_b200.utils.metrics: {what} must be a CUDA tensor (there is no CPU path)")
-    return t.detach().to(torch.float32).contiguous()
+def _f32(t) -> torch.Tensor:
+    """t as contiguous fp32 (numpy input becomes a host tensor, which the kernels refuse: there is no CPU path)."""
+    return torch.as_tensor(t).detach().to(torch.float32).contiguous()
 
 
 def cal_cossim(feats1: torch.Tensor, feats2: torch.Tensor) -> torch.Tensor:
     """metrics.py:3-5: feats1 [N1, d] @ feats2 [N2, d].T -> [N1, N2] fp32 (fp32 FFMA accumulation on the device)."""
-    a, b = _f32_cuda(feats1, "feats1"), _f32_cuda(feats2, "feats2")
+    a, b = _f32(feats1), _f32(feats2)
     if a.shape[1] != b.shape[1]:
         raise ValueError("feature widths differ")
     out = torch.empty(a.shape[0], b.shape[0], dtype=torch.float32, device=a.device)
-    check(lib().xp_sim_f32(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.shape[0], b.shape[0], a.shape[1], out.stride(0),
-                           _stream()), "xp_sim_f32")
+    ops.sim_f32(a, b, out)
     return out
 
 
 def dsl(sim: torch.Tensor, theta: float = 100.0) -> torch.Tensor:
     """run_video_retrieval.py:169-170: sim * softmax(theta * sim, axis=0) (a new tensor; `sim` is left untouched)."""
-    out = _f32_cuda(sim, "sim").clone()
+    out = _f32(sim).clone()
     scratch = torch.empty(2 * out.shape[1], dtype=torch.float32, device=out.device)
-    check(lib().xp_dsl_reweight(out.data_ptr(), out.shape[0], out.shape[1], out.stride(0), float(theta), scratch.data_ptr(),
-                                _stream()), "xp_dsl_reweight")
+    ops.dsl_reweight(out, theta, scratch)
     return out
 
 
 def rank_counts(sim: torch.Tensor, transpose: bool = False):
     """(greater, equal) int32 device vectors: entries of row i (column i if transpose) larger than / equal to sim[i, i]."""
-    s = _f32_cuda(sim, "sim")
+    s = _f32(sim)
     if s.shape[0] != s.shape[1]:
         raise ValueError("compute_metrics needs a square similarity matrix (query i pairs with item i)")
     n = s.shape[0]
-    greater = torch.empty(n, dtype=torch.int32, device=s.device)
-    equal = torch.empty(n, dtype=torch.int32, device=s.device)
-    check(lib().xp_rank_counts(s.data_ptr(), n, s.stride(0), 1 if transpose else 0, greater.data_ptr(), equal.data_ptr(),
-                               _stream()), "xp_rank_counts")
+    greater, equal = (torch.empty(n, dtype=torch.int32, device=s.device) for _ in range(2))
+    ops.rank_counts(s, transpose, greater, equal)
     return greater, equal
 
 
