@@ -7,6 +7,9 @@
                (NaN, or the dtype's guard pattern for integer dtypes), every other element holds the guard pattern and
                must keep it
   same_bits    equality of the bit patterns (tells -0 from +0, compares NaN payloads)
+  reordering   two runs of the same model on the same inputs that may differ only in the order of fp32 atomic additions
+               (split-K weight gradients, column sums): outputs with the same bits, every gradient within GRAD_REL x
+               its scale (reordering_violations)
 """
 import contextlib
 
@@ -219,6 +222,50 @@ def calibrated_model_rows(tag, rows, slices=None):
           + (f", worst slice {worst_sl[0]:.3f} ({worst_sl[1]})" if slices else "")
           + (f"; worst err / autocast err {worst_ac[0]:.2f} ({worst_ac[1]})" if worst_ac[1] else ""))
     return bad, worst, worst_sl
+
+
+GRAD_REL = 1e-5         # max |g - g_ref| <= GRAD_REL x scale: split-K atomics reorder (about 1e-7 between runs)
+
+
+def grad_scale(grads, n):
+    """max |g| of gradient n.  k_proj.bias is measured against its layer's whole q/k/v bias gradient: its exact value is zero
+    (a key bias shifts every logit of a query row equally), so what the kernels compute is the rounding residue of a column
+    sum that cancels, accumulated with fp32 atomics, and its own maximum is that residue."""
+    if n.endswith("self_attn.k_proj.bias"):
+        return max(float(grads[n.replace("k_proj", p)].abs().max()) for p in ("q_proj", "k_proj", "v_proj"))
+    return float(grads[n].abs().max())
+
+
+def reordering_violations(ref_out, got_out, ref_grads, got_grads, rel=GRAD_REL):
+    """Two runs that may differ only in the order of fp32 atomic additions.  ref_out / got_out: {name: tensor}, which must
+    be finite and have the same bits; ref_grads / got_grads: {name: tensor or None}, the same names receiving a gradient
+    and max |got - ref| <= rel x grad_scale(ref_grads, name) for each.  Returns (violations, (worst |got - ref| / scale,
+    its name)); the worst ratio is over the gradients."""
+    bad = []
+    for n, r in ref_out.items():
+        g = got_out[n]
+        if not bool(torch.isfinite(g.float()).all()):
+            bad.append(f"{n}: not finite")
+        elif not same_bits(r, g):
+            d = float((g.double() - r.double()).abs().max())
+            bad.append(f"{n}: bits differ (max |difference| {d:.3e})")
+    if set(ref_grads) != set(got_grads):
+        bad.append(f"gradients on one side only: {sorted(set(ref_grads) ^ set(got_grads))}")
+    worst = (0.0, None)
+    for n in sorted(set(ref_grads) & set(got_grads)):
+        r, g = ref_grads[n], got_grads[n]
+        if (r is None) != (g is None):
+            bad.append(f"{n}: gradient {'missing' if g is None else 'unexpected'}")
+            continue
+        if r is None:
+            continue
+        scale = grad_scale(ref_grads, n)
+        diff = float((g.double() - r.double()).abs().max())
+        if not diff <= rel * scale:          # NaN fails
+            bad.append(f"{n}: max |difference| {diff:.3e} > {rel:.0e} x scale {scale:.3e}")
+        if scale > 0 and diff / scale > worst[0]:
+            worst = (diff / scale, n)
+    return bad, worst
 
 
 @contextlib.contextmanager

@@ -152,6 +152,66 @@ def test_declarations_match_the_header(tmp_path):
     assert not bad, "the Python declarations disagree with include/xpretrain_b200.h:\n  " + "\n  ".join(bad)
 
 
+def _stream_functions():
+    """The header's functions whose last parameter is `void* stream`: the kernel launches."""
+    src = open(os.path.join(ROOT, "include", "xpretrain_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", " ", src, flags=re.S)
+    src = "\n".join(line for line in src.splitlines() if not line.lstrip().startswith("#"))
+    out = set()
+    for chunk in src.split(";"):
+        m = re.search(r"\b(xp_\w+)\s*\(([^)]*)\)\s*$", chunk)
+        if m and re.sub(r"\s+", " ", m.group(2).split(",")[-1]).strip() == "void* stream":
+            out.add(m.group(1))
+    return out
+
+
+def test_every_launch_goes_through_ops_call():
+    """ops._call is the one place a kernel is launched: it appends the current stream, and wrapping it sees every launch
+    (test_gpu_stream_schedule.py delays chosen streams that way).  In the package's code (its syntax tree: docstrings,
+    comments and error-message labels may name a function), every header function taking `void* stream` is reached only
+    as the quoted first argument of `_call(...)` in ops.py, never as an attribute or through getattr; a launch function
+    declared but never called is allowed.  No module other than ops.py and _lib.py calls or imports `lib`."""
+    import ast
+    launches = _stream_functions()
+    assert len(launches) >= 40, f"the header parse found only {len(launches)} launch functions"
+    pkg = os.path.join(ROOT, "xpretrain_b200")
+    own = {os.path.join("xpretrain_b200", "ops.py"), os.path.join("xpretrain_b200", "_lib.py")}
+    bad, used = [], set()
+    for dirpath, _, files in os.walk(pkg):
+        for f in sorted(files):
+            if not f.endswith(".py"):
+                continue
+            path = os.path.join(dirpath, f)
+            rel = os.path.relpath(path, ROOT)
+            for node in ast.walk(ast.parse(open(path).read(), path)):
+                where = f"{rel}:{getattr(node, 'lineno', 0)}"
+                if isinstance(node, ast.Attribute) and node.attr in launches:
+                    bad.append(f"{where}: .{node.attr} launched outside ops._call")
+                if not isinstance(node, ast.Call):
+                    if isinstance(node, ast.ImportFrom) and rel not in own and any(a.name == "lib" for a in node.names):
+                        bad.append(f"{where}: imports lib")
+                    continue
+                fn = node.func.id if isinstance(node.func, ast.Name) else getattr(node.func, "attr", None)
+                first = node.args[0] if node.args else None
+                name = first.value if isinstance(first, ast.Constant) and isinstance(first.value, str) else None
+                if fn == "_call" and rel == os.path.join("xpretrain_b200", "ops.py") and name in launches:
+                    used.add(name)
+                elif fn == "_call":
+                    bad.append(f"{where}: _call outside ops.py or with no launch function name")
+                if fn == "getattr" and len(node.args) > 1 and getattr(node.args[1], "value", None) in launches:
+                    bad.append(f"{where}: getattr reaches {node.args[1].value}")
+                if fn == "lib" and rel not in own:
+                    bad.append(f"{where}: calls lib()")
+    assert not bad, "launches that bypass ops._call:\n  " + "\n  ".join(bad)
+    assert len(used) >= 40, f"only {len(used)} launch functions are called through ops._call"
+    # the stream _call appends is the current one, as the last argument
+    ops_src = open(os.path.join(pkg, "ops.py")).read()
+    assert re.search(r"def _call\(name: str, \*args\) -> None:.*?getattr\(lib\(\), name\)\(\*args, "
+                     r"torch\.cuda\.current_stream\(\)\.cuda_stream\)", ops_src, flags=re.S)
+    assert len(re.findall(r"getattr\(lib\(\)", ops_src)) == 1
+    print(f"\n{len(used)} of {len(launches)} launch functions called through ops._call; unused: {sorted(launches - used)}")
+
+
 def test_no_cpu_fallback():
     """The product path must fail loudly off-GPU instead of computing on the host."""
     from types import SimpleNamespace

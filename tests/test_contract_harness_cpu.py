@@ -1,10 +1,12 @@
 """The shared rule and output checks of contract_harness.py at their boundaries, on the CPU: the calibrated slice rule at
 exactly FACTOR x the arm, the absolute floor, empty slices, the element check on NaN and zero bounds, write coverage and
-guard elements for every guarded dtype, and bitwise comparison of signed zeros."""
+guard elements for every guarded dtype, bitwise comparison of signed zeros, and the reordering rule of two runs that differ
+only in the order of fp32 atomic additions."""
 import pytest
 import torch
 
-from contract_harness import ABS_FLOOR, DTYPES, FACTOR, FLOOR, Guarded, Out, Report, calibrated, same_bits, within
+from contract_harness import (ABS_FLOOR, DTYPES, FACTOR, FLOOR, GRAD_REL, Guarded, Out, Report, calibrated,
+                              reordering_violations, same_bits, within)
 
 F64 = torch.float64
 
@@ -110,3 +112,56 @@ def test_same_bits_tells_signed_zeros_apart(dtype):
     neg[1] = -0.0
     assert bool((pos == neg).all()) and not same_bits(pos, neg)
     assert same_bits(neg, neg.clone())
+
+
+def _layer_grads(seed=0):
+    g = torch.Generator().manual_seed(seed)
+    pre = "clipmodel.vision_model.encoder.layers.0.self_attn."
+    grads = {pre + f"{n}.bias": torch.randn(8, generator=g) for n in ("q_proj", "k_proj", "v_proj")}
+    grads[pre + "k_proj.bias"] *= 1e-4                # the cancelling key bias: a rounding residue
+    grads[pre + "out_proj.weight"] = torch.randn(8, 8, generator=g)
+    grads["clipmodel.text_model.embeddings.token_embedding.weight"] = None
+    return pre, grads
+
+
+def test_reordering_rule_flags_1e4_passes_1e7_and_scales_k_bias_by_qkv():
+    pre, ref = _layer_grads()
+    out = {"loss": torch.tensor(1.25), "vis": torch.randn(4, 8, generator=torch.Generator().manual_seed(1))}
+    w = pre + "out_proj.weight"
+    scale = float(ref[w].abs().max())
+    for rel, flagged in ((1e-4, True), (1e-7, False)):
+        got = dict(ref)
+        got[w] = ref[w].clone()
+        got[w][3, 5] += rel * scale
+        bad, worst = reordering_violations(out, {k: v.clone() for k, v in out.items()}, ref, got)
+        assert bool(bad) == flagged and (not bad or w in bad[0]), bad
+        assert worst[1] == w and worst[0] == pytest.approx(rel, rel=0.1)     # fp32 rounding of the planted add
+    # k_proj.bias: a difference of 1e-6 x the q/k/v maximum passes although it is ~1e-2 of its own maximum, and 1e-4 of
+    # the q/k/v maximum fails
+    k = pre + "k_proj.bias"
+    qkv = max(float(ref[pre + f"{n}.bias"].abs().max()) for n in ("q_proj", "k_proj", "v_proj"))
+    assert float(ref[k].abs().max()) < 1e-3 * qkv
+    for rel, flagged in ((1e-6, False), (1e-4, True)):
+        got = dict(ref)
+        got[k] = ref[k] + rel * qkv
+        bad, worst = reordering_violations(out, out, ref, got)
+        assert bool(bad) == flagged, bad
+        assert worst[1] == k and worst[0] == pytest.approx(rel, rel=1e-3)
+    assert GRAD_REL == 1e-5
+
+
+def test_reordering_rule_wants_the_same_output_bits_and_the_same_gradients():
+    _, ref = _layer_grads()
+    out = {"loss": torch.tensor(0.0), "vis": torch.ones(2, 3)}
+    neg = {"loss": torch.tensor(-0.0), "vis": torch.ones(2, 3)}
+    bad, _ = reordering_violations(out, neg, ref, ref)
+    assert len(bad) == 1 and bad[0].startswith("loss: bits differ"), bad
+    nan = {"loss": torch.tensor(0.0), "vis": torch.full((2, 3), float("nan"))}
+    assert reordering_violations(nan, nan, ref, ref)[0] == ["vis: not finite"]
+    name = "clipmodel.text_model.embeddings.token_embedding.weight"
+    assert any(name in b for b in reordering_violations(out, out, ref, dict(ref, **{name: torch.zeros(2)}))[0])
+    nang = {k: (None if v is None else v.clone()) for k, v in ref.items()}
+    w = next(k for k in ref if k.endswith("out_proj.weight"))
+    nang[w][0, 0] = float("nan")
+    assert any(w in b for b in reordering_violations(out, out, ref, nang)[0])
+    assert reordering_violations(out, out, ref, {k: v for k, v in ref.items() if k != w})[0]

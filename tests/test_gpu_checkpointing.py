@@ -2,7 +2,8 @@
 
 A checkpointed tower keeps only each block's input and rebuilds the block's saved tensors in the backward by rerunning the
 same kernels.  The recompute must reproduce the forward bit for bit, so loss and features must be equal with the switch on and
-off, and gradients may differ only by the reordering of the split-K fp32 atomics of the weight-gradient GEMMs.
+off, and gradients may differ only by the reordering of the split-K fp32 atomics of the weight-gradient GEMMs
+(contract_harness.reordering_violations).
 """
 import gc
 import os
@@ -11,9 +12,9 @@ from types import SimpleNamespace
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from contract_harness import GRAD_REL, reordering_violations
 
-GRAD_REL = 1e-5          # max |g_on - g_off| <= GRAD_REL * max |g_off|: split-K atomics reorder (about 1e-7 between runs)
+pytestmark = pytest.mark.gpu
 
 # the bars of test_gpu_parity.py's small-golden case (set there from the reference's own bf16 deviation)
 EMB_REL_L2 = 1.2e-2
@@ -68,31 +69,11 @@ def _step(model, video, ids, mask):
     return loss.detach(), out["vis_features"].detach(), out["text_features"].detach(), grads
 
 
-def _grad_scale(grads, n):
-    """max |g| of gradient n.  k_proj.bias is measured against its layer's whole q/k/v bias gradient: its exact value is zero
-    (a key bias shifts every logit of a query row equally), so what the kernels compute is the rounding residue of a column
-    sum that cancels, accumulated with fp32 atomics, and its own maximum is that residue."""
-    if n.endswith("self_attn.k_proj.bias"):
-        return max(float(grads[n.replace("k_proj", p)].abs().max()) for p in ("q_proj", "k_proj", "v_proj"))
-    return float(grads[n].abs().max())
-
-
 def _assert_same(off, on):
-    assert torch.equal(off[0], on[0]), (float(off[0]), float(on[0]))
-    assert torch.equal(off[1], on[1])
-    assert torch.equal(off[2], on[2])
-    worst = (0.0, None)
-    for n, g_off in off[3].items():
-        g_on = on[3][n]
-        if g_off is None:
-            assert g_on is None, n
-            continue
-        scale = _grad_scale(off[3], n)
-        diff = float((g_on - g_off).abs().max())
-        assert diff <= GRAD_REL * scale, (n, diff, scale)
-        if scale > 0 and diff / scale > worst[0]:
-            worst = (diff / scale, n)
+    bad, worst = reordering_violations({"loss": off[0], "vis": off[1], "txt": off[2]},
+                                       {"loss": on[0], "vis": on[1], "txt": on[2]}, off[3], on[3])
     print(f"  worst gradient difference {worst[0]:.2e} (relative to max |g|) at {worst[1]}")
+    assert not bad, "\n".join(bad)
 
 
 def _off_on(model, video, ids, mask):
