@@ -93,7 +93,7 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64
                       uint32_t box_inner, uint32_t box_outer) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return fail("cuTensorMapEncodeTiled unavailable (no CUDA driver / no GPU): this library has no CPU path");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("tensor map: base pointer must be 16-byte aligned");
+  if (!aligned(base, 16)) return fail("tensor map: base pointer must be 16-byte aligned");
   if ((row_stride * 2) % 16 != 0) return fail("tensor map: row stride must be a multiple of 8 bf16 elements");
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {row_stride * 2};
@@ -110,7 +110,7 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t inner, uint64
                       uint64_t row_stride, uint64_t mid_stride, uint32_t box_inner, uint32_t box_mid) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return fail("cuTensorMapEncodeTiled unavailable (no CUDA driver / no GPU): this library has no CPU path");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("tensor map: base pointer must be 16-byte aligned");
+  if (!aligned(base, 16)) return fail("tensor map: base pointer must be 16-byte aligned");
   if ((row_stride * 2) % 16 != 0 || (mid_stride * 2) % 16 != 0)
     return fail("tensor map: strides must be multiples of 8 bf16 elements");
   cuuint64_t dims[3] = {inner, mid, outer};

@@ -1,11 +1,16 @@
 // Host-side helpers shared by the C-ABI translation units.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <atomic>
 #include <string>
+#include <type_traits>
+
+#include "../../include/xpretrain_b200.h"
 
 namespace xp {
 
@@ -47,5 +52,34 @@ int ensure_context(const void* device_ptr);
     if (_e != cudaSuccess) return ::xp::fail(std::string(name) + " launch: " + cudaGetErrorString(_e)); \
     ::xp::count_launch();                                                                                 \
   } while (0)
+
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// Raises kernel K's dynamic shared-memory limit to `bytes` on the first call (once per process); 0 or -1 as fail().
+template <auto K>
+int smem_limit(int bytes) {
+  static bool done = false;
+  if (!done) {
+    XP_CHECK_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done = true;
+  }
+  return 0;
+}
+
+// Runtime value -> template argument: f(std::integral_constant<int, V>{}) for the V in Vs equal to v, else fail(what).
+template <int... Vs, class F>
+int dispatch(int v, const char* what, F&& f) {
+  int rc = 0;
+  const bool found = ((v == Vs && (rc = f(std::integral_constant<int, Vs>{}), true)) || ...);
+  return found ? rc : fail(what);
+}
+
+// Element type of an XP_DTYPE_* code, and f(T{}) for the element type T of `dtype` (fail(what) for another code).
+template <int D>
+using dtype_t = std::conditional_t<D == XP_DTYPE_F32, float, std::conditional_t<D == XP_DTYPE_BF16, __nv_bfloat16, __half>>;
+template <class F>
+int dispatch_dtype(int dtype, const char* what, F&& f) {
+  return dispatch<XP_DTYPE_F32, XP_DTYPE_BF16, XP_DTYPE_F16>(dtype, what, [&](auto d) { return f(dtype_t<d.value>{}); });
+}
 
 }  // namespace xp

@@ -180,12 +180,7 @@ extern "C" int xp_dense_attention_fwd(const void* qkv, void* out, float* lse, co
   if (int rc = to_dims(desc, d, "xp_dense_attention_fwd")) return rc;
   CUtensorMap tm;
   if (seq_tmap(&tm, qkv, d.ld_qkv, d)) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(
-        cudaFuncSetAttribute(stream_fwd_kernel<DenseFwd>, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_FWD_SMEM));
-    attr = true;
-  }
+  if (smem_limit<stream_fwd_kernel<DenseFwd>>(DENSE_FWD_SMEM)) return -1;
   const DenseFwd p{{d}, static_cast<__nv_bfloat16*>(out), lse};
   stream_fwd_kernel<<<dense_grid(d), STREAM_THREADS, DENSE_FWD_SMEM, static_cast<cudaStream_t>(stream)>>>(tm, p);
   XP_CHECK_LAUNCH("dense_fwd_kernel");
@@ -197,17 +192,12 @@ extern "C" int xp_dense_attention_bwd(const void* qkv, const void* out, const vo
   XP_ENTER(qkv);
   DenseDims d;
   if (int rc = to_dims(desc, d, "xp_dense_attention_bwd")) return rc;
-  if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) return fail("xp_dense_attention_bwd: out must be 16-byte aligned");
+  if (!aligned(out, 16)) return fail("xp_dense_attention_bwd: out must be 16-byte aligned");
   CUtensorMap tm, tdo;
   if (seq_tmap(&tm, qkv, d.ld_qkv, d) || seq_tmap(&tdo, dout, d.ld_o, d)) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_kv_kernel<DenseBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       DENSE_BWD_KV_SMEM));
-    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_q_kernel<DenseBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       DENSE_BWD_Q_SMEM));
-    attr = true;
-  }
+  if (smem_limit<stream_bwd_kv_kernel<DenseBwd>>(DENSE_BWD_KV_SMEM) ||
+      smem_limit<stream_bwd_q_kernel<DenseBwd>>(DENSE_BWD_Q_SMEM))
+    return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long items = static_cast<long long>(d.n_seq) * d.L * d.H * 8;
   const unsigned blocks = static_cast<unsigned>(std::min<long long>((items + 255) / 256, 65535LL * 16));

@@ -9,16 +9,6 @@
 
 namespace xp {
 
-__device__ __forceinline__ uint4 pack8f(const float (&f)[8]) {
-  uint4 u;
-  u.x = pack_bf16(f[0], f[1]); u.y = pack_bf16(f[2], f[3]); u.z = pack_bf16(f[4], f[5]); u.w = pack_bf16(f[6], f[7]);
-  return u;
-}
-__device__ __forceinline__ void unpack8f(const uint4& u, float (&f)[8]) {
-  f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
-  f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
-}
-
 // F.interpolate(mode="linear", align_corners=False) source taps for output index i (CLIP_ViP.py:172-174).
 __device__ __forceinline__ void linear_taps(int i, int n_in, int n_out, int& i0, int& i1, float& w1) {
   if (n_in == n_out) {
@@ -38,29 +28,6 @@ __device__ __forceinline__ void linear_taps(int i, int n_in, int n_out, int& i0,
 // video [F, 3, H, W] (F = B*T frames) -> patches [F * (H/p) * (W/p), 3*p*p] bf16, column = c*p*p + kh*p + kw
 // (the flattening order of Conv2d.weight [out, c, kh, kw]); patch order row-major over the grid (flatten(2), :179).
 template <typename T>
-__device__ __forceinline__ void load8(const T* p, float (&f)[8]);
-template <>
-__device__ __forceinline__ void load8<float>(const float* p, float (&f)[8]) {
-  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <>
-__device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* p, float (&f)[8]) {
-  unpack8f(*reinterpret_cast<const uint4*>(p), f);
-}
-template <>
-__device__ __forceinline__ void load8<__half>(const __half* p, float (&f)[8]) {
-  const uint4 u = *reinterpret_cast<const uint4*>(p);
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 v = __half22float2(h[i]);
-    f[2 * i] = v.x;
-    f[2 * i + 1] = v.y;
-  }
-}
-
-template <typename T>
 __global__ void __launch_bounds__(256)
 patchify_kernel(const T* __restrict__ video, __nv_bfloat16* __restrict__ out, long long frames, int H, int W, int p) {
   // one thread per 8 consecutive pixels of an image row; p % 8 == 0
@@ -75,11 +42,11 @@ patchify_kernel(const T* __restrict__ video, __nv_bfloat16* __restrict__ out, lo
   const int c = static_cast<int>(rest % 3);
   const long long f = rest / 3;
   float v[8];
-  load8<T>(video + ((f * 3 + c) * H + y) * W + wc * 8, v);
+  load8(video + ((f * 3 + c) * H + y) * W + wc * 8, v);
   const int gw = W / p, gh = H / p;
   const int pw = (wc * 8) / p, kw = (wc * 8) % p, ph = y / p, kh = y % p;
   const long long row = (f * gh + ph) * gw + pw;
-  *reinterpret_cast<uint4*>(out + row * (3 * p * p) + c * p * p + kh * p + kw) = pack8f(v);
+  store8(out + row * (3 * p * p) + c * p * p + kh * p + kw, v);
 }
 
 // uint8 frames as the decoder delivers them, [frames, H, W, 3] (HWC), to the same bf16 patch matrix, with the reference's
@@ -116,20 +83,13 @@ patchify_u8_kernel(const uint8_t* __restrict__ frames, __nv_bfloat16* __restrict
       const float x = static_cast<float>((w[byte >> 2] >> ((byte & 3) * 8)) & 0xffu);
       v[px] = __fdiv_rn(__fsub_rn(__fdiv_rn(x, 255.f), mean[ch]), sd[ch]);
     }
-    *reinterpret_cast<uint4*>(out + row * (3 * p * p) + ch * p * p + kh * p + kw) = pack8f(v);
+    store8(out + row * (3 * p * p) + ch * p * p + kh * p + kw, v);
   }
 }
 
 // Any patch size dividing H and W (ViT-L/14: p = 14).  The patch matrix row pitch is ld = round_up(3 p^2, 8) (16-byte rows
 // for TMA and the GEMM); columns [3 p^2, ld) are written as zero.  One thread per 8 consecutive columns of a patch row: a
 // gather of 8 input values (the same conversion and rounding as the vectorised kernels above) and one 16-byte store.
-template <typename T>
-__device__ __forceinline__ float to_f32(T v) { return static_cast<float>(v); }
-template <>
-__device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <>
-__device__ __forceinline__ float to_f32<__half>(__half v) { return __half2float(v); }
-
 template <typename T, bool U8>
 __global__ void __launch_bounds__(256)
 patchify_any_kernel(const T* __restrict__ src, __nv_bfloat16* __restrict__ out, long long frames, int H, int W, int p,
@@ -160,7 +120,7 @@ patchify_any_kernel(const T* __restrict__ src, __nv_bfloat16* __restrict__ out, 
       }
     }
   }
-  *reinterpret_cast<uint4*>(out + row * ld + cc * 8) = pack8f(v);
+  store8(out + row * ld + cc * 8, v);
 }
 
 // ------------------------------------------------------------ embedding tables
@@ -210,7 +170,7 @@ vip_embed_bwd_kernel(const __nv_bfloat16* __restrict__ d_patch, const __nv_bfloa
 #pragma unroll 4
   for (int b = 0; b < B; ++b) {
     float v[8];
-    unpack8f(*reinterpret_cast<const uint4*>(src + b * bstride + c0), v);
+    load8(src + b * bstride + c0, v);
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[i] += v[i];
   }
@@ -310,55 +270,43 @@ eos_offsets_kernel(const long long* __restrict__ ids, long long* __restrict__ of
 
 using namespace xp;
 
-static bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
-
 extern "C" int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_t frames, int32_t H,
                                int32_t W, int32_t patch, void* stream) {
   XP_ENTER(video);
   if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify: patch must divide H and W");
   // every path stores the patch matrix in 16-byte vectors; the p % 8 == 0 path also loads the video in 16-byte vectors
-  if (!aligned_to(patches_bf16, 16)) return fail("xp_vip_patchify: patches must be 16-byte aligned");
-  if (patch % 8 == 0 && !aligned_to(video, 16)) return fail("xp_vip_patchify: video must be 16-byte aligned");
+  if (!aligned(patches_bf16, 16)) return fail("xp_vip_patchify: patches must be 16-byte aligned");
+  if (patch % 8 == 0 && !aligned(video, 16)) return fail("xp_vip_patchify: video must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   __nv_bfloat16* out = static_cast<__nv_bfloat16*>(patches_bf16);
   if (patch % 8) {
     const long long total = frames * (H / patch) * (W / patch) * (((3 * patch * patch + 7) & ~7) / 8);
     if (total <= 0) return 0;
     const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-    if (dtype == XP_DTYPE_F32)
-      patchify_any_kernel<float, false><<<grid, 256, 0, st>>>(static_cast<const float*>(video), out, frames, H, W, patch,
-                                                              0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
-    else if (dtype == XP_DTYPE_BF16)
-      patchify_any_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(video), out, frames,
-                                                                      H, W, patch, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
-    else if (dtype == XP_DTYPE_F16)
-      patchify_any_kernel<__half, false><<<grid, 256, 0, st>>>(static_cast<const __half*>(video), out, frames, H, W, patch,
-                                                               0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
-    else
-      return fail("xp_vip_patchify: dtype must be XP_DTYPE_F32 / BF16 / F16");
-    XP_CHECK_LAUNCH("patchify_any_kernel");
-    return 0;
+    return dispatch_dtype(dtype, "xp_vip_patchify: dtype must be XP_DTYPE_F32 / BF16 / F16", [&](auto t) {
+      using T = decltype(t);
+      patchify_any_kernel<T, false><<<grid, 256, 0, st>>>(static_cast<const T*>(video), out, frames, H, W, patch, 0.f, 0.f,
+                                                          0.f, 1.f, 1.f, 1.f);
+      XP_CHECK_LAUNCH("patchify_any_kernel");
+      return 0;
+    });
   }
   const long long total = frames * 3 * H * (W / 8);
   if (total <= 0) return 0;
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  if (dtype == XP_DTYPE_F32)
-    patchify_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(video), out, frames, H, W, patch);
-  else if (dtype == XP_DTYPE_BF16)
-    patchify_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(video), out, frames, H, W, patch);
-  else if (dtype == XP_DTYPE_F16)
-    patchify_kernel<__half><<<grid, 256, 0, st>>>(static_cast<const __half*>(video), out, frames, H, W, patch);
-  else
-    return fail("xp_vip_patchify: dtype must be XP_DTYPE_F32 / BF16 / F16");
-  XP_CHECK_LAUNCH("patchify_kernel");
-  return 0;
+  return dispatch_dtype(dtype, "xp_vip_patchify: dtype must be XP_DTYPE_F32 / BF16 / F16", [&](auto t) {
+    using T = decltype(t);
+    patchify_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T*>(video), out, frames, H, W, patch);
+    XP_CHECK_LAUNCH("patchify_kernel");
+    return 0;
+  });
 }
 
 extern "C" int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W,
                                   int32_t patch, const float* mean3, const float* std3, void* stream) {
   XP_ENTER(frames_hwc);
   if (patch < 1 || W % patch || H % patch) return fail("xp_vip_patchify_u8: patch must divide H and W");
-  if (!aligned_to(patches_bf16, 16)) return fail("xp_vip_patchify_u8: patches must be 16-byte aligned");
+  if (!aligned(patches_bf16, 16)) return fail("xp_vip_patchify_u8: patches must be 16-byte aligned");
   if (patch % 8) {
     const long long total = frames * (H / patch) * (W / patch) * (((3 * patch * patch + 7) & ~7) / 8);
     if (total <= 0) return 0;
@@ -368,7 +316,7 @@ extern "C" int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16,
     XP_CHECK_LAUNCH("patchify_any_kernel");
     return 0;
   }
-  if ((reinterpret_cast<uintptr_t>(frames_hwc) & 7) != 0) return fail("xp_vip_patchify_u8: frames must be 8-byte aligned");
+  if (!aligned(frames_hwc, 8)) return fail("xp_vip_patchify_u8: frames must be 8-byte aligned");
   const long long total = frames * H * (W / 8);
   if (total <= 0) return 0;
   patchify_u8_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -397,7 +345,7 @@ extern "C" int xp_vip_embed_bwd(const void* d_patch_bf16, const void* d_global_b
   XP_ENTER(d_patch_bf16);
   if (C % 8 || C > 1024) return fail("xp_vip_embed_bwd: C must be a multiple of 8 and <= 1024");
   if (d_pos == nullptr) return fail("xp_vip_embed_bwd: d_pos is required");
-  if (!aligned_to(d_patch_bf16, 16) || !aligned_to(d_global_bf16, 16))
+  if (!aligned(d_patch_bf16, 16) || !aligned(d_global_bf16, 16))
     return fail("xp_vip_embed_bwd: d_patch and d_global must be 16-byte aligned");
   const long long S = static_cast<long long>(M) + static_cast<long long>(T) * L;
   vip_embed_bwd_kernel<<<static_cast<unsigned>(S), 128, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -411,8 +359,8 @@ extern "C" int xp_text_embed_fwd(const int64_t* ids, const float* tok, const flo
                                  int32_t Lt, int32_t C, int32_t vocab, int32_t* err_flag, void* stream) {
   XP_ENTER(ids);
   if (C % 4) return fail("xp_text_embed_fwd: C must be a multiple of 4");
-  if (!aligned_to(tok, 16) || !aligned_to(pos, 16)) return fail("xp_text_embed_fwd: tok and pos must be 16-byte aligned");
-  if (!aligned_to(x_bf16, 8)) return fail("xp_text_embed_fwd: x must be 8-byte aligned");
+  if (!aligned(tok, 16) || !aligned(pos, 16)) return fail("xp_text_embed_fwd: tok and pos must be 16-byte aligned");
+  if (!aligned(x_bf16, 8)) return fail("xp_text_embed_fwd: x must be 8-byte aligned");
   if (rows <= 0) return 0;
   text_embed_fwd_kernel<<<rows, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(ids), tok, pos, static_cast<__nv_bfloat16*>(x_bf16), Lt, C, vocab, err_flag);

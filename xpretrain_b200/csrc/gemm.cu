@@ -365,55 +365,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
-template <int BN, int A_MN, int B_MN, int OUT, int ACT>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, OUT, ACT>;
-  static bool attr_set = false;  // per instantiation
-  if (!attr_set) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_set = true;
-  }
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, dev);
-  XP_CHECK_LAUNCH("gemm_kernel");
-  return 0;
-}
-
-template <int BN, int OUT, int ACT>
-static int dispatch_layout(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev,
-                           int grid, cudaStream_t stream) {
-  if (g->a_layout == 0 && g->b_layout == 0) return launch_gemm<BN, 0, 0, OUT, ACT>(tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 0 && g->b_layout == 1) return launch_gemm<BN, 0, 1, OUT, ACT>(tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 1 && g->b_layout == 1) return launch_gemm<BN, 1, 1, OUT, ACT>(tmA, tmB, dev, grid, stream);
-  if (g->a_layout == 1 && g->b_layout == 0) return launch_gemm<BN, 1, 0, OUT, ACT>(tmA, tmB, dev, grid, stream);
-  return fail("xp_gemm: a_layout/b_layout must be 0 or 1");
-}
-
-// The activation epilogues exist for bf16 outputs only (forward activations / their gradients).
-template <int BN>
-static int dispatch_act_bf16(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int grid,
-                             cudaStream_t stream) {
-  switch (g->act) {
-    case XP_ACT_NONE: return dispatch_layout<BN, XP_OUT_BF16, XP_ACT_NONE>(g, tmA, tmB, dev, grid, stream);
-    case XP_ACT_QUICK_GELU: return dispatch_layout<BN, XP_OUT_BF16, XP_ACT_QUICK_GELU>(g, tmA, tmB, dev, grid, stream);
-    case XP_ACT_DQUICK_GELU: return dispatch_layout<BN, XP_OUT_BF16, XP_ACT_DQUICK_GELU>(g, tmA, tmB, dev, grid, stream);
-    case XP_ACT_GELU_ERF: return dispatch_layout<BN, XP_OUT_BF16, XP_ACT_GELU_ERF>(g, tmA, tmB, dev, grid, stream);
-    case XP_ACT_DGELU_ERF: return dispatch_layout<BN, XP_OUT_BF16, XP_ACT_DGELU_ERF>(g, tmA, tmB, dev, grid, stream);
-  }
-  return fail("xp_gemm: bad act");
-}
-
-template <int BN>
-static int dispatch_out(const XpGemm* g, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& dev, int grid,
-                        cudaStream_t stream) {
-  switch (g->out) {
-    case XP_OUT_BF16: return dispatch_act_bf16<BN>(g, tmA, tmB, dev, grid, stream);
-    case XP_OUT_F32: return dispatch_layout<BN, XP_OUT_F32, XP_ACT_NONE>(g, tmA, tmB, dev, grid, stream);
-    case XP_OUT_F32_ATOMIC: return dispatch_layout<BN, XP_OUT_F32_ATOMIC, XP_ACT_NONE>(g, tmA, tmB, dev, grid, stream);
-  }
-  return fail("xp_gemm: bad out mode");
-}
-
 static int g_dbg_mn_lbo = 0, g_dbg_mn_sbo = 0;
 }  // namespace xp
 
@@ -443,12 +394,12 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
   if (g->aux && g->c_group > 0) return fail("xp_gemm: aux cannot be combined with grouped rows (c_group > 0)");
   if (g->scale_cols < 0 || g->scale_cols % 2) return fail("xp_gemm: scale_cols must be even and non-negative");
   const int elem_c = g->out == XP_OUT_BF16 ? 2 : 4;
-  if ((reinterpret_cast<uintptr_t>(g->c) & 15) || (g->ldc * elem_c) % 16)
+  if (!aligned(g->c, 16) || (g->ldc * elem_c) % 16)
     return fail("xp_gemm: C must be 16-byte aligned with a 16-byte multiple row pitch");
-  if (g->bias && (reinterpret_cast<uintptr_t>(g->bias) & 15)) return fail("xp_gemm: bias must be 16-byte aligned");
-  if (g->residual && ((reinterpret_cast<uintptr_t>(g->residual) & 15) || (g->ldr % 8)))
+  if (g->bias && !aligned(g->bias, 16)) return fail("xp_gemm: bias must be 16-byte aligned");
+  if (g->residual && (!aligned(g->residual, 16) || (g->ldr % 8)))
     return fail("xp_gemm: residual must be 16-byte aligned, ldr % 8 == 0");
-  if (g->aux && ((reinterpret_cast<uintptr_t>(g->aux) & 15) || (g->ld_aux % 8)))
+  if (g->aux && (!aligned(g->aux, 16) || (g->ld_aux % 8)))
     return fail("xp_gemm: aux must be 16-byte aligned, ld_aux % 8 == 0");
   if ((g->c_group > 0 && g->c_group_stride % 8) || (g->r_group > 0 && g->r_group_stride % 8))
     return fail("xp_gemm: c_group_stride / r_group_stride must be multiples of 8 elements");
@@ -466,7 +417,8 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
     const bool short_k_fwd = g->b_layout == 0 && kb_split <= 16;
     bn = (g->N >= 256 && tiles256 >= nsm && !short_k_fwd) ? 256 : 128;
   }
-  if (bn != 128 && bn != 256) return fail("xp_gemm: block_n must be 0, 128 or 256");
+  const char* bad_bn = "xp_gemm: block_n must be 0, 128 or 256";
+  if (bn != 128 && bn != 256) return fail(bad_bn);
   // sm_90 has no CTA pairs: cta_pair 0 (auto) and 1 (never) both run the single-CTA kernel
   if (g->cta_pair < 0 || g->cta_pair > 1) return fail("xp_gemm: cta_pair must be 0 or 1 (no CTA pairs on sm_90)");
   const long long total = static_cast<long long>(num_m) * ((g->N + bn - 1) / bn) * splits;
@@ -510,6 +462,28 @@ extern "C" int xp_gemm(const XpGemm* g, void* stream_v) {
   dev.mn_lbo = g_dbg_mn_lbo ? g_dbg_mn_lbo : BK * 128;
   dev.mn_sbo = g_dbg_mn_sbo ? g_dbg_mn_sbo : 1024;
 
-  return bn == 256 ? dispatch_out<256>(g, tmA, tmB, dev, grid, stream)
-                   : dispatch_out<128>(g, tmA, tmB, dev, grid, stream);
+  const char* bad_layout = "xp_gemm: a_layout/b_layout must be 0 or 1";
+  auto launch = [&](auto tile_n, auto out, auto act) {
+    return dispatch<0, 1>(g->a_layout, bad_layout, [&](auto a_mn) {
+      return dispatch<0, 1>(g->b_layout, bad_layout, [&](auto b_mn) {
+        constexpr auto kern = gemm_kernel<tile_n.value, a_mn.value, b_mn.value, out.value, act.value>;
+        constexpr int smem = GemmCfg<tile_n.value>::SMEM_BYTES;
+        if (smem_limit<kern>(smem)) return -1;
+        kern<<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, dev);
+        XP_CHECK_LAUNCH("gemm_kernel");
+        return 0;
+      });
+    });
+  };
+  // The activation epilogues exist for bf16 outputs only (forward activations / their gradients).
+  using no_act = std::integral_constant<int, XP_ACT_NONE>;
+  return dispatch<256, 128>(bn, bad_bn, [&](auto tile_n) {
+    return dispatch<XP_OUT_BF16, XP_OUT_F32, XP_OUT_F32_ATOMIC>(g->out, "xp_gemm: bad out mode", [&](auto out) {
+      if constexpr (out.value != XP_OUT_BF16)
+        return launch(tile_n, out, no_act{});
+      else
+        return dispatch<XP_ACT_NONE, XP_ACT_QUICK_GELU, XP_ACT_DQUICK_GELU, XP_ACT_GELU_ERF, XP_ACT_DGELU_ERF>(
+            g->act, "xp_gemm: bad act", [&](auto act) { return launch(tile_n, out, act); });
+    });
+  });
 }

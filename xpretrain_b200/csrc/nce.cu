@@ -135,23 +135,18 @@ __device__ void tile_partials(const float (&rv)[kRowsPerWarp][4], const float (&
       float t = 0.f;
 #pragma unroll
       for (int k = 0; k < 4; ++k) t += keep(r, k) ? rv[r][k] : 0.f;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-      acc = make_float2(t, 0.f);
+      acc = make_float2(warp_sum(t), 0.f);
     } else {
       float mx = -INFINITY;
 #pragma unroll
       for (int k = 0; k < 4; ++k) mx = fmaxf(mx, keep(r, k) ? rv[r][k] : -INFINITY);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      mx = warp_max(mx);
       float t = 0.f;
       if (mx != -INFINITY) {
 #pragma unroll
         for (int k = 0; k < 4; ++k) t += keep(r, k) ? __expf(rv[r][k] - mx) : 0.f;
       }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-      acc = make_float2(mx, t);
+      acc = make_float2(mx, warp_sum(t));
     }
     if (lane == 0) rowdst[i] = acc;
   }
@@ -263,8 +258,7 @@ __global__ void __launch_bounds__(kCombineThreads) nce_combine_kernel(const NceP
 }
 
 __device__ __forceinline__ float block_sum(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();

@@ -45,8 +45,7 @@ opt_sumsq_kernel(const XpOptTensor* __restrict__ table, const int2* __restrict__
   } else {
     for (long long i = lo + threadIdx.x; i < hi; i += OPT_THREADS) acc += g[i] * g[i];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -64,8 +63,7 @@ opt_norm_finalize_kernel(const float* __restrict__ partial, int n, float max_nor
   __shared__ double red[32];
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += 1024) acc += static_cast<double>(partial[i]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {

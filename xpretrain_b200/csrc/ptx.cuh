@@ -5,6 +5,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -233,6 +234,87 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
+
+// ------------------------------------------------------- 8-wide conversions
+// Eight consecutive elements <-> float[8]: one 16-byte access for bf16 / fp16, two for fp32.
+__device__ __forceinline__ void unpack8_bf16(const uint4& u, float (&f)[8]) {
+  f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
+  f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
+}
+__device__ __forceinline__ uint4 pack8_bf16(const float (&f)[8]) {
+  uint4 u;
+  u.x = pack_bf16(f[0], f[1]); u.y = pack_bf16(f[2], f[3]); u.z = pack_bf16(f[4], f[5]); u.w = pack_bf16(f[6], f[7]);
+  return u;
+}
+__device__ __forceinline__ void unpack8_f16(const uint4& u, float (&f)[8]) {
+  const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 v = __half22float2(h[i]);
+    f[2 * i] = v.x;
+    f[2 * i + 1] = v.y;
+  }
+}
+// Saturating: a value beyond fp16's range becomes +-65504, not inf (the row kernels' fp16 residual stream, DESIGN §3).
+__device__ __forceinline__ uint4 pack8_f16_satfinite(const float (&f)[8]) {
+  uint4 u;
+  uint32_t* w = reinterpret_cast<uint32_t*>(&u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(w[i]) : "f"(f[2 * i + 1]), "f"(f[2 * i]));
+  return u;
+}
+__device__ __forceinline__ void load8(const float* p, float (&f)[8]) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+__device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8]) {
+  unpack8_bf16(*reinterpret_cast<const uint4*>(p), f);
+}
+__device__ __forceinline__ void load8(const __half* p, float (&f)[8]) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  unpack8_f16(u, f);
+}
+__device__ __forceinline__ void store8(float* p, const float (&f)[8]) {
+  *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
+}
+__device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
+  *reinterpret_cast<uint4*>(p) = pack8_bf16(f);
+}
+__device__ __forceinline__ void store8_satfinite(__half* p, const float (&f)[8]) {
+  *reinterpret_cast<uint4*>(p) = pack8_f16_satfinite(f);
+}
+
+// Scalar conversions (round to nearest; fp16 overflows to inf).
+template <typename T>
+__device__ __forceinline__ float to_f32(T v) { return static_cast<float>(v); }
+template <>
+__device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <>
+__device__ __forceinline__ float to_f32<__half>(__half v) { return __half2float(v); }
+template <typename T>
+__device__ __forceinline__ T from_f32(float v);
+template <>
+__device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <>
+__device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16(v); }
+template <>
+__device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half(v); }
+
+// ------------------------------------------------------- warp reductions
+// Over all 32 lanes, xor butterfly: every lane gets the result.
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
 
 // sigmoid(y) = 0.5 + 0.5 * tanh(y / 2): ONE MUFU op (tanh.approx) instead of ex2 + rcp — the GELU epilogues of
 // the fc1 GEMMs issue many MUFU ops per output element.  tanh.approx is good to ~2^-11, below bf16's 2^-9.

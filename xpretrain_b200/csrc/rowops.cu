@@ -7,7 +7,6 @@
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "ptx.cuh"
-#include <cuda_fp16.h>
 
 namespace xp {
 
@@ -31,69 +30,12 @@ static RowMapDev to_dev(const XpRowMap& m) {
 
 constexpr int LN_MAX_VEC = 4;  // C <= 4 * 32 * 8 = 1024
 
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
-  f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u;
-  u.x = pack_bf16(f[0], f[1]); u.y = pack_bf16(f[2], f[3]); u.z = pack_bf16(f[4], f[5]); u.w = pack_bf16(f[6], f[7]);
-  return u;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ------------------------------------------------------------------ LayerNorm forward
 // Optionally fused with the residual add in fp32 (the reference keeps the residual stream in fp32 under autocast; a bf16
 // stream multiplies its feature error):  s = x (+ add);  sum_out = s (fp32);
-// y = LN(s).  x is bf16 or fp32 (XF32), y bf16 or fp32 (YF32), add is the bf16 branch output (ADD).
-__device__ __forceinline__ void unpack8_h(const uint4& u, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 v = __half22float2(h[i]);
-    f[2 * i] = v.x;
-    f[2 * i + 1] = v.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8_h(const float (&f)[8]) {   // saturating: a value beyond fp16's range becomes +-65504, not inf
-  uint4 u;
-  uint32_t* w = reinterpret_cast<uint32_t*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(w[i]) : "f"(f[2 * i + 1]), "f"(f[2 * i]));
-  return u;
-}
-// DT: 0 = bf16, 1 = fp32, 2 = fp16 (the residual stream may be kept in fp32, or in fp16 as under the reference's apex O2)
-template <int DT>
-__device__ __forceinline__ void ld8(const void* base, long long off, float (&f)[8]) {
-  if (DT == 2) {
-    unpack8_h(*reinterpret_cast<const uint4*>(static_cast<const __half*>(base) + off), f);
-  } else if (DT == 1) {
-    const float* p = static_cast<const float*>(base) + off;
-    const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
-    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-  } else {
-    unpack8(*reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(base) + off), f);
-  }
-}
-template <int DT>
-__device__ __forceinline__ void st8(void* base, long long off, const float (&f)[8]) {
-  if (DT == 2) {
-    *reinterpret_cast<uint4*>(static_cast<__half*>(base) + off) = pack8_h(f);
-  } else if (DT == 1) {
-    float* p = static_cast<float*>(base) + off;
-    *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
-    *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
-  } else {
-    *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(base) + off) = pack8(f);
-  }
-}
-
-template <int XT, int YT, bool ADD>
+// y = LN(s).  XT / YT are the element types of x and y: bf16, fp32, or fp16 (the residual stream may be kept in fp32,
+// or in fp16 as under the reference's apex O2); add is the bf16 branch output (ADD).
+template <class XT, class YT, bool ADD>
 __global__ void __launch_bounds__(128)
 ln_fwd_kernel(const void* __restrict__ x, RowMapDev xm, const __nv_bfloat16* __restrict__ add, RowMapDev am,
               void* __restrict__ sum_out, RowMapDev sm, void* __restrict__ y, RowMapDev ym,
@@ -112,18 +54,21 @@ ln_fwd_kernel(const void* __restrict__ x, RowMapDev xm, const __nv_bfloat16* __r
   for (int i = 0; i < LN_MAX_VEC; ++i) {
     const int c = lane + i * 32;
     if (c < nvec) {
-      ld8<XT>(x, xo + c * 8, v[i]);
+      if constexpr (std::is_same_v<XT, __half>)
+        unpack8_f16(*reinterpret_cast<const uint4*>(static_cast<const __half*>(x) + xo + c * 8), v[i]);
+      else
+        load8(static_cast<const XT*>(x) + xo + c * 8, v[i]);
       if (ADD) {
         float a[8];
-        unpack8(*reinterpret_cast<const uint4*>(add + ao + c * 8), a);
+        load8(add + ao + c * 8, a);
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[i][j] += a[j];
-        if (XT == 2) {                       // fp16 stream: normalise exactly the rounded values that are stored / read back later
-          const uint4 hv = pack8_h(v[i]);
-          unpack8_h(hv, v[i]);
+        if constexpr (std::is_same_v<XT, __half>) {   // fp16 stream: normalise exactly the rounded values that are stored / read back later
+          const uint4 hv = pack8_f16_satfinite(v[i]);
+          unpack8_f16(hv, v[i]);
           if (sum_out) *reinterpret_cast<uint4*>(static_cast<__half*>(sum_out) + so + c * 8) = hv;
         } else if (sum_out) {                // bf16 / fp32 x: the stream is stored in fp32
-          st8<1>(sum_out, so + c * 8, v[i]);
+          store8(static_cast<float*>(sum_out) + so + c * 8, v[i]);
         }
       }
 #pragma unroll
@@ -155,7 +100,8 @@ ln_fwd_kernel(const void* __restrict__ x, RowMapDev xm, const __nv_bfloat16* __r
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[i][j] - mean) * rstd * gg[j] + bb[j];
-      st8<YT>(y, yo + c * 8, o);
+      if constexpr (std::is_same_v<YT, __half>) store8_satfinite(static_cast<__half*>(y) + yo + c * 8, o);
+      else store8(static_cast<YT*>(y) + yo + c * 8, o);
     }
   }
   if (lane == 0) {
@@ -171,7 +117,7 @@ constexpr int LNB_WARPS = 8;
 // RSUM: additionally accumulate the column sums of dres into dres_sum — dres is the gradient of a residual add whose other
 // branch ends in a Linear, so its column sum IS that Linear's bias gradient (fc2.bias from LN2's dres, out_proj.bias from
 // LN1's): the pass that already streams dres produces it, and the standalone colsum launches disappear.
-template <int NVEC, bool RSUM, int XT>
+template <int NVEC, bool RSUM, class XT>
 __global__ void __launch_bounds__(LNB_WARPS * 32, 2)
 ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowMapDev dym, const void* __restrict__ x, RowMapDev xm,
               const float* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ rstd,
@@ -198,7 +144,7 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowMapDev dym, const void* _
     const __nv_bfloat16* dyr = dy + row_addr(dym, r);
     const __nv_bfloat16* drr = dres ? dres + row_addr(drm, r) : nullptr;
     const float mu = mean[r], rs = rstd[r];
-    constexpr bool XF32 = XT == 1;
+    constexpr bool XF32 = std::is_same_v<XT, float>;
     uint4 xraw[XF32 ? 1 : NVEC], draw[NVEC], rraw[NVEC];     // an fp32 x is re-read (L1) in the second pass, not kept
 #pragma unroll
     for (int i = 0; i < NVEC; ++i) {
@@ -215,10 +161,10 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowMapDev dym, const void* _
       const int c = lane + i * 32;
       if (c < nvec) {
         float xv[8], dv[8];
-        if (XF32) ld8<1>(x, xo + c * 8, xv);
-        else if (XT == 2) unpack8_h(xraw[i], xv);
-        else unpack8(xraw[i], xv);
-        unpack8(draw[i], dv);
+        if (XF32) load8(static_cast<const float*>(x) + xo + c * 8, xv);
+        else if (std::is_same_v<XT, __half>) unpack8_f16(xraw[i], xv);
+        else unpack8_bf16(xraw[i], xv);
+        unpack8_bf16(draw[i], dv);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float xh = (xv[j] - mu) * rs;
@@ -238,10 +184,10 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowMapDev dym, const void* _
       const int c = lane + i * 32;
       if (c < nvec) {
         float xv[8], dv[8], o[8];
-        if (XF32) ld8<1>(x, xo + c * 8, xv);
-        else if (XT == 2) unpack8_h(xraw[i], xv);
-        else unpack8(xraw[i], xv);
-        unpack8(draw[i], dv);
+        if (XF32) load8(static_cast<const float*>(x) + xo + c * 8, xv);
+        else if (std::is_same_v<XT, __half>) unpack8_f16(xraw[i], xv);
+        else unpack8_bf16(xraw[i], xv);
+        unpack8_bf16(draw[i], dv);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float xh = (xv[j] - mu) * rs;
@@ -249,14 +195,14 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowMapDev dym, const void* _
         }
         if (drr) {
           float rv[8];
-          unpack8(rraw[i], rv);
+          unpack8_bf16(rraw[i], rv);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             o[j] += rv[j];
             if (RSUM) ar[i][j] += rv[j];
           }
         }
-        *reinterpret_cast<uint4*>(dxr + c * 8) = pack8(o);
+        store8(dxr + c * 8, o);
       }
     }
   }
@@ -415,7 +361,7 @@ colsum_kernel(const __nv_bfloat16* __restrict__ x, long long ld, float* __restri
   if (c0 < C) {
     for (long long r = static_cast<long long>(blockIdx.y) * 8 + rl; r < rows; r += static_cast<long long>(gridDim.y) * 8) {
       float v[8];
-      unpack8(*reinterpret_cast<const uint4*>(x + r * ld + c0), v);
+      load8(x + r * ld + c0, v);
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] += v[j];
     }
@@ -437,9 +383,9 @@ __global__ void __launch_bounds__(256)
 cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
   const long long i = (static_cast<long long>(blockIdx.x) * 256 + threadIdx.x) * 8;
   if (i + 8 <= n) {
-    const float4 a = *reinterpret_cast<const float4*>(src + i), b = *reinterpret_cast<const float4*>(src + i + 4);
-    const float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    *reinterpret_cast<uint4*>(dst + i) = pack8(f);
+    float f[8];
+    load8(src + i, f);
+    store8(dst + i, f);
   } else {
     for (long long j = i; j < n; ++j) dst[j] = __float2bfloat16(src[j]);
   }
@@ -458,17 +404,17 @@ rowscale_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ s
   const long long off = r * C + (idx - r * vec) * 8;
   const float s = scale[r];
   float v[8];
-  unpack8(*reinterpret_cast<const uint4*>(x + off), v);
+  load8(x + off, v);
   if (res != nullptr) {
     float q[8];
-    unpack8(*reinterpret_cast<const uint4*>(res + off), q);
+    load8(res + off, q);
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[j] = q[j] + s * v[j];
   } else {
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[j] *= s;
   }
-  *reinterpret_cast<uint4*>(out + off) = pack8(v);
+  store8(out + off, v);
 }
 
 // ------------------------------------------------- LayerNorm over rows wider than 1024 columns
@@ -478,8 +424,7 @@ rowscale_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ s
 constexpr int LNW_THREADS = 256;
 constexpr int LNW_MAXK = 2;            // C <= 2 * 2048
 __device__ __forceinline__ float block_sum256(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   __syncthreads();                     // protects `red` against the previous use
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -501,7 +446,7 @@ ln_wide_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restric
   for (int k = 0; k < LNW_MAXK; ++k) {
     const int c = threadIdx.x * 8 + k * LNW_THREADS * 8;
     if (c < C) {
-      unpack8(*reinterpret_cast<const uint4*>(xr + c), v[k]);
+      load8(xr + c, v[k]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) s += v[k][j];
     }
@@ -522,7 +467,7 @@ ln_wide_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restric
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[k][j] - mean) * rstd * gamma[c + j] + beta[c + j];
-      *reinterpret_cast<uint4*>(y + r * C + c) = pack8(o);
+      store8(y + r * C + c, o);
     }
   }
   if (threadIdx.x == 0) {
@@ -547,8 +492,8 @@ ln_wide_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __
       const int c = threadIdx.x * 8 + k * LNW_THREADS * 8;
       if (c < C) {
         float d[8], xv[8];
-        unpack8(*reinterpret_cast<const uint4*>(dy + r * C + c), d);
-        unpack8(*reinterpret_cast<const uint4*>(x + r * C + c), xv);
+        load8(dy + r * C + c, d);
+        load8(x + r * C + c, xv);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           xh[k][j] = (xv[j] - mu) * rs;
@@ -569,7 +514,7 @@ ln_wide_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = rs * (g[k][j] - m1 - xh[k][j] * m2);
-        *reinterpret_cast<uint4*>(dx + r * C + c) = pack8(o);
+        store8(dx + r * C + c, o);
       }
     }
   }
@@ -689,9 +634,10 @@ extern "C" int xp_layernorm_add_fwd(const void* x, const XpRowMap* xmap, int32_t
                                     float* rstd, int64_t rows, int32_t C, float eps, void* stream) {
   XP_ENTER(x);
   if (C % 8 || C > LN_MAX_VEC * 256) return fail("xp_layernorm_fwd: C must be a multiple of 8 and <= 1024");
+  const char* bad_dtype = "xp_layernorm_add_fwd: x / y dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16";
   if ((x_dtype != XP_DTYPE_BF16 && x_dtype != XP_DTYPE_F32 && x_dtype != XP_DTYPE_F16) ||
       (y_dtype != XP_DTYPE_BF16 && y_dtype != XP_DTYPE_F32 && y_dtype != XP_DTYPE_F16))
-    return fail("xp_layernorm_add_fwd: x / y dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16");
+    return fail(bad_dtype);
   if (add_bf16 != nullptr && addmap == nullptr) return fail("xp_layernorm_add_fwd: add needs its row map");
   if (sum_out != nullptr && (add_bf16 == nullptr || summap == nullptr)) return fail("xp_layernorm_add_fwd: sum_out needs add and its row map");
   if (rows <= 0) return 0;
@@ -700,26 +646,16 @@ extern "C" int xp_layernorm_add_fwd(const void* x, const XpRowMap* xmap, int32_t
   XpRowMap none = {0, 0, 0, nullptr};
   const RowMapDev xm = to_dev(*xmap), am = to_dev(addmap ? *addmap : none), sm = to_dev(summap ? *summap : none), ym = to_dev(*ymap);
   const __nv_bfloat16* add = static_cast<const __nv_bfloat16*>(add_bf16);
-#define XP_LNF(XT_, YT_, AD) \
-  ln_fwd_kernel<XT_, YT_, AD><<<grid, 128, 0, st>>>(x, xm, add, am, sum_out, sm, y, ym, gamma, beta, mean, rstd, rows, C, eps)
-  // dtype codes of the kernels: 0 bf16, 1 fp32, 2 fp16
-  const int xt = x_dtype == XP_DTYPE_F32 ? 1 : (x_dtype == XP_DTYPE_F16 ? 2 : 0);
-  const int yt = y_dtype == XP_DTYPE_F32 ? 1 : (y_dtype == XP_DTYPE_F16 ? 2 : 0);
-  const bool ad = add_bf16 != nullptr;
-#define XP_LNF_Y(XT_)                                      \
-  do {                                                     \
-    if (yt == 0 && !ad) XP_LNF(XT_, 0, false);             \
-    else if (yt == 0 && ad) XP_LNF(XT_, 0, true);          \
-    else if (yt == 1 && !ad) XP_LNF(XT_, 1, false);        \
-    else if (yt == 1 && ad) XP_LNF(XT_, 1, true);          \
-    else if (yt == 2 && !ad) XP_LNF(XT_, 2, false);        \
-    else XP_LNF(XT_, 2, true);                             \
-  } while (0)
-  if (xt == 0) XP_LNF_Y(0);
-  else if (xt == 1) XP_LNF_Y(1);
-  else XP_LNF_Y(2);
-#undef XP_LNF_Y
-#undef XP_LNF
+  int rc = dispatch_dtype(x_dtype, bad_dtype, [&](auto xt) {
+    return dispatch_dtype(y_dtype, bad_dtype, [&](auto yt) {
+      return dispatch<0, 1>(add != nullptr, bad_dtype, [&](auto ad) {
+        ln_fwd_kernel<decltype(xt), decltype(yt), ad.value><<<grid, 128, 0, st>>>(x, xm, add, am, sum_out, sm, y, ym, gamma,
+                                                                                 beta, mean, rstd, rows, C, eps);
+        return 0;
+      });
+    });
+  });
+  if (rc) return rc;
   XP_CHECK_LAUNCH("ln_fwd_kernel");
   return 0;
 }
@@ -729,9 +665,10 @@ extern "C" int xp_layernorm_bwd(const void* dy, const XpRowMap* dymap, const voi
                                 const XpRowMap* drmap, void* dx, const XpRowMap* dxmap, float* dgamma, float* dbeta,
                                 float* dres_colsum, int64_t rows, int32_t C, void* stream) {
   XP_ENTER(dy);
-  if (x_dtype != XP_DTYPE_BF16 && x_dtype != XP_DTYPE_F32 && x_dtype != XP_DTYPE_F16)
-    return fail("xp_layernorm_bwd: x dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16");
-  if (C % 8 || C > LN_MAX_VEC * 256) return fail("xp_layernorm_bwd: C must be a multiple of 8 and <= 1024");
+  const char* bad_dtype = "xp_layernorm_bwd: x dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16";
+  const char* bad_c = "xp_layernorm_bwd: C must be a multiple of 8 and <= 1024";
+  if (x_dtype != XP_DTYPE_BF16 && x_dtype != XP_DTYPE_F32 && x_dtype != XP_DTYPE_F16) return fail(bad_dtype);
+  if (C % 8 || C > LN_MAX_VEC * 256) return fail(bad_c);
   if (dres_colsum != nullptr && dres == nullptr) return fail("xp_layernorm_bwd: dres_colsum needs dres");
   if (rows <= 0) return 0;
   long long want = (rows + LNB_WARPS - 1) / LNB_WARPS;
@@ -740,35 +677,20 @@ extern "C" int xp_layernorm_bwd(const void* dy, const XpRowMap* dymap, const voi
   const size_t smem = (static_cast<size_t>(LNB_WARPS) * (rsum ? 3 : 2) + 1) * C * sizeof(float);
   XpRowMap none = {0, 0, 0, nullptr};
   const int nv = (C / 8 + 31) / 32;
-  const int xt = x_dtype == XP_DTYPE_F32 ? 1 : (x_dtype == XP_DTYPE_F16 ? 2 : 0);
-#define XP_LNB_LAUNCH(NV, RS, XF)                                                                                   \
-  do {                                                                                                              \
-    static bool attr = false;                                                                                       \
-    if (!attr) {                                                                                                    \
-      XP_CHECK_CUDA(cudaFuncSetAttribute(ln_bwd_kernel<NV, RS, XF>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
-                                         (LNB_WARPS * (RS ? 3 : 2) + 1) * 1024 * 4));                               \
-      attr = true;                                                                                                  \
-    }                                                                                                               \
-    ln_bwd_kernel<NV, RS, XF><<<grid, LNB_WARPS * 32, smem, static_cast<cudaStream_t>(stream)>>>(                   \
-        static_cast<const __nv_bfloat16*>(dy), to_dev(*dymap), x, to_dev(*xmap),                                    \
-        gamma, mean, rstd, static_cast<const __nv_bfloat16*>(dres), to_dev(drmap ? *drmap : none),                  \
-        static_cast<__nv_bfloat16*>(dx), to_dev(*dxmap), dgamma, dbeta, dres_colsum, rows, C);                      \
-  } while (0)
-#define XP_LNB_PICK(NV)                                    \
-  do {                                                     \
-    if (rsum && xt == 1) XP_LNB_LAUNCH(NV, true, 1);       \
-    else if (rsum && xt == 2) XP_LNB_LAUNCH(NV, true, 2);  \
-    else if (rsum) XP_LNB_LAUNCH(NV, true, 0);             \
-    else if (xt == 1) XP_LNB_LAUNCH(NV, false, 1);         \
-    else if (xt == 2) XP_LNB_LAUNCH(NV, false, 2);         \
-    else XP_LNB_LAUNCH(NV, false, 0);                      \
-  } while (0)
-  if (nv == 1) XP_LNB_PICK(1);
-  else if (nv == 2) XP_LNB_PICK(2);
-  else if (nv == 3) XP_LNB_PICK(3);
-  else XP_LNB_PICK(4);
-#undef XP_LNB_PICK
-#undef XP_LNB_LAUNCH
+  const int rc = dispatch<1, 2, 3, 4>(nv < 1 ? 4 : nv, bad_c, [&](auto nvec) {   // C <= 0: the widest variant, no columns
+    return dispatch<0, 1>(rsum, bad_c, [&](auto rs) {
+      return dispatch_dtype(x_dtype, bad_dtype, [&](auto xt) {
+        constexpr auto kern = ln_bwd_kernel<nvec.value, rs.value, decltype(xt)>;
+        if (smem_limit<kern>((LNB_WARPS * (rs.value ? 3 : 2) + 1) * 1024 * 4)) return -1;
+        kern<<<grid, LNB_WARPS * 32, smem, static_cast<cudaStream_t>(stream)>>>(
+            static_cast<const __nv_bfloat16*>(dy), to_dev(*dymap), x, to_dev(*xmap), gamma, mean, rstd,
+            static_cast<const __nv_bfloat16*>(dres), to_dev(drmap ? *drmap : none), static_cast<__nv_bfloat16*>(dx),
+            to_dev(*dxmap), dgamma, dbeta, dres_colsum, rows, C);
+        return 0;
+      });
+    });
+  });
+  if (rc) return rc;
   XP_CHECK_LAUNCH("ln_bwd_kernel");
   return 0;
 }
@@ -840,7 +762,7 @@ extern "C" int xp_colsum_bf16(const void* x, int64_t ld, float* out, int64_t row
 extern "C" int xp_cast_f32_bf16(const float* src, void* dst, int64_t n, void* stream) {
   XP_ENTER(src);
   if (n <= 0) return 0;
-  if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 15))
+  if (!aligned(src, 16) || !aligned(dst, 16))
     return fail("xp_cast_f32_bf16: pointers must be 16-byte aligned");
   const long long blocks = (n + 2047) / 2048;
   cast_f32_bf16_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(

@@ -46,9 +46,6 @@ __device__ __forceinline__ int seq_len(const SegDev& d, long long base) {
   const long long fit = (d.n_rows - base + d.tok_stride - 1) / d.tok_stride;
   return static_cast<int>(fit < d.L ? fit : d.L);
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // Token row of position i of sequence s.
 __device__ __forceinline__ long long tok_row(const SegDev& d, int s, long long base, int i) {
@@ -564,13 +561,15 @@ seg_attn_dq_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* _
   }
 }
 
+constexpr const char* SEG_BAD_HD = "xp_seg_attention: head_dim must be 64 (or 0) or 32";
+
 static int to_dev(const XpSegAttn* a, SegDev& d, const char* who) {
   if (a == nullptr) return fail("xp_seg_attention: null descriptor");
   if (a->heads <= 0 || a->n_rows <= 0 || a->n_seq <= 0 || a->seq_len <= 0 || a->seg_len <= 0 || a->inner <= 0 ||
       a->tok_stride <= 0)
     return fail("xp_seg_attention: heads, n_rows, n_seq, seq_len, seg_len, inner and tok_stride must be positive");
   d.hd = a->head_dim == 0 ? HD : a->head_dim;
-  if (d.hd != 64 && d.hd != 32) return fail("xp_seg_attention: head_dim must be 64 (or 0) or 32");
+  if (d.hd != 64 && d.hd != 32) return fail(SEG_BAD_HD);
   d.H = a->heads;
   d.C = a->heads * d.hd;
   d.idx = a->row_index;
@@ -596,29 +595,29 @@ constexpr int SEG_DQ_SMEM = 6 * SEG_TILE_BYTES + 128;
 using namespace xp;
 
 // grid (64-row blocks, heads, sequences); the z limit of 65535 sequences is checked by the callers below
-#define SEG_GRID(d) dim3(((d).L + SEG_BLK - 1) / SEG_BLK, (d).H, (d).n_seq)
+static dim3 seg_grid(const SegDev& d) { return dim3((d.L + SEG_BLK - 1) / SEG_BLK, d.H, d.n_seq); }
+
+// f(head_dim, with_bias) as template arguments; to_dev has refused every other head_dim
+template <class F>
+static int seg_dispatch(const SegDev& d, F&& f) {
+  return dispatch<64, 32>(d.hd, SEG_BAD_HD, [&](auto hd) {
+    return dispatch<0, 1>(d.bias != nullptr, SEG_BAD_HD, [&](auto b) { return f(hd, b); });
+  });
+}
 
 extern "C" int xp_seg_attention_fwd(const void* qkv, void* out, float* lse, const XpSegAttn* desc, void* stream) {
   XP_ENTER(qkv);
   SegDev d;
   if (int rc = to_dev(desc, d, "fwd")) return rc;
   if (d.n_seq > 65535) return fail("xp_seg_attention_fwd: n_seq > 65535 (split the call)");
-  static bool attr = false;
-  if (!attr) {
-#define SEG_FOR_VARIANTS(X) X(64, false) X(64, true) X(32, false) X(32, true)
-#define SEG_ATTR_FWD(H, B) \
-    XP_CHECK_CUDA(cudaFuncSetAttribute(seg_attn_fwd_kernel<H, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, SEG_FWD_SMEM));
-    SEG_FOR_VARIANTS(SEG_ATTR_FWD)
-    attr = true;
-  }
-  const bool with_bias = d.bias != nullptr;
-#define SEG_LAUNCH_FWD(H, B)                                                                                       \
-  if (d.hd == H && with_bias == B)                                                                                 \
-    seg_attn_fwd_kernel<H, B><<<SEG_GRID(d), SEG_THREADS, SEG_FWD_SMEM, static_cast<cudaStream_t>(stream)>>>(      \
+  return seg_dispatch(d, [&](auto hd, auto b) {
+    constexpr auto kern = seg_attn_fwd_kernel<hd.value, b.value>;
+    if (smem_limit<kern>(SEG_FWD_SMEM)) return -1;
+    kern<<<seg_grid(d), SEG_THREADS, SEG_FWD_SMEM, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(out), lse, d);
-  SEG_FOR_VARIANTS(SEG_LAUNCH_FWD)
-  XP_CHECK_LAUNCH("seg_attn_fwd_kernel");
-  return 0;
+    XP_CHECK_LAUNCH("seg_attn_fwd_kernel");
+    return 0;
+  });
 }
 
 extern "C" int xp_seg_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta,
@@ -627,30 +626,22 @@ extern "C" int xp_seg_attention_bwd(const void* qkv, const void* out, const void
   SegDev d;
   if (int rc = to_dev(desc, d, "bwd")) return rc;
   if (d.n_seq > 65535) return fail("xp_seg_attention_bwd: n_seq > 65535 (split the call)");
-  static bool attr = false;
-  if (!attr) {
-#define SEG_ATTR_BWD(H, B)                                                                                                  \
-    XP_CHECK_CUDA(cudaFuncSetAttribute(seg_attn_dkv_kernel<H, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, SEG_DKV_SMEM)); \
-    XP_CHECK_CUDA(cudaFuncSetAttribute(seg_attn_dq_kernel<H, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, SEG_DQ_SMEM));
-    SEG_FOR_VARIANTS(SEG_ATTR_BWD)
-    attr = true;
-  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const long long items = d.n_rows * d.H * 8;
-  seg_attn_delta_kernel<<<static_cast<unsigned>((items + 255) / 256), 256, 0, st>>>(
-      static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), delta, d.n_rows, d.H, d.ld_o, d.hd);
-  XP_CHECK_LAUNCH("seg_attn_delta_kernel");
   const __nv_bfloat16* qp = static_cast<const __nv_bfloat16*>(qkv);
   const __nv_bfloat16* dop = static_cast<const __nv_bfloat16*>(dout);
   __nv_bfloat16* dqp = static_cast<__nv_bfloat16*>(dqkv);
-  const bool with_bias = d.bias != nullptr;
-#define SEG_LAUNCH_DKV(H, B) \
-  if (d.hd == H && with_bias == B) seg_attn_dkv_kernel<H, B><<<SEG_GRID(d), SEG_THREADS, SEG_DKV_SMEM, st>>>(qp, dop, lse, delta, dqp, d);
-  SEG_FOR_VARIANTS(SEG_LAUNCH_DKV)
-  XP_CHECK_LAUNCH("seg_attn_dkv_kernel");
-#define SEG_LAUNCH_DQ(H, B) \
-  if (d.hd == H && with_bias == B) seg_attn_dq_kernel<H, B><<<SEG_GRID(d), SEG_THREADS, SEG_DQ_SMEM, st>>>(qp, dop, lse, delta, dqp, d, q_scale);
-  SEG_FOR_VARIANTS(SEG_LAUNCH_DQ)
-  XP_CHECK_LAUNCH("seg_attn_dq_kernel");
-  return 0;
+  return seg_dispatch(d, [&](auto hd, auto b) {
+    constexpr auto dkv = seg_attn_dkv_kernel<hd.value, b.value>;
+    constexpr auto dq = seg_attn_dq_kernel<hd.value, b.value>;
+    if (smem_limit<dkv>(SEG_DKV_SMEM) || smem_limit<dq>(SEG_DQ_SMEM)) return -1;
+    const long long items = d.n_rows * d.H * 8;
+    seg_attn_delta_kernel<<<static_cast<unsigned>((items + 255) / 256), 256, 0, st>>>(
+        static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), delta, d.n_rows, d.H, d.ld_o, d.hd);
+    XP_CHECK_LAUNCH("seg_attn_delta_kernel");
+    dkv<<<seg_grid(d), SEG_THREADS, SEG_DKV_SMEM, st>>>(qp, dop, lse, delta, dqp, d);
+    XP_CHECK_LAUNCH("seg_attn_dkv_kernel");
+    dq<<<seg_grid(d), SEG_THREADS, SEG_DQ_SMEM, st>>>(qp, dop, lse, delta, dqp, d, q_scale);
+    XP_CHECK_LAUNCH("seg_attn_dq_kernel");
+    return 0;
+  });
 }

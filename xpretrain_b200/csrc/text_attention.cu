@@ -61,16 +61,14 @@ text_attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, const long long* __r
       }
       mx = fmaxf(mx, s[u]);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    mx = warp_max(mx);
     float sum = 0.f;
 #pragma unroll
     for (int u = 0; u < 3; ++u) {
       s[u] = (lane + u * 32 < Lt) ? __expf(s[u] - mx) : 0.f;
       sum += s[u];
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    sum = warp_sum(sum);
     const float inv = 1.f / sum;
 #pragma unroll
     for (int u = 0; u < 3; ++u) {
@@ -132,8 +130,7 @@ text_attn_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16*
         dot += acc * sp[i * (Lt + 1) + j];
       }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+    dot = warp_sum(dot);
 #pragma unroll
     for (int u = 0; u < 3; ++u) {
       const int j = lane + u * 32;
@@ -175,12 +172,7 @@ extern "C" int xp_text_attention_fwd(const void* qkv, const int64_t* mask, void*
   if (C != H * TA_HD) return fail("xp_text_attention_fwd: head_dim must be 64");
   if (Lt > TA_MAXL || Lt < 1) return fail("xp_text_attention_fwd: 1 <= Lt <= 96");
   const int smem = 3 * Lt * TA_LDS * 4;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(text_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       3 * TA_MAXL * TA_LDS * 4));
-    attr = true;
-  }
+  if (smem_limit<text_attn_fwd_kernel>(3 * TA_MAXL * TA_LDS * 4)) return -1;
   text_attn_fwd_kernel<<<dim3(H, B), 128, smem, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<const long long*>(mask), static_cast<__nv_bfloat16*>(out),
       probs, Lt, C, H);
@@ -194,12 +186,7 @@ extern "C" int xp_text_attention_bwd(const void* qkv, const void* dout, const fl
   if (C != H * TA_HD) return fail("xp_text_attention_bwd: head_dim must be 64");
   if (Lt > TA_MAXL || Lt < 1) return fail("xp_text_attention_bwd: 1 <= Lt <= 96");
   const int smem = (4 * Lt * TA_LDS + 2 * Lt * (Lt + 1)) * 4;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(text_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (4 * TA_MAXL * TA_LDS + 2 * TA_MAXL * (TA_MAXL + 1)) * 4));
-    attr = true;
-  }
+  if (smem_limit<text_attn_bwd_kernel>((4 * TA_MAXL * TA_LDS + 2 * TA_MAXL * (TA_MAXL + 1)) * 4)) return -1;
   text_attn_bwd_kernel<<<dim3(H, B), 128, smem, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(qkv), static_cast<const __nv_bfloat16*>(dout), probs,
       static_cast<__nv_bfloat16*>(dqkv), Lt, C, H, q_scale);

@@ -7,30 +7,11 @@
 // broadcast adds in the reference, one pass here (32x32 shared-memory tiles, coalesced on both sides).
 // Backward: d x[b,t,c,p] = d token[(b,p,t), c] — the transposed copy; the table gradients are column sums of the token
 // gradient (xp_colsum_bf16 on reshaped views, see modeling/timesformer.py).
-#include <cuda_fp16.h>
-
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
 #include "ptx.cuh"
 
 namespace xp {
-
-template <typename T>
-__device__ __forceinline__ float to_f32(T v);
-template <>
-__device__ __forceinline__ float to_f32<float>(float v) { return v; }
-template <>
-__device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <>
-__device__ __forceinline__ float to_f32<__half>(__half v) { return __half2float(v); }
-template <typename T>
-__device__ __forceinline__ T from_f32(float v);
-template <>
-__device__ __forceinline__ float from_f32<float>(float v) { return v; }
-template <>
-__device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16(v); }
-template <>
-__device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half(v); }
 
 // grid (ceil(HW/32), ceil(C/32), B*T), block (32, 8)
 template <typename T>
@@ -96,14 +77,12 @@ extern "C" int xp_tsf_embed_fwd(const void* x, int32_t x_dtype, const float* pos
   const dim3 grid((HW + 31) / 32, (C + 31) / 32, B * T), block(32, 8);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   __nv_bfloat16* tok = static_cast<__nv_bfloat16*>(tokens);
-  switch (x_dtype) {
-    case XP_DTYPE_F32: tsf_embed_fwd_kernel<float><<<grid, block, 0, st>>>(static_cast<const float*>(x), pos, time, tok, T, C, HW); break;
-    case XP_DTYPE_BF16: tsf_embed_fwd_kernel<__nv_bfloat16><<<grid, block, 0, st>>>(static_cast<const __nv_bfloat16*>(x), pos, time, tok, T, C, HW); break;
-    case XP_DTYPE_F16: tsf_embed_fwd_kernel<__half><<<grid, block, 0, st>>>(static_cast<const __half*>(x), pos, time, tok, T, C, HW); break;
-    default: return fail("xp_tsf_embed_fwd: x_dtype must be XP_DTYPE_F32 / BF16 / F16");
-  }
-  XP_CHECK_LAUNCH("tsf_embed_fwd_kernel");
-  return 0;
+  return dispatch_dtype(x_dtype, "xp_tsf_embed_fwd: x_dtype must be XP_DTYPE_F32 / BF16 / F16", [&](auto t) {
+    using E = decltype(t);
+    tsf_embed_fwd_kernel<E><<<grid, block, 0, st>>>(static_cast<const E*>(x), pos, time, tok, T, C, HW);
+    XP_CHECK_LAUNCH("tsf_embed_fwd_kernel");
+    return 0;
+  });
 }
 
 extern "C" int xp_tsf_untokenize(const void* tokens, void* x, int32_t x_dtype, int32_t B, int32_t T, int32_t C, int32_t HW,
@@ -114,12 +93,10 @@ extern "C" int xp_tsf_untokenize(const void* tokens, void* x, int32_t x_dtype, i
   const dim3 grid((HW + 31) / 32, (C + 31) / 32, B * T), block(32, 8);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const __nv_bfloat16* tok = static_cast<const __nv_bfloat16*>(tokens);
-  switch (x_dtype) {
-    case XP_DTYPE_F32: tsf_embed_bwd_kernel<float><<<grid, block, 0, st>>>(tok, static_cast<float*>(x), T, C, HW); break;
-    case XP_DTYPE_BF16: tsf_embed_bwd_kernel<__nv_bfloat16><<<grid, block, 0, st>>>(tok, static_cast<__nv_bfloat16*>(x), T, C, HW); break;
-    case XP_DTYPE_F16: tsf_embed_bwd_kernel<__half><<<grid, block, 0, st>>>(tok, static_cast<__half*>(x), T, C, HW); break;
-    default: return fail("xp_tsf_untokenize: x_dtype must be XP_DTYPE_F32 / BF16 / F16");
-  }
-  XP_CHECK_LAUNCH("tsf_embed_bwd_kernel");
-  return 0;
+  return dispatch_dtype(x_dtype, "xp_tsf_untokenize: x_dtype must be XP_DTYPE_F32 / BF16 / F16", [&](auto t) {
+    using E = decltype(t);
+    tsf_embed_bwd_kernel<E><<<grid, block, 0, st>>>(tok, static_cast<E*>(x), T, C, HW);
+    XP_CHECK_LAUNCH("tsf_embed_bwd_kernel");
+    return 0;
+  });
 }

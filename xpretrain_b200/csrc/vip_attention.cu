@@ -333,11 +333,7 @@ extern "C" int xp_vip_attention_fwd(const void* qkv, void* out, float* lse, floa
   } else {
     CUtensorMap mL, mM;
     if (make_row_maps(&mL, &mM, qkv, 3LL * C, d)) return -1;
-    static bool attr = false;
-    if (!attr) {
-      XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-      attr = true;
-    }
+    if (smem_limit<vip_attn_fwd_kernel>(FWD_SMEM)) return -1;
     vip_attn_fwd_kernel<<<dim3(T, H, B), ATT_THREADS, FWD_SMEM, st>>>(mL, mM, static_cast<__nv_bfloat16*>(out), lse, workspace, d);
     XP_CHECK_LAUNCH("vip_attn_fwd_kernel");
   }
@@ -358,11 +354,7 @@ extern "C" int xp_vip_attention_bwd(const void* qkv, const void* out, const void
   } else {
     CUtensorMap mL, mM, gL, gM;
     if (make_row_maps(&mL, &mM, qkv, 3LL * C, d) || make_row_maps(&gL, &gM, dout, C, d)) return -1;
-    static bool attr = false;
-    if (!attr) {
-      XP_CHECK_CUDA(cudaFuncSetAttribute(vip_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-      attr = true;
-    }
+    if (smem_limit<vip_attn_bwd_kernel>(BWD_SMEM)) return -1;
     vip_attn_bwd_kernel<<<dim3(T, H, B), ATT_THREADS, BWD_SMEM, st>>>(
         mL, mM, gL, gM, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse,
         static_cast<__nv_bfloat16*>(dqkv), workspace, d, q_scale);

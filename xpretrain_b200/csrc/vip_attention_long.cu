@@ -197,12 +197,7 @@ int vip_long_attn_fwd(const AttnDims& d, const void* qkv, void* out, float* lse,
   if (long_grid(d, grid)) return -1;
   CUtensorMap tm;
   if (make_tmap_bf16_2d(&tm, qkv, d.ld_qkv, static_cast<uint64_t>(d.B) * d.S, d.ld_qkv, HD, ATILE)) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_fwd_kernel<VipLongFwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       LONG_FWD_SMEM));
-    attr = true;
-  }
+  if (smem_limit<stream_fwd_kernel<VipLongFwd>>(LONG_FWD_SMEM)) return -1;
   const VipLongFwd p{{d, 0}, static_cast<__nv_bfloat16*>(out), lse, part};
   stream_fwd_kernel<<<grid, STREAM_THREADS, LONG_FWD_SMEM, st>>>(tm, p);
   XP_CHECK_LAUNCH("vip_long_fwd_kernel");
@@ -218,14 +213,9 @@ int vip_long_attn_bwd(const AttnDims& d, const void* qkv, const void* out, const
   if (make_tmap_bf16_2d(&tm, qkv, d.ld_qkv, rows, d.ld_qkv, HD, ATILE) ||
       make_tmap_bf16_2d(&tdo, dout, d.ld_o, rows, d.ld_o, HD, ATILE))
     return -1;
-  static bool attr = false;
-  if (!attr) {
-    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_kv_kernel<VipLongBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       LONG_BWD_KV_SMEM));
-    XP_CHECK_CUDA(cudaFuncSetAttribute(stream_bwd_q_kernel<VipLongBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       LONG_BWD_Q_SMEM));
-    attr = true;
-  }
+  if (smem_limit<stream_bwd_kv_kernel<VipLongBwd>>(LONG_BWD_KV_SMEM) ||
+      smem_limit<stream_bwd_q_kernel<VipLongBwd>>(LONG_BWD_Q_SMEM))
+    return -1;
   const VipLongBwd p{{d, 0}, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse,
                      static_cast<__nv_bfloat16*>(dqkv), gpart, q_scale};
   stream_bwd_kv_kernel<<<grid, STREAM_THREADS, LONG_BWD_KV_SMEM, st>>>(tm, tdo, p);
