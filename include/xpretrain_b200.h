@@ -83,7 +83,12 @@ int xp_gemm(const XpGemm* g, void* stream);
  *   (r / group) * group_stride + (r % group) * ld         if group > 0
  *   r * ld                                                otherwise.
  * This is how the kernels skip the M global tokens of each video, pick the CLS row
- * (CLIP_ViP.py:891) or the EOS row (CLIP_ViP.py:776) without a gather copy. */
+ * (CLIP_ViP.py:891) or the EOS row (CLIP_ViP.py:776) without a gather copy.
+ * The row kernels move 16-byte vectors, so every row must start at a 16-byte-aligned address: the base pointer,
+ * ld * elsize and (when group > 0) group_stride * elsize must be multiples of 16 bytes, or the call is refused before any
+ * launch (a map whose operand is NULL is not read, and not checked).
+ * offsets[] lives in device memory and is not read by the host: each entry times elsize must be a multiple of 16 bytes
+ * as well (xp_eos_offsets emits multiples of C, and C % 8 == 0 is required). */
 typedef struct XpRowMap {
   int64_t group, group_stride, ld;
   const int64_t* offsets;
@@ -123,7 +128,7 @@ int xp_frame_pool_fwd(const float* proj, float* feat, float* inv_frame, float* i
                       void* stream);
 int xp_frame_pool_bwd(const float* dfeat, const float* feat, const float* proj, const float* inv_frame,
                       const float* inv_video, void* dproj_bf16, int32_t B, int32_t T, int32_t P, float scale, void* stream);
-/* out[c] += scale * sum_r x[r,c]: bias gradients of every nn.Linear. */
+/* out[c] += scale * sum_r x[r,c]: bias gradients of every nn.Linear.  x must be 16-byte aligned. */
 int xp_colsum_bf16(const void* x, int64_t ld, float* out, int64_t rows, int32_t C, float scale, void* stream);
 /* fp32 master parameter -> bf16 compute copy. */
 int xp_cast_f32_bf16(const float* src, void* dst_bf16, int64_t n, void* stream);
@@ -366,7 +371,7 @@ int xp_tsf_untokenize(const void* tokens_bf16, void* x, int32_t x_dtype, int32_t
                       void* stream);
 /* Stochastic depth on a residual branch (DropPath, timesformer.py:98-121, as Block.forward applies it :212,:218,:225):
  * out[r,:] = (residual ? residual[r,:] : 0) + scale[r] * x[r,:], all [rows, C] bf16 contiguous, scale fp32 per row
- * (0 or 1/keep_prob of the row's sample/group).  out may alias x. */
+ * (0 or 1/keep_prob of the row's sample/group).  out may alias x.  x, residual and out must be 16-byte aligned. */
 int xp_rowscale_bf16(const void* x, const float* scale, const void* residual, void* out, int64_t rows, int32_t C,
                      void* stream);
 
@@ -374,7 +379,8 @@ int xp_rowscale_bf16(const void* x, const float* scale, const void* residual, vo
  * xp_layernorm_wide_*: nn.LayerNorm over 1024 < C <= 4096 contiguous columns — PatchMerging.norm (4C = 2048, :281,:304).
  * xp_gather_rows_bf16 / xp_scatter_rows_bf16: out[i, :] = src[index[i], :] (zeros for index < 0) and its inverse
  * dst[index[i], :] = in[i, :] — the 2x2 neighbour concatenation of PatchMerging.forward (:292-301; out viewed as
- * [n/4... , 4C]) with its odd-size zero padding, and its backward. */
+ * [n/4... , 4C]) with its odd-size zero padding, and its backward.
+ * Every bf16 row operand of these four (x, y, dy, dx, src, out, in, dst) must be 16-byte aligned. */
 int xp_layernorm_wide_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mean, float* rstd,
                           int64_t rows, int32_t C, float eps, void* stream);
 int xp_layernorm_wide_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, void* dx,
@@ -389,7 +395,9 @@ int xp_scatter_rows_bf16(const void* in, const int32_t* index, void* dst, int64_
  *                   col_scratch: 2*cols floats
  *   xp_rank_counts  compute_metrics' rank search (:41-48) without the sort: greater[i] / equal[i] = number of entries of row i
  *                   (transpose != 0: column i) strictly larger than / equal to sim[i, i]; the reference's rank list is
- *                   {greater[i] + t : 0 <= t < equal[i]} (ties counted once per tied entry, as np.where(ind == 0) does). */
+ *                   {greater[i] + t : 0 <= t < equal[i]} (ties counted once per tied entry, as np.where(ind == 0) does).
+ *                   A NaN or +-inf diagonal gives equal[i] = 0: the reference's sort(-x) - diag(-x) is NaN or inf there,
+ *                   never 0, so that query leaves its rank list. */
 int xp_sim_f32(const float* a, const float* b, float* out, int32_t Na, int32_t Nb, int32_t d, int64_t ld, void* stream);
 int xp_dsl_reweight(float* sim, int32_t rows, int32_t cols, int64_t ld, float theta, float* col_scratch, void* stream);
 int xp_rank_counts(const float* sim, int32_t N, int64_t ld, int32_t transpose, int32_t* greater, int32_t* equal, void* stream);

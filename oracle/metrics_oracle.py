@@ -30,9 +30,11 @@ def dsl(sim, theta=100.0):
 
 
 def rank_counts(x):
-    """(greater[i], equal[i]) = how many entries of row i are strictly larger than / equal to x[i, i] (equal >= 1)."""
+    """(greater[i], equal[i]) = how many entries of row i are strictly larger than / equal to x[i, i].  compute_metrics
+    finds the diagonal's positions as the zeros of sort(-x) - diag(-x); with a NaN or +-inf diagonal that difference is NaN
+    or inf everywhere, never 0, so such a row has no position in the rank list: equal[i] = 0."""
     d = np.diag(x)[:, None]
-    return (x > d).sum(1), (x == d).sum(1)
+    return (x > d).sum(1), ((x == d) & np.isfinite(d)).sum(1)
 
 
 def ranks_from_counts(greater, equal):

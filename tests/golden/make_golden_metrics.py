@@ -7,7 +7,9 @@ Needs a checkout of the reference, named by XP_REFERENCE_ROOT:
 Imports CLIP-ViP/src/utils/metrics.py unmodified (pure numpy), evaluates a synthetic text/video feature set the way
 validate() does (run_pretrain.py:173-176, tasks/run_video_retrieval.py:155-172: simple and DSL, both directions) — including
 duplicated items, which exercise compute_metrics' tie quirk — asserts oracle/metrics_oracle.py agrees bit-for-bit and stores
-the features and the metrics.
+the features and the metrics (retrieval_metrics_n57.pt).  Then the same for similarity matrices holding special values
+(NaN, +-inf and +-0, on and off the diagonal, and few distinct levels): the reference's metric tuples and rank lists `ind`
+in both directions (retrieval_metrics_specials.pt).
 """
 import importlib.util
 import os
@@ -25,10 +27,63 @@ sys.dont_write_bytecode = True
 from oracle import metrics_oracle as O  # noqa: E402
 
 
-def main():
+def reference():
     spec = importlib.util.spec_from_file_location("ref_metrics", os.path.join(REF, "CLIP-ViP/src/utils/metrics.py"))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
+    return ref
+
+
+def reference_ind(x):
+    """The rank list compute_metrics builds (metrics.py:42-47), restated to store it beside the reference's tuple."""
+    with np.errstate(invalid="ignore"):
+        return np.where(np.sort(-x, axis=1) - np.diag(-x)[:, None] == 0)[1]
+
+
+def special_matrices():
+    rng = np.random.RandomState(5)
+    out = []
+    x = rng.randn(6, 6).astype(np.float32)
+    x[1, 1], x[2, 2] = np.inf, -np.inf                              # infinite diagonals
+    out.append(x)
+    n = 40
+    x = rng.randn(n, n).astype(np.float32)
+    x[0, 0], x[1, 1], x[2, 2] = np.nan, np.inf, -np.inf
+    x[3, 3], x[3, 5], x[3, 6], x[3, 7] = 0.0, -0.0, 0.0, np.inf     # a +0 diagonal tied with -0 and +0
+    x[4, 4], x[4, 0], x[4, 9] = -0.0, 0.0, np.nan                   # a -0 diagonal
+    x[5, 5], x[5, 1], x[5, 2] = np.inf, np.inf, -np.inf             # +inf tied with +inf on the diagonal
+    x[6, 6], x[6, 3] = -np.inf, -np.inf
+    mask = rng.rand(n, n)
+    x[(mask < 0.05) & ~np.eye(n, dtype=bool)] = np.nan
+    x[(mask > 0.95) & ~np.eye(n, dtype=bool)] = np.inf
+    x[(mask > 0.45) & (mask < 0.5) & ~np.eye(n, dtype=bool)] = -np.inf
+    out.append(x)
+    out.append((rng.randint(0, 4, (33, 33)) / 4).astype(np.float32))              # few levels: many ties
+    z = rng.randint(0, 3, (17, 17))
+    out.append(np.where(z == 0, np.float32(0.0), np.where(z == 1, np.float32(-0.0), np.float32(0.25))).astype(np.float32))
+    return out
+
+
+def specials(ref):
+    gold = {"sims": [], "tuples": [], "ind": []}
+    for x in special_matrices():
+        for m in (x, x.T):
+            with np.errstate(invalid="ignore"):
+                want = ref.compute_metrics(m)
+            got = O.compute_metrics(m)
+            assert all(np.array_equal(a, b) for a, b in zip(want, got)), (want, got)
+            ind = reference_ind(m)
+            assert np.array_equal(ind, O.ranks_from_counts(*O.rank_counts(m)))
+            gold["tuples"].append(tuple(float(v) for v in want))
+            gold["ind"].append(torch.from_numpy(ind.astype(np.int64)))
+        gold["sims"].append(torch.from_numpy(x))
+    print(gold["tuples"])
+    torch.save(gold, os.path.join(HERE, "retrieval_metrics_specials.pt"))
+
+
+def main():
+    ref = reference()
+    specials(ref)
 
     rng = np.random.RandomState(3)
     n, d = 57, 64

@@ -377,3 +377,102 @@ def test_l2norm_fwd_bwd_elementwise(dev, C):
     yd, dyd = yk.double(), dy.double()
     e = 0.5 * ik.double()[:, None] * (yd.abs() * k * (dyd * yd).abs().sum(-1, keepdim=True) + 4 * U * (dyd.abs() + ex.abs()))
     within(REPORT, f"l2norm bwd C{C}: dx", dx.check("l2norm dx"), ex, e + R.ulp_bf16(ex.abs() + e))
+
+
+# ==================================================================================== alignment
+def _refused(fn, *args, **kw):
+    from xpretrain_b200 import _lib
+    ops = _ops()
+    torch.cuda.synchronize()
+    n0 = ops.launch_count()
+    with pytest.raises(_lib.XpError, match="16-byte aligned"):
+        fn(*args, **kw)
+    assert ops.launch_count() == n0, "a refused call launched a kernel"
+
+
+def _at(dev, n, dtype, off, seed):
+    """n random elements starting `off` elements into a fresh allocation (off = 8 bf16 / 4 fp32: 16 bytes in)."""
+    buf = torch.randn(n + off, generator=_gen(seed)).to(dtype).to(dev)
+    return buf[off:]
+
+
+def test_aligned_offset_views_run_and_misaligned_views_are_refused(dev):
+    """Row operands 16 bytes into their allocations, with a row pitch of C + 8, run and match the references; the same
+    operands 2 bytes (one bf16) or 4 bytes (one fp32) off, a row pitch or group stride of C + 4 bf16 (8 bytes off every
+    other row), and gamma / beta one element off are refused before any launch."""
+    ops = _ops()
+    rows, C, ld = 37, 264, 272
+    gamma, beta = 1.0 + 0.3 * _at(dev, C, f32, 4, 1), 0.2 * _at(dev, C, f32, 4, 2)
+    # LayerNorm forward / backward through pitched maps at an element offset of 8
+    xb = _at(dev, rows * ld + 8, bf16, 0, 3)
+    x = xb[8:].view(rows, ld)[:, :C]
+    y = torch.full((rows * ld + 8,), float("nan"), dtype=bf16, device=dev)
+    mean, rstd = torch.empty(rows, device=dev), torch.empty(rows, device=dev)
+    m = ops.rowmap(ld)
+    ops.layernorm_fwd(xb, m, y, m, gamma, beta, mean, rstd, rows, C, EPS, x_off=8, y_off=8)
+    torch.cuda.synchronize()
+    yv = y[8:].view(rows, ld)[:, :C]
+    ex = R.layernorm_ref(x, None, gamma, beta, EPS)
+    per_row("LN offset views", "y", yv, ex["y"], R.layernorm_ref(x, None, gamma, beta, EPS, arm="kernel")["y"])
+    assert bool(torch.isnan(y[8:].view(rows, ld)[:, C:].float()).all()) and bool(torch.isnan(y[:8].float()).all()), \
+        "LN wrote outside its mapped rows"
+    for kw in ({"x_off": 1}, {"y_off": 1}, {"x_off": 8, "y_off": 4}):
+        _refused(ops.layernorm_fwd, xb, m, y, m, gamma, beta, mean, rstd, rows, C, EPS, **{"x_off": 8, "y_off": 8, **kw})
+    for bad in (ops.rowmap(C + 4), ops.rowmap(C, group=4, group_stride=4 * C + 4)):
+        _refused(ops.layernorm_fwd, xb, bad, y, m, gamma, beta, mean, rstd, rows, C, EPS, x_off=8, y_off=8)
+        _refused(ops.layernorm_fwd, xb, m, y, bad, gamma, beta, mean, rstd, rows, C, EPS, x_off=8, y_off=8)
+    g1, b1 = _at(dev, C, f32, 1, 4), _at(dev, C, f32, 1, 5)
+    _refused(ops.layernorm_fwd, xb, m, y, m, g1, beta, mean, rstd, rows, C, EPS, x_off=8, y_off=8)
+    _refused(ops.layernorm_fwd, xb, m, y, m, gamma, b1, mean, rstd, rows, C, EPS, x_off=8, y_off=8)
+    dyb = _at(dev, rows * ld + 8, bf16, 0, 6)
+    dx = torch.full((rows * ld + 8,), float("nan"), dtype=bf16, device=dev)
+    dgam, dbet = torch.zeros(C, device=dev), torch.zeros(C, device=dev)
+    ops.layernorm_bwd(dyb, m, xb, m, gamma, mean, rstd, None, None, dx, m, dgam, dbet, rows, C, dy_off=8, x_off=8, dx_off=8)
+    torch.cuda.synchronize()
+    b = R.layernorm_bwd_ref(dyb[8:].view(rows, ld)[:, :C], x, gamma, mean, rstd)
+    per_row("LN bwd offset views", "dx", dx[8:].view(rows, ld)[:, :C], b["dx"], R.bf(b["dx"]))
+    for kw in ({"dy_off": 1}, {"x_off": 1}, {"dx_off": 1}):
+        _refused(ops.layernorm_bwd, dyb, m, xb, m, gamma, mean, rstd, None, None, dx, m, dgam, dbet, rows, C,
+                 **{"dy_off": 8, "x_off": 8, "dx_off": 8, **kw})
+    _refused(ops.layernorm_bwd, dyb, m, xb, m, gamma, mean, rstd, None, None, dx, ops.rowmap(C + 4), dgam, dbet, rows, C,
+             dy_off=8, x_off=8, dx_off=8)
+    # wide LayerNorm
+    Cw, rw = 2048, 5
+    xw = _at(dev, rw * Cw, bf16, 8, 7).view(rw, Cw)
+    yw = _at(dev, rw * Cw, bf16, 8, 8).view(rw, Cw)
+    mw, sw = torch.empty(rw, device=dev), torch.empty(rw, device=dev)
+    gw, bw = torch.ones(Cw, device=dev), torch.zeros(Cw, device=dev)
+    ops.layernorm_any_fwd(xw, yw, gw, bw, mw, sw, rw, Cw, EPS)
+    torch.cuda.synchronize()
+    exw = R.layernorm_ref(xw, None, gw, bw, EPS)
+    per_row("LN wide offset views", "y", yw, exw["y"], R.layernorm_ref(xw, None, gw, bw, EPS, arm="kernel")["y"])
+    _refused(ops.layernorm_any_fwd, _at(dev, rw * Cw, bf16, 1, 9).view(rw, Cw), yw, gw, bw, mw, sw, rw, Cw, EPS)
+    _refused(ops.layernorm_any_fwd, xw, _at(dev, rw * Cw, bf16, 1, 9).view(rw, Cw), gw, bw, mw, sw, rw, Cw, EPS)
+    # gather / scatter / rowscale / colsum
+    n_src = 40
+    src = _at(dev, n_src * C, bf16, 8, 10).view(n_src, C)
+    index = torch.tensor([3, -1, 0, 39, 17], dtype=torch.int32, device=dev)
+    out = _at(dev, index.numel() * C, bf16, 8, 11).view(-1, C)
+    ops.gather_rows(src, index, out, C)
+    torch.cuda.synchronize()
+    assert same_bits(out, R.gather_rows_ref(src, index)), "gather_rows through offset views is not a bit-exact copy"
+    _refused(ops.gather_rows, _at(dev, n_src * C, bf16, 1, 12).view(n_src, C), index, out, C)
+    _refused(ops.gather_rows, src, index, _at(dev, index.numel() * C, bf16, 1, 13).view(-1, C), C)
+    _refused(ops.scatter_rows, _at(dev, index.numel() * C, bf16, 1, 14).view(-1, C), index, src, C)
+    _refused(ops.scatter_rows, out, index, _at(dev, n_src * C, bf16, 1, 15).view(n_src, C), C)
+    scale = torch.tensor([0.0, 2.0, 1.0 / 0.9] * 13, device=dev)[:rows]
+    xr = _at(dev, rows * C, bf16, 8, 16).view(rows, C)
+    o = _at(dev, rows * C, bf16, 8, 17).view(rows, C)
+    ops.rowscale(xr, scale, o)
+    torch.cuda.synchronize()
+    assert same_bits(o, R.bf(R.f32(R.rowscale_ref(xr, scale))).to(bf16)), "rowscale through offset views differs"
+    _refused(ops.rowscale, _at(dev, rows * C, bf16, 1, 18).view(rows, C), scale, o)
+    _refused(ops.rowscale, xr, scale, _at(dev, rows * C, bf16, 1, 19).view(rows, C))
+    _refused(ops.rowscale, xr, scale, o, residual=_at(dev, rows * C, bf16, 1, 20).view(rows, C))
+    cb = _at(dev, rows * ld, bf16, 0, 21).view(rows, ld)
+    cs = torch.zeros(C, device=dev)
+    ops.colsum(cb[:, 8:8 + C], cs)
+    torch.cuda.synchronize()
+    exc, abc = R.colsum_ref(cb[:, 8:8 + C])
+    within(REPORT, "colsum offset view: out", cs, exc, (rows + 32) * U * abc + 1e-30)
+    _refused(ops.colsum, cb[:, 1:1 + C], cs)

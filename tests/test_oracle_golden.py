@@ -229,6 +229,27 @@ def test_retrieval_metrics_oracle_replays_reference_golden(golden_dir):
     assert int(gold["simple_t2v_equal"].max()) >= 2                       # the fixture really contains ties
 
 
+def test_retrieval_metrics_oracle_replays_reference_on_special_values(golden_dir):
+    """§8(f).3: compute_metrics of the reference on matrices holding NaN, +-inf and +-0 on and off the diagonal, and few
+    distinct levels: the oracle's count-based rank list `ind` and metric tuple equal the reference's sort-based ones.  A
+    NaN or +-inf diagonal drops its query from `ind` (sort(-x) - diag(-x) is never 0 there)."""
+    import numpy as np
+    from oracle import metrics_oracle as MO
+    from xpretrain_b200.utils.metrics import metrics_from_counts
+
+    gold = torch.load(os.path.join(golden_dir, "retrieval_metrics_specials.pt"), weights_only=False)
+    mats = [m for x in gold["sims"] for m in (x.numpy(), x.numpy().T)]           # both directions, as stored
+    assert len(mats) == len(gold["tuples"]) == len(gold["ind"])
+    dropped = 0
+    for x, want, ind in zip(mats, gold["tuples"], gold["ind"]):
+        g, e = MO.rank_counts(x)
+        assert np.array_equal(MO.ranks_from_counts(g, e), ind.numpy())
+        assert tuple(float(v) for v in MO.compute_metrics(x)) == want
+        assert tuple(float(v) for v in metrics_from_counts(g, e)) == want
+        dropped += int((e == 0).sum())
+    assert dropped >= 4, "the fixture must hold NaN and infinite diagonals"
+
+
 # ------------------------------------------------------------------ config #5: LF-VILA Swin-3D video encoder
 @pytest.mark.parametrize("name", ["swin3d_small_b2", "swin3d_padded_b1", "swin3d_train_droppath"])
 def test_swin3d_oracle_replays_reference_golden(golden_dir, name):

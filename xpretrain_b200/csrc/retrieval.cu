@@ -8,7 +8,9 @@
 //   sim_f32_kernel      sim = A B^T in fp32 FFMA (fp32 like numpy's dot — ranks must not depend on a bf16 rounding)
 //   dsl_*               column-wise softmax re-weighting, in place
 //   rank_counts_kernel  for row (or column) i: how many entries are strictly larger than / equal to the diagonal entry;
-//                       the rank list of compute_metrics (including its tie quirk) follows from those two counts.
+//                       the rank list of compute_metrics (including its tie quirk) follows from those two counts.  The
+//                       reference finds the diagonal's positions as zeros of sort(-x) - diag(-x), which is never 0 when
+//                       the diagonal is NaN or +-inf (NaN, or inf - inf): such a query has no equal entries.
 // Integer outputs are exact functions of the similarity matrix they are computed from.
 #include "../../include/xpretrain_b200.h"
 #include "common.h"
@@ -102,7 +104,7 @@ rank_counts_kernel(const float* __restrict__ sim, int N, long long ld, int trans
   }
   if (lane == 0) {
     greater[i] = g;
-    equal[i] = e;
+    equal[i] = isfinite(dg) ? e : 0;   // a NaN / +-inf diagonal leaves the reference's rank list (see above)
   }
 }
 

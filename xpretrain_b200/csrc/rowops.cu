@@ -563,10 +563,31 @@ scatter_rows_kernel(const __nv_bfloat16* __restrict__ in, const int* __restrict_
 
 using namespace xp;
 
+// Alignment refusals for the operands the kernels above move as 16-byte vectors (uint4 / float4 / load8 / store8).
+// Pure argument checks: every entry point runs them before XP_ENTER, so no misaligned operand reaches a launch.
+static bool misaligned(const char* fn, const char* name, const void* p, int& rc) {
+  if (aligned(p, 16)) return false;                      // NULL passes: optional operands
+  rc = fail(std::string(fn) + ": " + name + " must be 16-byte aligned");
+  return true;
+}
+// A row map's explicit offsets are device data (documented in the header); ld and group_stride are checked here.
+static bool misaligned_rows(const char* fn, const char* name, const void* p, const XpRowMap* m, int elsize, int& rc) {
+  if (misaligned(fn, name, p, rc)) return true;
+  if (p == nullptr || m == nullptr || m->offsets != nullptr) return false;   // a map without its operand is never read
+  if ((m->ld * elsize) % 16 == 0 && (m->group <= 0 || (m->group_stride * elsize) % 16 == 0)) return false;
+  rc = fail(std::string(fn) + ": " + name + " rows must be 16-byte aligned (ld and group_stride times the element size "
+            "must be multiples of 16 bytes)");
+  return true;
+}
+static int dtype_bytes(int32_t dtype) { return dtype == XP_DTYPE_F32 ? 4 : 2; }
+
 extern "C" int xp_layernorm_wide_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mean, float* rstd,
                                      int64_t rows, int32_t C, float eps, void* stream) {
-  XP_ENTER(x);
+  const char* fn = "xp_layernorm_wide_fwd";
   if (C % 8 || C > LNW_MAXK * LNW_THREADS * 8) return fail("xp_layernorm_wide_fwd: C must be a multiple of 8 and <= 4096");
+  int rc = 0;
+  if (misaligned(fn, "x", x, rc) || misaligned(fn, "y", y, rc)) return rc;
+  XP_ENTER(x);
   if (rows <= 0) return 0;
   ln_wide_fwd_kernel<<<static_cast<unsigned>(rows), LNW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), gamma, beta, mean, rstd, C, eps);
@@ -576,8 +597,11 @@ extern "C" int xp_layernorm_wide_fwd(const void* x, void* y, const float* gamma,
 
 extern "C" int xp_layernorm_wide_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd,
                                      void* dx, float* dgamma, float* dbeta, int64_t rows, int32_t C, void* stream) {
-  XP_ENTER(dy);
+  const char* fn = "xp_layernorm_wide_bwd";
   if (C % 8 || C > LNW_MAXK * LNW_THREADS * 8) return fail("xp_layernorm_wide_bwd: C must be a multiple of 8 and <= 4096");
+  int rc = 0;
+  if (misaligned(fn, "dy", dy, rc) || misaligned(fn, "x", x, rc) || misaligned(fn, "dx", dx, rc)) return rc;
+  XP_ENTER(dy);
   if (rows <= 0) return 0;
   const long long cap = 2LL * sm_count();
   ln_wide_bwd_kernel<<<static_cast<unsigned>(rows < cap ? rows : cap), LNW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -588,8 +612,10 @@ extern "C" int xp_layernorm_wide_bwd(const void* dy, const void* x, const float*
 }
 
 extern "C" int xp_gather_rows_bf16(const void* src, const int32_t* index, void* out, int64_t n_items, int32_t C, void* stream) {
-  XP_ENTER(src);
   if (C % 8) return fail("xp_gather_rows_bf16: C must be a multiple of 8");
+  int rc = 0;
+  if (misaligned("xp_gather_rows_bf16", "src", src, rc) || misaligned("xp_gather_rows_bf16", "out", out, rc)) return rc;
+  XP_ENTER(src);
   if (n_items <= 0) return 0;
   const long long n = n_items * (C / 8);
   gather_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -599,8 +625,10 @@ extern "C" int xp_gather_rows_bf16(const void* src, const int32_t* index, void* 
 }
 
 extern "C" int xp_scatter_rows_bf16(const void* in, const int32_t* index, void* dst, int64_t n_items, int32_t C, void* stream) {
-  XP_ENTER(in);
   if (C % 8) return fail("xp_scatter_rows_bf16: C must be a multiple of 8");
+  int rc = 0;
+  if (misaligned("xp_scatter_rows_bf16", "in", in, rc) || misaligned("xp_scatter_rows_bf16", "dst", dst, rc)) return rc;
+  XP_ENTER(in);
   if (n_items <= 0) return 0;
   const long long n = n_items * (C / 8);
   scatter_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -611,8 +639,11 @@ extern "C" int xp_scatter_rows_bf16(const void* in, const int32_t* index, void* 
 
 extern "C" int xp_rowscale_bf16(const void* x, const float* scale, const void* residual, void* out, int64_t rows, int32_t C,
                                 void* stream) {
-  XP_ENTER(x);
+  const char* fn = "xp_rowscale_bf16";
   if (C % 8) return fail("xp_rowscale_bf16: C must be a multiple of 8");
+  int rc = 0;
+  if (misaligned(fn, "x", x, rc) || misaligned(fn, "residual", residual, rc) || misaligned(fn, "out", out, rc)) return rc;
+  XP_ENTER(x);
   if (rows <= 0) return 0;
   const long long n = rows * (C / 8);
   rowscale_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -632,7 +663,6 @@ extern "C" int xp_layernorm_add_fwd(const void* x, const XpRowMap* xmap, int32_t
                                     const XpRowMap* addmap, void* sum_out, const XpRowMap* summap, void* y,
                                     const XpRowMap* ymap, int32_t y_dtype, const float* gamma, const float* beta, float* mean,
                                     float* rstd, int64_t rows, int32_t C, float eps, void* stream) {
-  XP_ENTER(x);
   if (C % 8 || C > LN_MAX_VEC * 256) return fail("xp_layernorm_fwd: C must be a multiple of 8 and <= 1024");
   const char* bad_dtype = "xp_layernorm_add_fwd: x / y dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16";
   if ((x_dtype != XP_DTYPE_BF16 && x_dtype != XP_DTYPE_F32 && x_dtype != XP_DTYPE_F16) ||
@@ -640,13 +670,21 @@ extern "C" int xp_layernorm_add_fwd(const void* x, const XpRowMap* xmap, int32_t
     return fail(bad_dtype);
   if (add_bf16 != nullptr && addmap == nullptr) return fail("xp_layernorm_add_fwd: add needs its row map");
   if (sum_out != nullptr && (add_bf16 == nullptr || summap == nullptr)) return fail("xp_layernorm_add_fwd: sum_out needs add and its row map");
+  const char* fn = "xp_layernorm_add_fwd";
+  int rc = 0;
+  if (misaligned_rows(fn, "x", x, xmap, dtype_bytes(x_dtype), rc) || misaligned_rows(fn, "add", add_bf16, addmap, 2, rc) ||
+      misaligned_rows(fn, "sum_out", sum_out, summap, x_dtype == XP_DTYPE_F16 ? 2 : 4, rc) ||
+      misaligned_rows(fn, "y", y, ymap, dtype_bytes(y_dtype), rc) || misaligned(fn, "gamma", gamma, rc) ||
+      misaligned(fn, "beta", beta, rc))
+    return rc;
+  XP_ENTER(x);
   if (rows <= 0) return 0;
   const unsigned grid = static_cast<unsigned>((rows + 3) / 4);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   XpRowMap none = {0, 0, 0, nullptr};
   const RowMapDev xm = to_dev(*xmap), am = to_dev(addmap ? *addmap : none), sm = to_dev(summap ? *summap : none), ym = to_dev(*ymap);
   const __nv_bfloat16* add = static_cast<const __nv_bfloat16*>(add_bf16);
-  int rc = dispatch_dtype(x_dtype, bad_dtype, [&](auto xt) {
+  rc = dispatch_dtype(x_dtype, bad_dtype, [&](auto xt) {
     return dispatch_dtype(y_dtype, bad_dtype, [&](auto yt) {
       return dispatch<0, 1>(add != nullptr, bad_dtype, [&](auto ad) {
         ln_fwd_kernel<decltype(xt), decltype(yt), ad.value><<<grid, 128, 0, st>>>(x, xm, add, am, sum_out, sm, y, ym, gamma,
@@ -664,12 +702,17 @@ extern "C" int xp_layernorm_bwd(const void* dy, const XpRowMap* dymap, const voi
                                 const float* gamma, const float* mean, const float* rstd, const void* dres,
                                 const XpRowMap* drmap, void* dx, const XpRowMap* dxmap, float* dgamma, float* dbeta,
                                 float* dres_colsum, int64_t rows, int32_t C, void* stream) {
-  XP_ENTER(dy);
   const char* bad_dtype = "xp_layernorm_bwd: x dtype must be XP_DTYPE_BF16, XP_DTYPE_F32 or XP_DTYPE_F16";
   const char* bad_c = "xp_layernorm_bwd: C must be a multiple of 8 and <= 1024";
   if (x_dtype != XP_DTYPE_BF16 && x_dtype != XP_DTYPE_F32 && x_dtype != XP_DTYPE_F16) return fail(bad_dtype);
   if (C % 8 || C > LN_MAX_VEC * 256) return fail(bad_c);
   if (dres_colsum != nullptr && dres == nullptr) return fail("xp_layernorm_bwd: dres_colsum needs dres");
+  const char* fn = "xp_layernorm_bwd";        // gamma is staged through shared memory element by element
+  int rc = 0;
+  if (misaligned_rows(fn, "dy", dy, dymap, 2, rc) || misaligned_rows(fn, "x", x, xmap, dtype_bytes(x_dtype), rc) ||
+      misaligned_rows(fn, "dres", dres, drmap, 2, rc) || misaligned_rows(fn, "dx", dx, dxmap, 2, rc))
+    return rc;
+  XP_ENTER(dy);
   if (rows <= 0) return 0;
   long long want = (rows + LNB_WARPS - 1) / LNB_WARPS;
   const int grid = static_cast<int>(want < 4LL * sm_count() ? want : 4LL * sm_count());
@@ -677,7 +720,7 @@ extern "C" int xp_layernorm_bwd(const void* dy, const XpRowMap* dymap, const voi
   const size_t smem = (static_cast<size_t>(LNB_WARPS) * (rsum ? 3 : 2) + 1) * C * sizeof(float);
   XpRowMap none = {0, 0, 0, nullptr};
   const int nv = (C / 8 + 31) / 32;
-  const int rc = dispatch<1, 2, 3, 4>(nv < 1 ? 4 : nv, bad_c, [&](auto nvec) {   // C <= 0: the widest variant, no columns
+  rc = dispatch<1, 2, 3, 4>(nv < 1 ? 4 : nv, bad_c, [&](auto nvec) {   // C <= 0: the widest variant, no columns
     return dispatch<0, 1>(rsum, bad_c, [&](auto rs) {
       return dispatch_dtype(x_dtype, bad_dtype, [&](auto xt) {
         constexpr auto kern = ln_bwd_kernel<nvec.value, rs.value, decltype(xt)>;
@@ -746,8 +789,10 @@ extern "C" int xp_frame_pool_bwd(const float* dfeat, const float* feat, const fl
 
 extern "C" int xp_colsum_bf16(const void* x, int64_t ld, float* out, int64_t rows, int32_t C, float scale,
                               void* stream) {
-  XP_ENTER(x);
   if (C % 8 || ld % 8) return fail("xp_colsum_bf16: C and ld must be multiples of 8");
+  int rc = 0;
+  if (misaligned("xp_colsum_bf16", "x", x, rc)) return rc;
+  XP_ENTER(x);
   if (rows <= 0) return 0;
   const int gx = (C + 255) / 256;
   long long gy = (rows + 63) / 64;

@@ -464,19 +464,46 @@ def tsf_untokenize(tokens, x, B, T, C_, HW):
 
 
 # ------------------------------------------------------------------------------------- retrieval
+def _require(ok: bool, what: str, msg: str) -> None:
+    if not ok:
+        raise _lib.XpError(f"{what}: {msg}")
+
+
+def _rows_f32(t, what: str, name: str) -> None:
+    """t: a 2-D fp32 matrix with unit column stride (its row pitch t.stride(0) goes to the kernel)."""
+    _require(t.dtype == f32 and t.dim() == 2 and t.stride(1) == 1, what,
+             f"{name} must be a 2-D fp32 matrix with unit column stride (got {t.dtype}, strides {tuple(t.stride())})")
+
+
 def sim_f32(a, b, out):
-    """out[Na, Nb] (row pitch out.stride(0)) = a[Na, d] @ b[Nb, d]^T, fp32 FFMA accumulation."""
+    """out[Na, Nb] (row pitch out.stride(0)) = a[Na, d] @ b[Nb, d]^T, fp32 FFMA accumulation.  a and b are read with
+    row pitch d, so they must be contiguous."""
+    for name, t in (("a", a), ("b", b), ("out", out)):
+        _rows_f32(t, "sim_f32", name)
+    _require(a.is_contiguous() and b.is_contiguous(), "sim_f32", "a and b must be contiguous")
+    _require(a.shape[1] == b.shape[1], "sim_f32", f"a and b widths differ ({a.shape[1]} vs {b.shape[1]})")
+    _require(tuple(out.shape) == (a.shape[0], b.shape[0]), "sim_f32",
+             f"out must be [{a.shape[0]}, {b.shape[0]}] (got {list(out.shape)})")
     _call("xp_sim_f32", _p(a), _p(b), _p(out), a.shape[0], b.shape[0], a.shape[1], out.stride(0))
 
 
 def dsl_reweight(sim, theta: float, scratch):
-    """sim *= softmax(theta * sim, axis=0) in place; scratch: 2 * cols fp32."""
+    """sim *= softmax(theta * sim, axis=0) in place; scratch: at least 2 * cols fp32."""
+    _rows_f32(sim, "dsl_reweight", "sim")
+    _require(scratch.dtype == f32 and scratch.is_contiguous() and scratch.numel() >= 2 * sim.shape[1], "dsl_reweight",
+             f"scratch must be contiguous fp32 of at least 2 * cols = {2 * sim.shape[1]} elements")
     _call("xp_dsl_reweight", _p(sim), sim.shape[0], sim.shape[1], sim.stride(0), float(theta), _p(scratch))
 
 
 def rank_counts(sim, transpose: bool, greater, equal):
     """greater[i] / equal[i] = entries of row (column) i of the square sim larger than / equal to sim[i, i]."""
-    _call("xp_rank_counts", _p(sim), sim.shape[0], sim.stride(0), 1 if transpose else 0, _p(greater), _p(equal))
+    _rows_f32(sim, "rank_counts", "sim")
+    n = sim.shape[0]
+    _require(sim.shape[1] == n, "rank_counts", f"sim must be square (got {list(sim.shape)})")
+    for name, t in (("greater", greater), ("equal", equal)):
+        _require(t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n, "rank_counts",
+                 f"{name} must be contiguous int32 of {n} elements")
+    _call("xp_rank_counts", _p(sim), n, sim.stride(0), 1 if transpose else 0, _p(greater), _p(equal))
 
 
 # ------------------------------------------------------------------------------------- optimizer

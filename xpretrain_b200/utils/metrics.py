@@ -58,7 +58,9 @@ def compute_metrics(x: torch.Tensor, transpose: bool = False):
 
 def metrics_from_counts(g: np.ndarray, e: np.ndarray):
     """The O(N) host part of compute_metrics: the reference's rank list `ind` (metrics.py:42-47) is, per query,
-    g_i, g_i + 1, .., g_i + e_i - 1 (one entry per value tied with the diagonal), then recall@1/5/10, median and mean rank."""
+    g_i, g_i + 1, .., g_i + e_i - 1 (one entry per value tied with the diagonal), then recall@1/5/10, median and mean rank.
+    A query whose diagonal is NaN or +-inf has e_i = 0 and drops out of `ind`, as in the reference (its sort(-x) -
+    diag(-x) is never 0 there)."""
     g, e = np.asarray(g, dtype=np.int64), np.asarray(e, dtype=np.int64)
     ind = np.repeat(g, e) + (np.arange(int(e.sum())) - np.repeat(np.cumsum(e) - e, e))
     r1 = float(np.sum(ind == 0)) / len(ind)
