@@ -153,6 +153,17 @@ int xp_vip_patchify(const void* video, int32_t dtype, void* patches_bf16, int64_
  * patch matrix as xp_vip_patchify does.  Alignment: patches_bf16 16 bytes; for p % 8 == 0 also frames_hwc 8 bytes. */
 int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W, int32_t patch,
                        const float* mean3, const float* std3, void* stream);
+/* xp_vip_patchify_u8 for frames of any size 1 <= H, W <= 4096: the reference's Resize([S, S], BICUBIC) + CenterCrop(S)
+ * (init_transform_dict_simple, CLIP-ViP/src/datasets/dataloader.py:209-233) fused in as well.  The pinned torchvision 0.9.0
+ * runs it as F.interpolate(x / 255, size=(S, S), mode="bicubic", align_corners=False): A = -0.75, border-clamped taps, no
+ * antialias, no clamp of the result.  The source coordinate scale * (d + 0.5) - 0.5, scale = in / out, is torch's fp32
+ * value bit for bit (one rounding: a fused multiply-add); the cubic weights are float64 of its t rounded to fp32; taps are accumulated in fp32 in a fixed order
+ * (bitwise repeatable), then Normalize, one rounding to bf16.  At H = W = S the bits equal xp_vip_patchify_u8's.  Writes
+ * the frames*(S/p)^2 x round_up(3p^2, 8) patch matrix of xp_vip_patchify (pad columns zero) and nothing else.  mean3 /
+ * std3 are HOST arrays of 3 floats.  Refused before any launch: H, W or S outside [1, 4096], S % patch != 0, a
+ * patches_bf16 not 16-byte aligned.  frames_hwc may have any alignment. */
+int xp_vip_resize_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W, int32_t S,
+                              int32_t patch, const float* mean3, const float* std3, void* stream);
 /* CLIP_ViP.py:170-176,183-195: table[t*L+l] = interp(temporal_embedding)[t] + position_embedding[1+l] (bf16,
  * [T*L, C]) and the M = 1 + add_cls_num global rows x[b, m] = (class_embedding | added_cls[m-1]) + position_embedding[0]
  * written into x_bf16 [B, M+T*L, C].  temporal may be NULL (if_use_temporal_embed = 0); added is read only when M > 1.

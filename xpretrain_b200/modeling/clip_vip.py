@@ -576,6 +576,29 @@ def _encoder_bwd(model: CLIPModel, tower: str, pool_ln: str, proj: str, pk: _Wei
 
 
 # ------------------------------------------------------------------------------ vision tower
+def frame_input_path(dtype: torch.dtype, H: int, W: int, image_size: int) -> str:
+    """Which patch extraction takes frames of `dtype` and size H x W into a tower of `image_size`: "patchify_u8" (uint8 at
+    the input resolution: /255 + Normalize fused in), "resize_u8" (uint8 of another size: the reference's bicubic Resize
+    fused in as well) or "patchify" (float frames, already transformed).  Float frames of another size raise ValueError:
+    the reference transform is the caller's there, and the patch matrix is sized for image_size."""
+    if dtype == torch.uint8:
+        return "patchify_u8" if (H, W) == (image_size, image_size) else "resize_u8"
+    if (H, W) != (image_size, image_size):
+        raise ValueError(f"{dtype} frames must be {image_size} x {image_size} (got {H} x {W}); uint8 decoder frames of any "
+                         f"size are resized on the GPU")
+    return "patchify"
+
+
+def _frame_path(cfg: ClipVipConfig, video: torch.Tensor) -> str:
+    """The layout checks of the vision input, then frame_input_path; raises ValueError before anything is launched."""
+    if cfg.per_frame and video.dim() not in (4, 5):
+        raise ValueError("the per-frame model takes images [N, 3, H, W] or video [B, T, 3, H, W] (uint8: channels-last)")
+    u8 = video.dtype == torch.uint8
+    if u8 and ((video.dim() != 5 and not cfg.per_frame) or video.shape[-1] != 3):
+        raise ValueError("uint8 video must be channels-last [B, T, H, W, 3] (decoder layout)")
+    return frame_input_path(video.dtype, video.shape[-3 if u8 else -2], video.shape[-2 if u8 else -1], cfg.image_size)
+
+
 def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = False):
     """ckpt (with save): keep each block's input only (gradient checkpointing); the backward rebuilds the rest per block.
     The per-frame model folds the frames into the batch (CLIP.py sees [B*T, 3, H, W]): B*T sequences of one frame and one
@@ -583,14 +606,11 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     cfg = model.config
     vm = model.vision_model
     emb = vm.embeddings
+    path = _frame_path(cfg, video)
     if cfg.per_frame:
-        if video.dim() not in (4, 5):
-            raise ValueError("the per-frame model takes images [N, 3, H, W] or video [B, T, 3, H, W] (uint8: channels-last)")
         B, T = video.numel() // (video.shape[-3] * video.shape[-2] * video.shape[-1]), 1
     else:
         B, T = video.shape[0], video.shape[1]
-    if video.dtype == torch.uint8 and ((video.dim() != 5 and not cfg.per_frame) or video.shape[-1] != 3):
-        raise ValueError("uint8 video must be channels-last [B, T, H, W, 3] (decoder layout)")
     C_, L, M = cfg.vision.hidden_size, cfg.num_patches, cfg.num_global_tokens
     H = cfg.vision.num_attention_heads
     S = M + T * L
@@ -602,9 +622,11 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     ldp = ops.patch_pitch(cfg.patch_size)    # patch-matrix row pitch: Kp rounded up to 8 columns, pad columns zero
 
     patches = torch.empty(B * T * L, ldp, dtype=bf16, device=dev)
-    if video.dtype == torch.uint8:      # raw decoder frames: the reference's /255 + Normalize is fused into the patch extraction
-        ops.vip_patchify_u8(video.contiguous(), patches, cfg.patch_size, getattr(model, "pixel_mean", ops.CLIP_MEAN),
-                            getattr(model, "pixel_std", ops.CLIP_STD))
+    mean, std = getattr(model, "pixel_mean", ops.CLIP_MEAN), getattr(model, "pixel_std", ops.CLIP_STD)
+    if path == "patchify_u8":      # raw decoder frames: the reference's /255 + Normalize is fused into the patch extraction
+        ops.vip_patchify_u8(video.contiguous(), patches, cfg.patch_size, mean, std)
+    elif path == "resize_u8":      # ... and its bicubic Resize to image_size as well
+        ops.vip_resize_patchify_u8(video.contiguous(), patches, cfg.image_size, cfg.patch_size, mean, std)
     else:
         ops.vip_patchify(video.contiguous(), patches, cfg.patch_size)
     table = torch.empty(T * L, C_, dtype=bf16, device=dev)
@@ -908,6 +930,8 @@ def _overlap_stream(model: CLIPModel, dev, option: str):
 def _run(model: CLIPModel, video, input_ids, attention_mask, normalize: bool = True):
     if not model.logit_scale.is_cuda:
         raise _lib.XpError("xpretrain_b200.CLIPModel must live on a CUDA (H100) device: there is no CPU path")
+    if video is not None:
+        _frame_path(model.config, video)
     params = [p for n, p in model.named_parameters() if n != "logit_scale"]
     vis, txt = _ClipVipFunction.apply(model, video, input_ids, attention_mask, normalize, torch.is_grad_enabled(), *params)
     return (vis if video is not None else None), (txt if input_ids is not None else None)

@@ -252,6 +252,19 @@ def vip_patchify_u8(frames_hwc: torch.Tensor, patches: torch.Tensor, patch: int,
     _call("xp_vip_patchify_u8", _p(frames_hwc), _p(patches), n, H, W, patch, m3, s3)
 
 
+def vip_resize_patchify_u8(frames_hwc: torch.Tensor, patches: torch.Tensor, size: int, patch: int, mean=CLIP_MEAN,
+                           std=CLIP_STD):
+    """frames_hwc uint8 [..., H, W, 3] of any size -> the bf16 patch matrix of vip_patchify_u8 at size x size: the
+    reference's bicubic Resize([size, size]) + CenterCrop + /255 + Normalize fused into the patch extraction."""
+    assert frames_hwc.dtype == torch.uint8 and frames_hwc.dim() >= 3 and frames_hwc.shape[-1] == 3
+    _aligned_output(patches, 16, "vip_resize_patchify_u8")
+    frames_hwc = aligned_input(frames_hwc)
+    H, W = frames_hwc.shape[-3], frames_hwc.shape[-2]
+    n = frames_hwc.numel() // (3 * H * W) if H * W else 0
+    m3, s3 = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+    _call("xp_vip_resize_patchify_u8", _p(frames_hwc), _p(patches), n, H, W, size, patch, m3, s3)
+
+
 def vip_embed_tables(pos, temporal, cls, added, table, x, B, T, L, M, C_, temporal_size):
     _call("xp_vip_embed_tables", _p(pos), _p(temporal), _p(cls), _p(added), _p(table), _p(x), B, T, L, M, C_, temporal_size)
 
