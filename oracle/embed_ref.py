@@ -142,13 +142,16 @@ def _atomic_bound(n: torch.Tensor, abs_sum: torch.Tensor) -> torch.Tensor:
     return (n - 1).clamp_min(0).to(F64) * U * abs_sum * SLACK
 
 
-def vip_bwd_ref(d_patch, d_global, init, B: int, T: int, L: int, M: int, temporal_size: int):
+def vip_bwd_ref(d_patch, d_global, init, B: int, T: int, L: int, M: int, temporal_size: int, counts=None):
     """xp_vip_embed_bwd on top of existing gradients init = dict(pos, temporal, cls, added) (fp32; temporal / added may be
     None).  Returns {name: (exact f64, bound f64)}.  Addends per element: the existing value, B*(rows that map to it) bf16
-    values; d_temporal also rounds one weight product per frame and carries the weight error of weight_error()."""
+    values; d_temporal also rounds one weight product per frame and carries the weight error of weight_error().
+    counts [B]: sample b stands for counts[b] identical samples (a periodic batch; B is then the period)."""
     C = d_patch.shape[-1]
-    dp = d_patch.to(F64).reshape(B, T, L, C)
-    dg = d_global.to(F64).reshape(B, M, C)
+    w = torch.ones(B, dtype=F64, device=d_patch.device) if counts is None else counts.to(F64).to(d_patch.device)
+    dp = d_patch.to(F64).reshape(B, T, L, C) * w[:, None, None, None]
+    dg = d_global.to(F64).reshape(B, M, C) * w[:, None, None]
+    B = float(w.sum())
     out = {}
     p0 = init["pos"].to(F64)
     pos = p0.clone()

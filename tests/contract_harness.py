@@ -10,6 +10,11 @@
   reordering   two runs of the same model on the same inputs that may differ only in the order of fp32 atomic additions
                (split-K weight gradients, column sums): outputs with the same bits, every gradient within GRAD_REL x
                its scale (reordering_violations)
+  periodic     operands past 2^31 bytes or elements: rows (or samples) repeat a small base block (`periodic`, the period
+               checked against wrapped offsets by `no_aliasing`), every output row must have the bits of its representative
+               in a small run (`same_as_representatives`), and Big outputs are scanned for coverage and guards chunk by
+               chunk, with no full-size mask, clone or cast; a reduction over such an operand has no row to compare, so
+               `has_power` asserts that the value a planted defect would give falls outside its bound
 """
 import contextlib
 
@@ -222,6 +227,126 @@ def calibrated_model_rows(tag, rows, slices=None):
           + (f", worst slice {worst_sl[0]:.3f} ({worst_sl[1]})" if slices else "")
           + (f"; worst err / autocast err {worst_ac[0]:.2f} ({worst_ac[1]})" if worst_ac[1] else ""))
     return bad, worst, worst_sl
+
+
+# ------------------------------------------------------------------------------ periodic operands past 2^31
+CHUNK = 1 << 26         # elements per step of the scans over multi-GB outputs
+WRAP = 1 << 31          # a 32-bit offset wraps (or turns negative) at a multiple of 2^31 bytes or elements
+
+
+def periodic(base, rows, out=None, weights=None):
+    """[rows, ...] with row r = base[r % P] (P = base.shape[0]), written by broadcast copies: nothing of the full size is
+    built besides the result.  `out` (contiguous, [rows, ...]) receives it in place when given.  weights [ceil(rows / P)]
+    (powers of two, so exact): period j is scaled by weights[j] in place."""
+    P = base.shape[0]
+    if out is None:
+        out = torch.empty((rows,) + tuple(base.shape[1:]), dtype=base.dtype, device=base.device)
+    full = rows // P
+    w = None if weights is None else weights.to(base.dtype).to(base.device)
+    if full:
+        body = out[:full * P].view((full,) + tuple(base.shape))
+        body.copy_(base)
+        if w is not None:
+            body.mul_(w[:full].view((full,) + (1,) * base.dim()))
+    if rows > full * P:
+        out[full * P:rows].copy_(base[:rows - full * P])
+        if w is not None:
+            out[full * P:rows].mul_(w[full])
+    return out
+
+
+def no_aliasing(name, period_rows, row_elems, elsize, nbytes):
+    """The displacement rule: in a buffer of `nbytes` whose rows of `row_elems` elements (`elsize` bytes each) repeat every
+    `period_rows` rows, a move by a multiple of 2^31 bytes (and so of 2^32) must never land on an element of the same
+    residue and column, i.e. must not be a multiple of one period.  Otherwise an offset that wrapped would read or write
+    the very value a correct one does, and no comparison could see it."""
+    period = period_rows * row_elems * elsize
+    for k in range(1, nbytes // WRAP + 1):
+        assert (k * WRAP) % period != 0, (f"{name}: a period of {period_rows} rows x {row_elems} elements ({period} bytes) "
+                                          f"divides {k} x 2^31 bytes: a wrapped offset would alias onto its own residue")
+
+
+def crossing(report, case, name, t, claim):
+    """Assert that tensor t (the logical operand) reaches past `claim`, one of '2^31 bytes', '2^32 bytes', '2^31 elements',
+    at its largest byte or element offset; records the largest offset / the boundary."""
+    last = t.numel() - 1
+    off, bound = {"2^31 bytes": (last * t.element_size(), 1 << 31), "2^32 bytes": (last * t.element_size(), 1 << 32),
+                  "2^31 elements": (last, 1 << 31)}[claim]
+    report.record(f"{case}: {name} past {claim} (largest offset / boundary)", off / bound)
+    assert off >= bound, f"{case}: {name} reaches offset {off}, short of {claim}: the case no longer tests what it claims"
+
+
+def same_as_representatives(what, big, rep, chunk=CHUNK):
+    """Every row r of big ([rows, ...]) has the bits of rep[r % P] (rep [P, ...]), compared over whole periods at about
+    `chunk` elements a step.  The message names the first differing row, its residue and its first differing column."""
+    P = rep.shape[0]
+    rb = bits(rep).reshape(P, -1)
+    per = rb.shape[1]
+    step = max(1, chunk // (P * per)) * P
+    rows = big.shape[0]
+    for r0 in range(0, rows, step):
+        n = min(step, rows - r0)
+        g = bits(big[r0:r0 + n]).reshape(n, per)
+        full = n // P
+        diff = torch.empty(n, dtype=torch.bool, device=g.device)
+        if full:
+            diff[:full * P] = (g[:full * P].view(full, P, per) != rb).any(-1).view(-1)
+        if n > full * P:
+            diff[full * P:] = (g[full * P:] != rb[:n - full * P]).any(-1)
+        if bool(diff.any()):
+            r = int(diff.nonzero()[0])
+            c = int((g[r] != rb[(r0 + r) % P]).nonzero()[0])
+            raise AssertionError(f"{what}: {int(diff.sum())} rows of [{r0}, {r0 + n}) differ from their representatives, "
+                                 f"the first row {r0 + r} (residue {(r0 + r) % P}) at flat column {c}")
+
+
+def has_power(report, key, exact, planted, bound):
+    """The self-check of a reduction over a periodic operand: the value a planted defect gives (rows past a boundary
+    dropped, or read from the wrong place) must fall outside the bound at every element, or the check could not see that
+    defect.  Records the largest bound / |planted - exact|, which is below 1 when the check has power everywhere."""
+    gap = (planted.double() - exact.double()).abs()
+    ratio = bound.double() / gap
+    worst = float(ratio.max())
+    report.record(f"{key}: self-check, largest bound / |planted - exact|", worst)
+    assert worst < 1.0, (f"{key}: the planted defect stays inside the bound at {int((ratio >= 1).sum())} of {ratio.numel()} "
+                         f"elements (worst bound / gap {worst:.3g}): this check cannot see it")
+
+
+class Big:
+    """A multi-GB output of `shape` inside one allocation with PAD bytes of guard pattern before and after it.  Its elements
+    start unwritten (NaN, or the pattern for integer dtypes); `check` scans it in chunks of about CHUNK elements for
+    unwritten or non-finite elements and checks the guards against the pattern, without a full-size mask, clone or cast."""
+
+    def __init__(self, dev, shape, dtype, chunk=CHUNK):
+        n = 1
+        for s in shape:
+            n *= s
+        self.pre, self.n, self.chunk = PAD // torch.empty(0, dtype=dtype).element_size(), n, chunk
+        self.buf = torch.empty(n + 2 * self.pre, dtype=dtype, device=dev)
+        iv = self.buf.view(DTYPES[dtype][0])
+        iv[:self.pre].fill_(DTYPES[dtype][1])
+        iv[self.pre + n:].fill_(DTYPES[dtype][1])
+        self.t = self.buf[self.pre:self.pre + n].view(shape)
+        _start(self.t)
+
+    def guards(self, what):
+        iv, pat = self.buf.view(DTYPES[self.buf.dtype][0]), DTYPES[self.buf.dtype][1]
+        for side, g in (("before", iv[:self.pre]), ("after", iv[self.pre + self.n:])):
+            moved = int((g != pat).sum())
+            assert moved == 0, f"{what}: {moved} guard elements {side} the output overwritten"
+
+    def check(self, what):
+        """Guards intact and every element written and finite; returns the output."""
+        self.guards(what)
+        pat = DTYPES[self.buf.dtype][1]
+        flat = self.buf[self.pre:self.pre + self.n]
+        for i in range(0, self.n, self.chunk):
+            c = flat[i:i + self.chunk]
+            bad = ~torch.isfinite(c) if c.dtype.is_floating_point else c == pat
+            if bool(bad.any()):
+                raise AssertionError(f"{what}: {int(bad.sum())} elements of [{i}, {i + c.numel()}) not written or not "
+                                     f"finite, the first at flat index {i + int(bad.nonzero()[0])}")
+        return self.t
 
 
 GRAD_REL = 1e-5         # max |g - g_ref| <= GRAD_REL x scale: split-K atomics reorder (about 1e-7 between runs)

@@ -165,3 +165,120 @@ def test_reordering_rule_wants_the_same_output_bits_and_the_same_gradients():
     nang[w][0, 0] = float("nan")
     assert any(w in b for b in reordering_violations(out, out, ref, nang)[0])
     assert reordering_violations(out, out, ref, {k: v for k, v in ref.items() if k != w})[0]
+
+
+# ------------------------------------------------------------------ periodic operands past 2^31 (small, tiny chunks)
+from contract_harness import WRAP, Big, crossing, no_aliasing, periodic, same_as_representatives  # noqa: E402
+
+
+def _periodic_case(rows=999, P=7, W=24, dtype=torch.bfloat16):
+    base = torch.randn(P, W, generator=torch.Generator().manual_seed(P)).to(dtype)
+    return base, periodic(base, rows)
+
+
+def test_periodic_builder_repeats_the_base_with_a_partial_tail_and_fills_in_place():
+    base, big = _periodic_case()
+    want = base.repeat(999 // 7 + 1, 1)[:999]
+    assert same_bits(big, want)
+    out = torch.full((999, 24), float("nan"), dtype=torch.bfloat16)
+    assert periodic(base, 999, out=out) is out and same_bits(out, want)
+    assert same_bits(periodic(base, 5), base[:5])            # fewer rows than one period
+
+
+def test_displacement_rule_refuses_a_period_that_divides_2e31_bytes():
+    no_aliasing("GEMM 41 x 128 rows", 41 * 128, 3072, 2, 803_328 * 3072 * 2)      # 2^17 x 123 bytes: never divides
+    no_aliasing("below 2^31: nothing to wrap", 128, 1024, 2, WRAP - 1)
+    with pytest.raises(AssertionError, match="divides 1 x 2"):
+        no_aliasing("128 rows x 1024", 128, 1024, 2, WRAP + 1)                     # 2^18 bytes divides 2^31
+    with pytest.raises(AssertionError, match="divides 2 x 2"):
+        no_aliasing("2^32 bytes", 1, 1 << 30, 4, 2 * WRAP)                         # divides 2^32, not 2^31
+
+
+def test_big_coverage_scan_finds_a_nan_in_the_last_chunk_and_both_guards():
+    b = Big("cpu", (10, 7), torch.bfloat16, chunk=16)                              # 70 elements: the last chunk holds 6
+    b.t.fill_(1.0)
+    assert b.check("all written") is b.t
+    b.t.view(-1)[-1] = float("nan")
+    with pytest.raises(AssertionError, match=r"\[64, 70\).*flat index 69"):
+        b.check("last")
+    b.t.fill_(float("inf"))
+    with pytest.raises(AssertionError, match="not finite"):
+        b.check("inf")
+    b.t.fill_(1.0)
+    b.buf.view(torch.int16)[b.pre - 1] = 0
+    with pytest.raises(AssertionError, match="before"):
+        b.check("guard before")
+    b.buf.view(torch.int16)[b.pre - 1] = DTYPES[torch.bfloat16][1]
+    b.buf.view(torch.int16)[b.pre + b.n] = 0
+    with pytest.raises(AssertionError, match="after"):
+        b.check("guard after")
+
+
+def test_big_starts_unwritten_for_an_integer_dtype():
+    b = Big("cpu", (5,), torch.int32, chunk=2)
+    with pytest.raises(AssertionError, match="not written"):
+        b.check("int32")
+    b.t.fill_(3)
+    b.check("int32")
+
+
+def test_representatives_catch_a_block_moved_by_a_multiple_of_2e31_bytes_modulo_the_buffer():
+    """The block of rows a wrapped offset would write: the data of the position k x 2^31 bytes further on, taken modulo the
+    buffer's size.  The period keeps that move off the element's own residue and column, so the block differs."""
+    base, big = _periodic_case()
+    same_as_representatives("clean", big, base, chunk=100)
+    flat = big.view(-1)
+    n = flat.numel()
+    for k in (1, 2, 3):
+        d = (k * WRAP // 2) % n                                                  # elements (bf16)
+        assert d % (7 * 24) != 0
+        bad = big.clone()
+        rows = torch.arange(400 * 24, 410 * 24)
+        bad.view(-1)[rows] = flat[(rows + d) % n]
+        with pytest.raises(AssertionError, match=r"row 40\d \(residue"):
+            same_as_representatives(f"moved by {k} x 2^31 bytes", bad, base, chunk=100)
+
+
+def test_representatives_catch_a_sample_that_read_its_neighbour():
+    B, P, S, W = 8, 3, 5, 16
+    base = torch.randn(P, S * W, generator=torch.Generator().manual_seed(1))
+    big = periodic(base, B)
+    same_as_representatives("clean", big, base, chunk=64)
+    big[4] = big[5]
+    with pytest.raises(AssertionError, match="first row 4 \\(residue 1\\)"):
+        same_as_representatives("neighbour", big, base, chunk=64)
+    big = periodic(base, B)
+    big[7, 3] = -big[7, 3]                                                       # the partial last period
+    with pytest.raises(AssertionError, match="row 7 .*column 3"):
+        same_as_representatives("tail", big, base, chunk=64)
+
+
+def test_crossing_claims_are_checked_on_the_operands_extent():
+    report = Report("test")
+    huge = torch.zeros(1, dtype=torch.bfloat16).expand((1 << 31) + 1)            # no memory behind it
+    crossing(report, "case", "x", huge, "2^31 elements")
+    crossing(report, "case", "x", huge, "2^32 bytes")
+    assert report.worst["case: x past 2^31 elements (largest offset / boundary)"] == 1.0
+    with pytest.raises(AssertionError, match="short of 2\\^31 elements"):
+        crossing(report, "case", "y", huge[:1 << 31], "2^31 elements")
+    with pytest.raises(AssertionError, match="short of 2\\^31 bytes"):
+        crossing(report, "case", "z", huge[:1 << 30], "2^31 bytes")
+
+
+def test_periodic_builder_scales_each_period_by_its_weight():
+    from oracle.gemm_ref import block_weights
+    base, _ = _periodic_case()
+    w = block_weights((999 + 6) // 7)
+    big = periodic(base, 999, weights=w)
+    want = torch.stack([base[r % 7] * w[r // 7].to(torch.bfloat16) for r in range(999)])
+    assert same_bits(big, want)
+
+
+def test_has_power_fails_when_a_planted_defect_stays_inside_the_bound():
+    from contract_harness import has_power
+    report = Report("test")
+    exact = torch.tensor([10.0, -10.0], dtype=F64)
+    has_power(report, "k", exact, exact * 0.9, torch.tensor([0.5, 0.5], dtype=F64))
+    assert report.worst["k: self-check, largest bound / |planted - exact|"] == pytest.approx(0.5)
+    with pytest.raises(AssertionError, match="1 of 2 elements"):
+        has_power(report, "weak", exact, torch.tensor([9.0, -9.9], dtype=F64), torch.tensor([0.5, 0.5], dtype=F64))

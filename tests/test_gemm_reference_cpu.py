@@ -140,3 +140,94 @@ def test_small_row_references():
     assert torch.equal(sc[5], x[5]) and torch.equal(sc[1], torch.zeros(24, dtype=F64))
     s = torch.tensor([0.0, 2.0, 1.0, 0.5, 3.0, 1.0], dtype=F64)
     _close(R.rowscale_ref(x, s, x), x + s[:, None] * x)
+
+
+# ---------------------------------------------------------- count-weighted references of periodic operands
+def _repeated(base, rows):
+    P = base.shape[0]
+    return base.repeat((rows + P - 1) // P, *([1] * (base.dim() - 1)))[:rows]
+
+
+def test_repeat_counts():
+    c = R.repeat_counts(1000, 7)
+    assert torch.equal(c, torch.bincount(torch.arange(1000) % 7).double())
+
+
+def test_counted_gemm_equals_the_repeated_reduction_and_its_bound():
+    g = torch.Generator().manual_seed(3)
+    P, rows, n_out, n_in = 7, 100, 16, 24
+    dyb = torch.randn(P, n_out, generator=g).to(torch.bfloat16)
+    xb = torch.randn(P, n_in, generator=g).to(torch.bfloat16)
+    c0 = torch.randn(n_out, n_in, generator=g)
+    got = R.gemm_ref_counted(dyb.T, xb.T, R.repeat_counts(rows, P), out_mode=R.OUT_F32_ATOMIC, c0=c0)
+    want = R.gemm_ref(_repeated(dyb, rows).T, _repeated(xb, rows).T, out_mode=R.OUT_F32_ATOMIC, c0=c0)
+    for k in ("exact", "pre", "absprod"):
+        _close(got[k], want[k])
+    bg = R.gemm_element_bound(got, 64, 2, c0=c0, out_mode=R.OUT_F32_ATOMIC)
+    bw = R.gemm_element_bound(want, 64, 2, c0=c0, out_mode=R.OUT_F32_ATOMIC)
+    _close(bg, bw)
+
+
+def test_counted_layernorm_bwd_and_colsum_equal_the_repeated_sums():
+    g = torch.Generator().manual_seed(4)
+    P, rows, C = 5, 37, 24
+    x, dy, dres = (torch.randn(P, C, generator=g) for _ in range(3))
+    gamma = torch.randn(C, generator=g)
+    st = R.layernorm_ref(x, None, gamma, gamma, 1e-5)
+    got = R.layernorm_bwd_ref(dy, x, gamma, st["mean"], st["rstd"], dres, counts=R.repeat_counts(rows, P))
+    rep = [_repeated(t, rows) for t in (dy, x, st["mean"], st["rstd"], dres)]
+    want = R.layernorm_bwd_ref(rep[0], rep[1], gamma, rep[2], rep[3], rep[4])
+    for k in ("dgamma", "dbeta", "dres_colsum", "abs_dgamma", "abs_dbeta", "abs_dres_colsum"):
+        _close(got[k], want[k])
+    _close(got["dx"], want["dx"][:P])                      # dx stays per row
+    for a, b in zip(R.colsum_ref(dy, -0.5, counts=R.repeat_counts(rows, P)), R.colsum_ref(_repeated(dy, rows), -0.5)):
+        _close(a, b)
+
+
+def test_counted_embedding_bwd_equals_the_repeated_batch():
+    from oracle import embed_ref as E
+    g = torch.Generator().manual_seed(5)
+    P, B, T, L, M, C, Tsz = 3, 8, 4, 5, 4, 16, 3
+    dp = torch.randn(P * T * L, C, generator=g).to(torch.bfloat16)
+    dg = torch.randn(P * M, C, generator=g).to(torch.bfloat16)
+    init = {"pos": torch.randn(1 + L, C, generator=g), "temporal": torch.randn(Tsz, C, generator=g),
+            "cls": torch.randn(C, generator=g), "added": torch.randn(M - 1, C, generator=g)}
+    got = E.vip_bwd_ref(dp, dg, init, P, T, L, M, Tsz, counts=R.repeat_counts(B, P))
+    want = E.vip_bwd_ref(_repeated(dp.view(P, -1), B).reshape(-1, C), _repeated(dg.view(P, -1), B).reshape(-1, C), init,
+                         B, T, L, M, Tsz)
+    assert set(got) == set(want)
+    for k in got:
+        _close(got[k][0], want[k][0])
+        _close(got[k][1], want[k][1])
+
+
+def test_block_weights_grow_along_the_rows_in_powers_of_two():
+    w = R.block_weights(10)
+    assert torch.equal(w, torch.tensor([1.0, 1, 1, 2, 2, 4, 4, 4, 8, 8], dtype=F64))
+
+
+def test_weighted_counts_over_a_row_range_equal_the_explicit_rows():
+    P, rows = 7, 100
+    w = R.block_weights((rows + P - 1) // P)
+    row_w = w[torch.arange(rows) // P]
+    for start, stop in ((0, rows), (0, 37), (20, 93)):
+        want = torch.zeros(P, dtype=F64).index_add_(0, torch.arange(start, stop) % P, row_w[start:stop])
+        assert torch.equal(R.repeat_counts(stop, P, weights=w, start=start), want)
+
+
+def test_wrapped_column_sums_equal_dropped_and_displaced_reads_of_the_explicit_operand():
+    """Against the flat [rows x W] operand built row by row: elements at flat offset >= wrap set to zero (never read) or
+    taken from wrap elements earlier, for a wrap inside a row and one on a row boundary."""
+    g = torch.Generator().manual_seed(6)
+    P, W, rows = 7, 24, 101
+    xb = torch.randn(P, W, generator=g, dtype=F64)
+    w = R.block_weights((rows + P - 1) // P)
+    flat = torch.stack([xb[r % P] * w[r // P] for r in range(rows)]).reshape(-1)
+    for wrap in (1000, 48 * W):
+        dropped, displaced = R.wrapped_column_sums(xb, rows, w, wrap)
+        d = flat.clone()
+        d[wrap:] = 0
+        _close(dropped, d.view(rows, W).sum(0))
+        d[wrap:] = flat[:flat.numel() - wrap]
+        _close(displaced, d.view(rows, W).sum(0))
+    _close(R.repeat_counts(rows, P, weights=w) @ xb, flat.view(rows, W).sum(0))
