@@ -21,6 +21,8 @@ $(OBJDIR)/%.o: $(CSRC)/%.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.inc) 
 # retrieval.cu feeds integer rank logic from float comparisons: IEEE exp / division and denormals (no flush-to-zero), so
 # that tiny DSL weights stay distinct exactly as in the reference's numpy code
 $(OBJDIR)/retrieval.o: NVFLAGS := $(filter-out --use_fast_math,$(NVFLAGS))
+# lfvila_head.cu: IEEE division, sqrt, exp and log in the pooled means, the norms and the log-sum-exps
+$(OBJDIR)/lfvila_head.o: NVFLAGS := $(filter-out --use_fast_math,$(NVFLAGS))
 
 $(LIB): $(OBJS)
 	@mkdir -p $(LIBDIR)

@@ -128,6 +128,36 @@ int xp_frame_pool_fwd(const float* proj, float* feat, float* inv_frame, float* i
                       void* stream);
 int xp_frame_pool_bwd(const float* dfeat, const float* feat, const float* proj, const float* inv_frame,
                       const float* inv_video, void* dproj_bf16, int32_t B, int32_t T, int32_t P, float scale, void* stream);
+/* Head of LF-VILA's video classification model (lfvila_video_classification.py:32-62).  Every reduction runs in a fixed
+ * order without atomics: repeated calls are bitwise equal.  Every pointer must be 16-byte aligned (optional ones may be
+ * NULL); refused before any launch.
+ * pool: x [B, N, Hp, Wp, C] of x_dtype (XP_DTYPE_F32 / _F16 / _BF16) -> MaxPool2d((2, 3), stride 1) per frame over the
+ * X = (Hp-1)(Wp-2) windows, torch's arg-max rule (first maximum of a tie in window scan order; a NaN replaces the running
+ * maximum); frame_raw [B*N, C] = mean over the X window maxima, global_raw [B, C] = mean over all N*X of them (one sum,
+ * one division), fp32 plus bf16 copies; argmax [B, N, X, C] uint8 = the winning position kh*3+kw of every window.
+ * Needs Hp >= 2, Wp >= 3, B*N < 2^31.  The backward writes every element of dx [B, N, Hp, Wp, C] (x_dtype) by gathering
+ * over the windows that cover it; d_frame [B*N, C] and d_global [B, C] may each be NULL (no gradient). */
+int xp_lfvila_pool_fwd(const void* x, int32_t x_dtype, float* frame_raw, void* frame_bf16, float* global_raw,
+                       void* global_bf16, uint8_t* argmax, int32_t B, int32_t N, int32_t Hp, int32_t Wp, int32_t C,
+                       void* stream);
+int xp_lfvila_pool_bwd(const float* d_frame, const float* d_global, const uint8_t* argmax, void* dx, int32_t x_dtype,
+                       int32_t B, int32_t N, int32_t Hp, int32_t Wp, int32_t C, void* stream);
+/* F.normalize(x, dim=-1) on fp32 rows [rows, C]: y = x / max(||x||, 1e-12), optional bf16 copy, norm [rows] = ||x||.
+ * Backward of dy (+ dy2, either may be NULL), written as bf16: (g - y (y . g)) / ||x||, or g / 1e-12 below the clamp. */
+int xp_lfvila_normalize_fwd(const float* x, float* y, void* y_bf16, float* norm, int32_t rows, int32_t C, void* stream);
+int xp_lfvila_normalize_bwd(const float* dy, const float* dy2, const float* y, const float* norm, void* dx_bf16,
+                            int32_t rows, int32_t C, void* stream);
+/* nn.CrossEntropyLoss (mean) and accuracy (argmax == label, first index of a tie, mean over B) of fp32 logits [B, n_labels]
+ * with row pitch ld, int64 labels [B]; 1 <= B <= 4096.  pred (optional) receives the logits with row pitch n_labels;
+ * lse [B] is kept for the backward.  Label -100 is ignored by the
+ * loss (ignore_index); any other label outside [0, n_labels) gives a NaN loss.  The backward writes dlogits bf16 [B, ld_out]
+ * = d_loss[0] / count * (softmax - onehot) (+ d_logits, pitch ld_d, if not NULL), the columns past n_labels zero; a NULL
+ * d_loss means no loss gradient. */
+int xp_lfvila_ce_fwd(const float* logits, int64_t ld, const int64_t* labels, int32_t B, int32_t n_labels, float* pred,
+                     float* lse, float* loss, float* acc, void* stream);
+int xp_lfvila_ce_bwd(const float* logits, int64_t ld, const float* lse, const int64_t* labels, const float* d_loss,
+                     const float* d_logits, int64_t ld_d, void* dlogits_bf16, int64_t ld_out, int32_t B, int32_t n_labels,
+                     void* stream);
 /* out[c] += scale * sum_r x[r,c]: bias gradients of every nn.Linear.  x must be 16-byte aligned. */
 int xp_colsum_bf16(const void* x, int64_t ld, float* out, int64_t rows, int32_t C, float scale, void* stream);
 /* fp32 master parameter -> bf16 compute copy. */

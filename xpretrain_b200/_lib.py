@@ -94,6 +94,16 @@ SIGNATURES = {
     "xp_frame_pool_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "xp_frame_pool_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                   c_float, c_void_p]),
+    "xp_lfvila_pool_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                   c_int, c_int, c_void_p]),
+    "xp_lfvila_pool_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                   c_void_p]),
+    "xp_lfvila_normalize_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "xp_lfvila_normalize_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "xp_lfvila_ce_fwd": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
+    "xp_lfvila_ce_bwd": (c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_int,
+                                 c_int, c_void_p]),
     "xp_colsum_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_int, c_float, c_void_p]),
     "xp_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_void_p]),
     "xp_vip_patchify": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_int, c_int, c_int, c_void_p]),

@@ -1,0 +1,182 @@
+"""LF-VILA's long-form video classification model (COIN, LVU) on the H100 kernels.
+
+Drop-in for `LFVILA_Video_Classification` of LF-VILA/src/models/lfvila_video_classification.py:16-68: the same constructor
+`(args, config)` (`config.VideoEncoder`, `config.bert_config` read for `hidden_size`, `config.DATA.classification_labels`),
+the same `state_dict()` (`video_encoder.*` of modeling/swin3d.py, `video_global_proj.*`, `video_frame_proj.*`,
+`classifier.*`; the max-pool holds nothing), and the same `forward(video_frames, labels) -> dict(video_global_feat,
+video_frame_feat, prediction, loss, acc)`.
+
+The encoder call is modeling/swin3d.py's, unchanged.  The head after it runs as ONE autograd.Function:
+  * xp_lfvila_pool_fwd: MaxPool2d((2, 3), stride 1) over each frame's Hp x Wp grid, the frame means `video_frame_feat`
+    [B*N, C] and the clip means `video_feat` [B, C] (mean over all N * X window maxima, :40) in fp32 with bf16 copies,
+    the arg-max window position saved as a byte; its backward gathers over the windows covering each element;
+  * video_global_proj / video_frame_proj: the wgmma GEMM (bf16 operands, fp32 out, bias in the epilogue);
+  * xp_lfvila_normalize_*: F.normalize (x / max(||x||, 1e-12)) and its gradient, below the clamp included;
+  * classifier: the same GEMM on a weight padded with zero rows to a multiple of 8 labels (the GEMM's N alignment), the
+    logits written with that padded pitch;
+  * xp_lfvila_ce_*: nn.CrossEntropyLoss and `acc` (first-index argmax) with a fixed reduction order.
+Outputs are fp32 whatever the video dtype (fp16 video, the trainer's --fp16 input, runs the encoder on fp16 input and the
+pool on its fp16 output).  There is no CPU path.
+"""
+from __future__ import annotations
+
+import json
+from typing import Dict
+
+import torch
+import torch.nn as nn
+
+from .. import _lib, ops
+from ._blocks import alloc_flat
+from ._weights import WeightMirror
+from .swin3d import SwinTransformer3D
+
+bf16, f32 = torch.bfloat16, torch.float32
+_HEAD = ("video_global_proj.weight", "video_global_proj.bias", "video_frame_proj.weight", "video_frame_proj.bias",
+         "classifier.weight", "classifier.bias")
+
+
+def _get(obj, key, default=None):
+    if isinstance(obj, dict):
+        return obj.get(key, default)
+    return getattr(obj, key, default)
+
+
+class LFVILA_Video_Classification(nn.Module):
+    """Constructor mirrors lfvila_video_classification.py:17-29."""
+
+    def __init__(self, args, config):
+        super().__init__()
+        self.cfg = config
+        self.video_encoder = SwinTransformer3D(**dict(_get(config, "VideoEncoder")))
+        with open(_get(config, "bert_config")) as f:       # BertConfig.from_json_file: only hidden_size is used
+            hidden = int(json.load(f).get("hidden_size", 768))
+        if hidden != self.video_encoder.num_features:
+            raise ValueError(f"bert_config hidden_size {hidden} must equal the video encoder's num_features "
+                             f"{self.video_encoder.num_features} (the projections take the encoder output)")
+        self.video_global_proj = nn.Linear(hidden, hidden)
+        self.video_frame_proj = nn.Linear(hidden, hidden)
+        self.n_labels = int(_get(_get(config, "DATA"), "classification_labels"))
+        self.classifier = nn.Linear(hidden, self.n_labels)
+        self._head: Dict[str, object] = {}
+
+    def forward(self, video_frames: torch.Tensor, labels=None):
+        if not isinstance(labels, torch.Tensor):
+            # nn.CrossEntropyLoss()(logits, labels) raises this for labels=None (:58-59)
+            raise TypeError(f"cross_entropy_loss(): argument 'target' (position 2) must be Tensor, not "
+                            f"{type(labels).__name__}")
+        if not video_frames.is_cuda:
+            raise _lib.XpError("xpretrain_b200 LFVILA_Video_Classification needs CUDA tensors on an H100: there is no "
+                               "CPU path")
+        if labels.dtype != torch.int64 or labels.dim() != 1 or labels.shape[0] != video_frames.shape[0]:
+            raise ValueError(f"labels must be int64 class indices of shape [{video_frames.shape[0]}] (got {labels.dtype} "
+                             f"{list(labels.shape)})")
+        video_embd, _ = self.video_encoder(video_frames)                  # [B, N, H, W, C]
+        params = [dict(self.named_parameters())[n] for n in _HEAD]
+        g, fr, pred, loss, acc = _HeadFunction.apply(self, torch.is_grad_enabled(), video_embd,
+                                                     labels.to(video_embd.device), *params)
+        return dict(video_global_feat=g, video_frame_feat=fr, prediction=pred, loss=loss, acc=acc)
+
+
+def _head_weights(model: LFVILA_Video_Classification):
+    """bf16 compute copies of the three head weights (the classifier's padded with zero rows to a multiple of 8) and the
+    classifier bias padded with zeros, re-cast on every forward by one launch (modeling/_weights.py)."""
+    dev = model.classifier.weight.device
+    h = model._head
+    if h.get("device") != dev:
+        C, n = model.classifier.weight.shape[1], model.n_labels
+        n_pad = (n + 7) // 8 * 8
+        h.clear()
+        h.update(device=dev, mirror=WeightMirror(), n_pad=n_pad,
+                 wg=torch.empty(C, C, dtype=bf16, device=dev), wf=torch.empty(C, C, dtype=bf16, device=dev),
+                 wc=torch.zeros(n_pad, C, dtype=bf16, device=dev), bc=torch.zeros(n_pad, dtype=f32, device=dev))
+    n = model.n_labels
+    h["mirror"].refresh([(model.video_global_proj.weight, h["wg"]), (model.video_frame_proj.weight, h["wf"]),
+                         (model.classifier.weight, h["wc"][:n]), (model.classifier.bias, h["bc"][:n])])
+    return h
+
+
+class _HeadFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, model: LFVILA_Video_Classification, grad_mode: bool, x: torch.Tensor, labels: torch.Tensor, *params):
+        # grad_mode = torch.is_grad_enabled() of the caller: evaluation keeps nothing for a backward
+        ctx.set_materialize_grads(False)
+        B, N, Hp, Wp, C = x.shape
+        dev = x.device
+        X = max(Hp - 1, 0) * max(Wp - 2, 0)
+        h = _head_weights(model)
+        n, n_pad = model.n_labels, h["n_pad"]
+        frame_raw = torch.empty(B * N, C, dtype=f32, device=dev)
+        frame_bf = torch.empty(B * N, C, dtype=bf16, device=dev)
+        global_raw = torch.empty(B, C, dtype=f32, device=dev)
+        global_bf = torch.empty(B, C, dtype=bf16, device=dev)
+        argmax = torch.empty(B, N, X, C, dtype=torch.uint8, device=dev)
+        ops.lfvila_pool_fwd(x, frame_raw, frame_bf, global_raw, global_bf, argmax)
+        gproj = torch.empty(B, C, dtype=f32, device=dev)
+        ops.linear_fwd(global_bf, h["wg"], model.video_global_proj.bias, gproj, out_mode=_lib.OUT_F32)
+        fproj = torch.empty(B * N, C, dtype=f32, device=dev)
+        ops.linear_fwd(frame_bf, h["wf"], model.video_frame_proj.bias, fproj, out_mode=_lib.OUT_F32)
+        gfeat, gfeat_bf, gnorm = torch.empty_like(gproj), torch.empty(B, C, dtype=bf16, device=dev), gproj.new_empty(B)
+        ops.lfvila_normalize_fwd(gproj, gfeat, gfeat_bf, gnorm)
+        ffeat, fnorm = torch.empty_like(fproj), fproj.new_empty(B * N)
+        ops.lfvila_normalize_fwd(fproj, ffeat, None, fnorm)
+        del gproj, fproj
+        logits = torch.empty(B, n_pad, dtype=f32, device=dev)
+        ops.linear_fwd(gfeat_bf, h["wc"], h["bc"], logits, out_mode=_lib.OUT_F32)
+        pred = torch.empty(B, n, dtype=f32, device=dev)
+        lse, loss, acc = logits.new_empty(B), logits.new_empty(()), logits.new_empty(1)
+        ops.lfvila_ce_fwd(logits, n, labels, pred, lse, loss, acc)
+        ctx.mark_non_differentiable(acc)
+        ctx.saved = None
+        if grad_mode and any(ctx.needs_input_grad[2:]):
+            ctx.model, ctx.x_meta = model, (x.shape, x.dtype)
+            ctx.saved = (argmax, frame_bf, global_bf, gfeat, gfeat_bf, gnorm, ffeat, fnorm, logits, lse, labels)
+        return gfeat, ffeat.view(B, N, C), pred, loss, acc
+
+    @staticmethod
+    def backward(ctx, d_gfeat, d_ffeat, d_pred, d_loss, _d_acc):
+        model = ctx.model
+        argmax, frame_bf, global_bf, gfeat, gfeat_bf, gnorm, ffeat, fnorm, logits, lse, labels = ctx.saved
+        ctx.saved = None
+        (B, N, Hp, Wp, C), xdt = ctx.x_meta
+        dev = logits.device
+        h = model._head
+        n, n_pad = model.n_labels, h["n_pad"]
+        named = dict(model.named_parameters())
+        grads: Dict[str, torch.Tensor] = {}
+        shapes = {k: tuple(named[k].shape) for k in _HEAD if not k.startswith("classifier.")}
+        shapes.update({"classifier.weight": (n_pad, C), "classifier.bias": (n_pad,)})   # padded: the GEMMs write n_pad rows
+        alloc_flat(shapes, grads, dev)
+        d_global = d_frame = None
+        # classifier, from the loss and / or a gradient of `prediction`
+        d_class = None
+        if d_loss is not None or d_pred is not None:
+            dlog = torch.empty(B, n_pad, dtype=bf16, device=dev)
+            ops.lfvila_ce_bwd(logits, n, lse, labels, d_loss, d_pred, dlog)
+            ops.linear_wgrad(dlog, gfeat_bf, grads["classifier.weight"])
+            ops.colsum(dlog, grads["classifier.bias"])
+            d_class = torch.empty(B, C, dtype=f32, device=dev)
+            ops.linear_dgrad(dlog, h["wc"], d_class, out_mode=_lib.OUT_F32)
+        # video_global_proj + normalize, from the classifier and / or a gradient of `video_global_feat`
+        if d_class is not None or d_gfeat is not None:
+            dg = torch.empty(B, C, dtype=bf16, device=dev)
+            ops.lfvila_normalize_bwd(d_class, None if d_gfeat is None else d_gfeat.to(f32).contiguous(), gfeat, gnorm, dg)
+            ops.linear_wgrad(dg, global_bf, grads["video_global_proj.weight"])
+            ops.colsum(dg, grads["video_global_proj.bias"])
+            d_global = torch.empty(B, C, dtype=f32, device=dev)
+            ops.linear_dgrad(dg, h["wg"], d_global, out_mode=_lib.OUT_F32)
+        # video_frame_proj + normalize, from a gradient of `video_frame_feat` (no loss uses it)
+        if d_ffeat is not None:
+            df = torch.empty(B * N, C, dtype=bf16, device=dev)
+            ops.lfvila_normalize_bwd(d_ffeat.to(f32).reshape(B * N, C).contiguous(), None, ffeat, fnorm, df)
+            ops.linear_wgrad(df, frame_bf, grads["video_frame_proj.weight"])
+            ops.colsum(df, grads["video_frame_proj.bias"])
+            d_frame = torch.empty(B * N, C, dtype=f32, device=dev)
+            ops.linear_dgrad(df, h["wf"], d_frame, out_mode=_lib.OUT_F32)
+        dx = None
+        if ctx.needs_input_grad[2]:
+            dx = torch.empty(B, N, Hp, Wp, C, dtype=xdt, device=dev)
+            ops.lfvila_pool_bwd(d_frame, d_global, argmax, dx)
+        grads["classifier.weight"] = grads["classifier.weight"][:n]
+        grads["classifier.bias"] = grads["classifier.bias"][:n]
+        return (None, None, dx, None) + tuple(grads[k] if ctx.needs_input_grad[4 + j] else None for j, k in enumerate(_HEAD))

@@ -171,7 +171,9 @@ class SwinTransformer3D(nn.Module):
                 self.draw_drop_masks(x.shape[0], x.device, x.dtype)
         names, params = zip(*[(n, p) for n, p in self.named_parameters()
                               if not n.startswith(("norm_local.", "local_feat_proj."))])
-        out = _Swin3DFunction.apply(self, list(names), masks, x, *params)
+        # torch.is_grad_enabled() of the caller: Function.forward always runs under no_grad, and needs_input_grad reflects
+        # requires_grad even then, so without it evaluation under torch.no_grad() would keep every activation to the end
+        out = _Swin3DFunction.apply(self, list(names), masks, torch.is_grad_enabled(), x, *params)
         return out, out
 
 
@@ -330,12 +332,12 @@ def _block_bwd(model, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads:
 # ------------------------------------------------------------------------------------------- function
 class _Swin3DFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, model: SwinTransformer3D, names: List[str], masks, video: torch.Tensor, *params):
+    def forward(ctx, model: SwinTransformer3D, names: List[str], masks, grad_mode: bool, video: torch.Tensor, *params):
         B, Cin, D, Hin, Win = video.shape
         ph, pw = model.patch_size[1], model.patch_size[2]
         if Cin != 3 or Hin % ph or Win % pw:
             raise ValueError("video must be [B, 3, D, H, W] with H, W divisible by the patch size")
-        save = any(ctx.needs_input_grad[4:])
+        save = grad_mode and any(ctx.needs_input_grad[5:])
         refresh_weights(model)
         dev = video.device
         C0 = model.embed_dim
@@ -433,4 +435,5 @@ class _Swin3DFunction(torch.autograd.Function):
         ops.linear_wgrad(dtok, patches, grads["patch_embed.proj.weight"].view(C0, -1))
         ops.colsum(dtok, grads["patch_embed.proj.bias"])
         ctx.saved = None
-        return (None, None, None, None) + tuple(grads[n] if ctx.needs_input_grad[4 + j] else None for j, n in enumerate(names))
+        return (None, None, None, None, None) + tuple(grads[n] if ctx.needs_input_grad[5 + j] else None
+                                                      for j, n in enumerate(names))

@@ -199,6 +199,74 @@ def frame_pool_bwd(dfeat, feat, proj, inv_frame, inv_video, dproj_bf16, T: int, 
     _call("xp_frame_pool_bwd", _p(dfeat), _p(feat), _p(proj), _p(inv_frame), _p(inv_video), _p(dproj_bf16), B, T, P, scale)
 
 
+def lfvila_pool_fwd(x, frame_raw, frame_bf16, global_raw, global_bf16, argmax):
+    """LF-VILA's MaxPool2d((2, 3), stride 1) + frame / clip means (lfvila_video_classification.py:32-43) on the encoder
+    output x [B, N, Hp, Wp, C] (fp32, fp16 or bf16): frame_raw fp32 [B*N, C], global_raw fp32 [B, C], their bf16 copies,
+    and the winning window position of every (b, n, window, c) in argmax uint8 [B, N, X, C]."""
+    B, N, Hp, Wp, C_ = x.shape
+    X = max(Hp - 1, 0) * max(Wp - 2, 0)
+    assert frame_raw.dtype == f32 and global_raw.dtype == f32 and frame_bf16.dtype == bf16 and global_bf16.dtype == bf16
+    assert argmax.dtype == torch.uint8 and argmax.numel() == B * N * X * C_
+    assert frame_raw.numel() == frame_bf16.numel() == B * N * C_ and global_raw.numel() == global_bf16.numel() == B * C_
+    x = aligned_input(x)
+    _call("xp_lfvila_pool_fwd", _p(x), _DT[x.dtype], _p(frame_raw), _p(frame_bf16), _p(global_raw), _p(global_bf16),
+          _p(argmax), B, N, Hp, Wp, C_)
+
+
+def lfvila_pool_bwd(d_frame, d_global, argmax, dx):
+    """dx [B, N, Hp, Wp, C] (the dtype of x) from d_frame fp32 [B*N, C] and / or d_global fp32 [B, C] (None: no gradient)."""
+    B, N, Hp, Wp, C_ = dx.shape
+    for t, n in ((d_frame, B * N * C_), (d_global, B * C_)):
+        assert t is None or (t.dtype == f32 and t.is_contiguous() and t.numel() == n)
+    assert dx.is_contiguous()
+    _call("xp_lfvila_pool_bwd", _p(d_frame), _p(d_global), _p(argmax), _p(dx), _DT[dx.dtype], B, N, Hp, Wp, C_)
+
+
+def lfvila_normalize_fwd(x, y, y_bf16, norm):
+    """y = F.normalize(x, dim=-1) (x / max(||x||, 1e-12)) on fp32 rows, with an optional bf16 copy; norm [rows] = ||x||."""
+    rows, C_ = x.shape
+    assert x.dtype == f32 and y.dtype == f32 and x.is_contiguous() and y.is_contiguous() and y.shape == x.shape
+    assert y_bf16 is None or (y_bf16.dtype == bf16 and y_bf16.is_contiguous() and y_bf16.shape == x.shape)
+    assert norm.dtype == f32 and norm.numel() == rows
+    _call("xp_lfvila_normalize_fwd", _p(x), _p(y), _p(y_bf16), _p(norm), rows, C_)
+
+
+def lfvila_normalize_bwd(dy, dy2, y, norm, dx_bf16):
+    """dx bf16 = gradient of lfvila_normalize_fwd for the sum of dy and dy2 (fp32 [rows, C], either may be None)."""
+    rows, C_ = y.shape
+    for t in (dy, dy2):
+        assert t is None or (t.dtype == f32 and t.is_contiguous() and t.shape == y.shape)
+    assert dx_bf16.dtype == bf16 and dx_bf16.is_contiguous() and dx_bf16.shape == y.shape
+    _call("xp_lfvila_normalize_bwd", _p(dy), _p(dy2), _p(y), _p(norm), _p(dx_bf16), rows, C_)
+
+
+def lfvila_ce_fwd(logits, n_labels: int, labels, pred, lse, loss, acc):
+    """nn.CrossEntropyLoss() and (argmax == label).float().mean(0, keepdim=True) of logits fp32 [B, >= n_labels] (row pitch
+    logits.stride(0)); pred (or None) receives the logits as a contiguous [B, n_labels], lse fp32 [B] is kept for the
+    backward, loss and acc are fp32 one-element tensors."""
+    B = logits.shape[0]
+    assert logits.dtype == f32 and logits.stride(1) == 1 and labels.dtype == torch.int64 and labels.numel() == B
+    assert pred is None or (pred.dtype == f32 and pred.is_contiguous() and pred.shape == (B, n_labels))
+    assert lse.dtype == f32 and lse.numel() == B and loss.dtype == f32 and acc.dtype == f32
+    labels = aligned_input(labels)
+    _call("xp_lfvila_ce_fwd", _p(logits), logits.stride(0), _p(labels), B, n_labels, _p(pred), _p(lse), _p(loss), _p(acc))
+
+
+def lfvila_ce_bwd(logits, n_labels: int, lse, labels, d_loss, d_logits, dlogits_bf16):
+    """dlogits bf16 [B, ld] = d_loss * d(loss)/d(logits) + d_logits (d_loss: fp32 scalar tensor or None; d_logits: fp32
+    [B, n_labels] or None); the columns past n_labels are written as zeros."""
+    B = logits.shape[0]
+    assert dlogits_bf16.dtype == bf16 and dlogits_bf16.stride(1) == 1 and dlogits_bf16.shape[0] == B
+    if d_loss is not None:
+        d_loss = d_loss.reshape(1).to(f32).contiguous()
+    if d_logits is not None:
+        d_logits = aligned_input(d_logits.to(f32))
+        assert d_logits.shape == (B, n_labels)
+    labels = aligned_input(labels)
+    _call("xp_lfvila_ce_bwd", _p(logits), logits.stride(0), _p(lse), _p(labels), _p(d_loss), _p(d_logits),
+          d_logits.stride(0) if d_logits is not None else 0, _p(dlogits_bf16), dlogits_bf16.stride(0), B, n_labels)
+
+
 def colsum(x: torch.Tensor, out: torch.Tensor, scale: float = 1.0):
     rows, C_ = x.shape
     _call("xp_colsum_bf16", _p(x), x.stride(0), _p(out), rows, C_, scale)
