@@ -211,12 +211,13 @@ def test_hidden_states_against_oracle(dev):
     """Layer-by-layer hidden states of a 2-layer model vs the oracle run on the host (seeded, not from goldens)."""
     from oracle import clipvip_oracle as O
     from xpretrain_b200.modeling import clip_vip as M
+    from xpretrain_b200.modeling._weights import param_layout
     cfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, 2, 3072), text=O.TowerCfg(512, 8, 2, 2048))
     sd = O.init_state_dict(cfg, seed=11)
     video, ids, mask = O.synthetic_batch(2, 3, 16, cfg, seed=5, ragged_text=True)
     _, vh = O.vision_tower(sd, video, cfg, return_hidden=True)
     model = _build(cfg, sd, dev)
-    M._refresh_weights(model.clipmodel)
+    param_layout(model.clipmodel).refresh()
     proj, sv = M._vision_fwd(model.clipmodel, video.to(dev), save=True)
     S = sv.S
     for i, want in enumerate(vh[:-1]):

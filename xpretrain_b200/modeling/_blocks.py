@@ -1,34 +1,20 @@
 """Pre-LN block pieces that TimeSformer (modeling/timesformer.py) and Swin-3D (modeling/swin3d.py) share.
 
-Both run their blocks over token-major bf16 matrices [rows, C] with the GEMM weights served by the named-weight cache of
-modeling/_weights.py and the gradients written into a `grads` dict keyed by parameter name.  The LayerNorm helpers take the
+Both run their blocks over token-major bf16 matrices [rows, C] with the GEMM weights `w[name]` of the model's parameter layout
+(modeling/_weights.py) and the gradients written into a `grads` dict keyed by parameter name.  The LayerNorm helpers take the
 kernel choice from `wide`: TimeSformer uses the row-mapped kernel, Swin-3D `layernorm_any_*` (the wide kernel above 1024
 columns, which its PatchMerging norms reach).
 """
 from __future__ import annotations
 
-from typing import Dict, NamedTuple, Optional
+from typing import NamedTuple, Optional
 
 import torch
 import torch.nn as nn
 
 from .. import _lib, ops
-from ._weights import weight
 
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def alloc_flat(shapes: Dict[str, tuple], grads: Dict[str, torch.Tensor], dev) -> torch.Tensor:
-    """One zeroed fp32 buffer holding all gradients of a group as 16-byte aligned views: the data-parallel
-    all-reduce of the group is then a single collective on `flat` (no packing copies)."""
-    offs, total = {}, 0
-    for n, shp in shapes.items():
-        offs[n] = total
-        total += (int(torch.Size(shp).numel()) + 3) // 4 * 4
-    flat = torch.zeros(total, dtype=f32, device=dev)
-    for n, shp in shapes.items():
-        grads[n] = flat[offs[n]:offs[n] + torch.Size(shp).numel()].view(shp)
-    return flat
 
 
 def layernorm(x, ln: nn.LayerNorm, wide: bool = False, out=None):
@@ -60,25 +46,25 @@ def layernorm_bwd(dy, x, ln: nn.LayerNorm, mean, rstd, dres, grads, name: str, w
     return dx
 
 
-def linear_bwd(model, name: str, dy, x_in, grads, out=None, **dgrad_kw):
+def linear_bwd(w, name: str, dy, x_in, grads, out=None, **dgrad_kw):
     """dW += dy^T x_in, db += colsum(dy), returns dx = dy W (bf16), written into `out` when given."""
     ops.linear_wgrad(dy, x_in, grads[name + ".weight"])
     ops.colsum(dy, grads[name + ".bias"])
-    w = weight(model, name + ".weight")
-    dx = torch.empty(dy.shape[0], w.shape[1], dtype=bf16, device=dy.device) if out is None else out
-    ops.linear_dgrad(dy, w, dx, **dgrad_kw)
+    wt = w[name + ".weight"]
+    dx = torch.empty(dy.shape[0], wt.shape[1], dtype=bf16, device=dy.device) if out is None else out
+    ops.linear_dgrad(dy, wt, dx, **dgrad_kw)
     return dx
 
 
-def residual_linear(model, name: str, lin: nn.Linear, a, residual, scale):
+def residual_linear(w, name: str, lin: nn.Linear, a, residual, scale):
     """residual + drop_path(lin(a)): fused into the GEMM epilogue when no path is dropped, else GEMM + one row-scale pass."""
     rows, N = a.shape[0], lin.weight.shape[0]
     out = torch.empty(rows, N, dtype=bf16, device=a.device)
     if scale is None:
-        ops.linear_fwd(a, weight(model, name + ".weight"), lin.bias, out, residual=residual, ldr=N)
+        ops.linear_fwd(a, w[name + ".weight"], lin.bias, out, residual=residual, ldr=N)
     else:
         tmp = torch.empty(rows, N, dtype=bf16, device=a.device)
-        ops.linear_fwd(a, weight(model, name + ".weight"), lin.bias, tmp)
+        ops.linear_fwd(a, w[name + ".weight"], lin.bias, tmp)
         ops.rowscale(tmp, scale, out, residual=residual)
     return out
 
@@ -101,7 +87,7 @@ class MlpSaved(NamedTuple):
     f1: torch.Tensor                 # GELU(fc1), fc2's input
 
 
-def mlp_fwd(model, p: str, blk, x, save: bool, scale, wide: bool = False):
+def mlp_fwd(w, p: str, blk, x, save: bool, scale, wide: bool = False):
     """x + drop_path(fc2(erf-GELU(fc1(norm2(x))))) for a block with `norm2` and `mlp.fc1` / `mlp.fc2` under prefix p.
     Returns (out, MlpSaved); the record holds the half's tensors whether or not the caller keeps it."""
     I = blk.mlp.fc1.weight.shape[0]
@@ -109,16 +95,16 @@ def mlp_fwd(model, p: str, blk, x, save: bool, scale, wide: bool = False):
     h, mean, rstd = layernorm(x, blk.norm2, wide)
     pre = torch.empty(rows, I, dtype=bf16, device=dev) if save else None
     f1 = torch.empty(rows, I, dtype=bf16, device=dev)
-    ops.linear_fwd(h, weight(model, p + "mlp.fc1.weight"), blk.mlp.fc1.bias, f1, act=_lib.ACT_GELU_ERF, aux=pre, ld_aux=I)
-    out = residual_linear(model, p + "mlp.fc2", blk.mlp.fc2, f1, x, scale)
+    ops.linear_fwd(h, w[p + "mlp.fc1.weight"], blk.mlp.fc1.bias, f1, act=_lib.ACT_GELU_ERF, aux=pre, ld_aux=I)
+    out = residual_linear(w, p + "mlp.fc2", blk.mlp.fc2, f1, x, scale)
     return out, MlpSaved(x, mean, rstd, h, pre, f1)
 
 
-def mlp_bwd(model, p: str, blk, dx, sv: MlpSaved, grads, scale, wide: bool = False):
+def mlp_bwd(w, p: str, blk, dx, sv: MlpSaved, grads, scale, wide: bool = False):
     """Backward of mlp_fwd: dx is d(loss)/d(out); returns d(loss)/d(x)."""
     I = blk.mlp.fc1.weight.shape[0]
-    dpre = linear_bwd(model, p + "mlp.fc2", drop_scale(dx, scale), sv.f1, grads, act=_lib.ACT_DGELU_ERF, aux=sv.pre,
+    dpre = linear_bwd(w, p + "mlp.fc2", drop_scale(dx, scale), sv.f1, grads, act=_lib.ACT_DGELU_ERF, aux=sv.pre,
                       ld_aux=I)
-    dh = linear_bwd(model, p + "mlp.fc1", dpre, sv.h, grads)
+    dh = linear_bwd(w, p + "mlp.fc1", dpre, sv.h, grads)
     del dpre
     return layernorm_bwd(dh, sv.x, blk.norm2, sv.mean, sv.rstd, dx, grads, p + "norm2", wide)

@@ -1,18 +1,24 @@
-"""bf16 compute copies of the fp32 master parameters, refreshed on EVERY forward by one table-driven launch.
+"""The parameter layout of a model: how its fp32 parameters map onto the operands the kernels read and the gradients they write.
 
-The reference modules read their own fp32 parameters at each call (CLIP_ViP.py:445-460), so any in-place write —
-including the ones autograd's version counter does not see: `p.data.addcdiv_` in the reference AdamW
-(CLIP-ViP/src/optimization/adamw.py:89,101), apex master->model copies, EMA swaps, `load_state_dict` — is visible to
-the next forward.  A cache keyed on `p._version` breaks that contract (VERDICT r1 / ADVICE r1), so there is no cache
-validity test at all: the cast is 6 B per parameter (~0.15 ms for the 150 M parameters of CLIP-ViP) and simply runs.
-Only the device-side pointer table is cached, keyed on the data pointers.
+Each model declares it once (`_declare_layout`), and `param_layout` builds it once per (model, device).  It provides:
+  * the parameter list its autograd.Function differentiates: every parameter but the `exclude`d prefixes, in
+    `named_parameters()` order (`params`, `names`), and the matching tuple of gradients for `backward` to return;
+  * the compute copies: every operand is a single parameter, or several stacked along rows (`fuse`, CLIP-ViP's q/k/v), zero-
+    padded to a multiple of 8 rows where the GEMM's N alignment needs it (`pad8`, LF-VILA's classifier).  Operands that
+    `cast` selects get a copy, bf16 for weights and fp32 for biases, looked up by operand name (`layout[name]`);
+  * the gradient groups: one zeroed fp32 flat buffer per group (`group`), with 16-byte aligned views shaped like the operands.
+    A parameter's gradient is the row slice of its operand's gradient, so a fused or padded operand is written down here only.
 
-Two layouts of the copies use this: CLIP-ViP's `_WeightPack` (q/k/v fused per layer, modeling/clip_vip.py) and the
-named-weight cache below (one copy per GEMM weight, `model._cache[name]`) of TimeSformer and Swin-3D.
+The copies are refreshed on EVERY forward by one table-driven launch.  The reference modules read their own fp32 parameters
+at each call (CLIP_ViP.py:445-460), so any in-place write — including the ones autograd's version counter does not see:
+`p.data.addcdiv_` in the reference AdamW (CLIP-ViP/src/optimization/adamw.py:89,101), apex master->model copies, EMA swaps,
+`load_state_dict` — is visible to the next forward.  A cache keyed on `p._version` breaks that contract (VERDICT r1 / ADVICE
+r1), so there is no cache validity test at all: the cast is 6 B per parameter (~0.15 ms for the 150 M parameters of
+CLIP-ViP) and simply runs.  Only the device-side pointer table is cached, keyed on the data pointers.
 """
 from __future__ import annotations
 
-from typing import List, Tuple
+from typing import Callable, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -51,21 +57,93 @@ class WeightMirror:
         ops.cast_table(self._table)
 
 
-def refresh_weights(model) -> None:
-    """Re-cast every GEMM weight (parameters with >= 2 dims that `weight` serves) of `model` into `model._cache` with ONE
-    launch on every forward."""
-    cache = model._cache
-    named = [(n, p) for n, p in model.named_parameters() if p.dim() >= 2 and n.endswith("weight")]
-    dev = named[0][1].device
-    if cache.get("__device__") != dev:
-        cache.clear()
-        cache["__device__"] = dev
-        cache["__mirror__"] = WeightMirror()
-        for n, p in named:
-            cache[n] = torch.empty(p.shape, dtype=bf16, device=dev)
-    cache["__mirror__"].refresh([(p, cache[n]) for n, p in named])
+def matrix_weight(name: str, p: torch.Tensor) -> bool:
+    """`cast` rule of the models whose GEMM weights are exactly their >= 2-D `weight` parameters."""
+    return p.dim() >= 2 and name.endswith("weight")
 
 
-def weight(model, name: str) -> torch.Tensor:
-    """bf16 compute copy of the GEMM weight `name` (refreshed for the whole model at the start of every forward)."""
-    return model._cache[name]
+class ParamLayout:
+    def __init__(self, model: torch.nn.Module, *, exclude: Sequence[str] = (), fuse: Optional[Dict[str, List[str]]] = None,
+                 cast: Callable[[str, torch.Tensor], bool] = lambda name, p: False, pad8: Iterable[str] = (),
+                 group: Callable[[str], Optional[str]] = lambda op: ""):
+        """exclude: name prefixes left out of the Function's parameters (their .grad stays None).  fuse: operand name ->
+        the parameters stacked along its rows, in order.  cast(operand name, its first parameter): whether the operand has a
+        compute copy.  pad8: operands padded with zero rows to a multiple of 8.  group(operand name): the key of its gradient
+        group, or None for a gradient the Function computes by other means."""
+        fuse, pad8 = fuse or {}, set(pad8)
+        named = [(n, p) for n, p in model.named_parameters() if not n.startswith(tuple(exclude))]
+        self.names = [n for n, _ in named]
+        self.params = [p for _, p in named]
+        self.device = self.params[0].device
+        param = dict(named)
+        owner = {m: op for op, members in fuse.items() for m in members}
+        members: Dict[str, List[str]] = {}
+        for n in self.names:                      # operands in the order of their first parameter
+            members.setdefault(owner.get(n, n), [])
+        for op in members:
+            members[op] = list(fuse.get(op, [op]))
+        # shapes[op]: the operand's shape; rows[name] = (operand, first row, end row) of each parameter inside it
+        self.shapes: Dict[str, Tuple[int, ...]] = {}
+        self.rows: Dict[str, Tuple[str, int, int]] = {}
+        for op, ms in members.items():
+            r = 0
+            for m in ms:
+                assert param[m].shape[1:] == param[ms[0]].shape[1:], (op, m)
+                self.rows[m] = (op, r, r + param[m].shape[0])
+                r += param[m].shape[0]
+            self.shapes[op] = (-(-r // 8) * 8 if op in pad8 else r,) + tuple(param[ms[0]].shape[1:])
+        # the gradient backward returns for each parameter: its operand's whole view, or a row slice of it
+        self._out = [(self.rows[n][0], None if self.shapes[self.rows[n][0]] == tuple(param[n].shape) else self.rows[n][1:])
+                     for n in self.names]
+        self._copies: Dict[str, torch.Tensor] = {}
+        self._items = []                          # (parameter, destination rows) pairs of the one re-cast launch
+        for op, ms in members.items():
+            if not cast(op, param[ms[0]]):
+                continue
+            dt = bf16 if param[ms[0]].dim() >= 2 else f32
+            self._copies[op] = buf = torch.zeros(self.shapes[op], dtype=dt, device=self.device)   # padding rows stay zero
+            self._items += [(param[m], buf[self.rows[m][1]:self.rows[m][2]]) for m in ms]
+        self._mirror = WeightMirror()
+        # groups[key] = (flat size, [(operand, offset, numel)]), each operand's view rounded up to 16 bytes
+        self.groups: Dict[str, Tuple[int, List[Tuple[str, int, int]]]] = {}
+        for op, shape in self.shapes.items():
+            key = group(op)
+            if key is None:
+                continue
+            total, views = self.groups.get(key, (0, []))
+            numel = int(torch.Size(shape).numel())
+            self.groups[key] = (total + (numel + 3) // 4 * 4, views + [(op, total, numel)])
+
+    def refresh(self) -> None:
+        """Re-cast every compute copy from the fp32 parameters with one launch."""
+        self._mirror.refresh(self._items)
+
+    def __getitem__(self, op: str) -> torch.Tensor:
+        """The compute copy of operand `op` (as of the last refresh)."""
+        return self._copies[op]
+
+    def alloc_grads(self, key: str, grads: Dict[str, torch.Tensor]) -> torch.Tensor:
+        """One zeroed fp32 buffer holding the gradients of group `key`, put into `grads` as operand-shaped views under the
+        operand names: the data-parallel all-reduce of the group is then a single collective on the returned buffer."""
+        total, views = self.groups[key]
+        flat = torch.zeros(total, dtype=f32, device=self.device)
+        for op, off, numel in views:
+            grads[op] = flat[off:off + numel].view(self.shapes[op])
+        return flat
+
+    def grads_out(self, grads: Dict[str, torch.Tensor], needs: Sequence[bool]) -> tuple:
+        """The parameter gradients for `backward` to return, from the operand gradients in `grads`: None where `needs`
+        (ctx.needs_input_grad of the parameters) is False or no gradient was computed."""
+        out = []
+        for (op, rows), need in zip(self._out, needs):
+            g = grads.get(op) if need else None
+            out.append(g if g is None or rows is None else g[rows[0]:rows[1]])
+        return tuple(out)
+
+
+def param_layout(model) -> ParamLayout:
+    """`model`'s layout, declared by its `_declare_layout()` and built once per device."""
+    lay = getattr(model, "_layout", None)
+    if lay is None or lay.params[0].device != lay.device:
+        lay = model._layout = model._declare_layout()
+    return lay

@@ -22,14 +22,13 @@ from __future__ import annotations
 
 from dataclasses import dataclass, field
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
 from .. import _lib, ops
-from ._blocks import alloc_flat
-from ._weights import WeightMirror
+from ._weights import ParamLayout, param_layout
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -80,8 +79,9 @@ class ClipVipConfig:
 
 # ----------------------------------------------------------------------- parameter containers
 class _Attention(nn.Module):
-    def __init__(self, width):
+    def __init__(self, width, heads):
         super().__init__()
+        self.scale = float(width // heads) ** -0.5          # CLIPAttention.scale = head_dim ** -0.5 (CLIP_ViP.py:245)
         self.k_proj = nn.Linear(width, width)
         self.v_proj = nn.Linear(width, width)
         self.q_proj = nn.Linear(width, width)
@@ -98,7 +98,7 @@ class _MLP(nn.Module):
 class _EncoderLayer(nn.Module):
     def __init__(self, tc: TowerConfig, eps):
         super().__init__()
-        self.self_attn = _Attention(tc.hidden_size)
+        self.self_attn = _Attention(tc.hidden_size, tc.num_attention_heads)
         self.layer_norm1 = nn.LayerNorm(tc.hidden_size, eps=eps)
         self.mlp = _MLP(tc.hidden_size, tc.intermediate_size)
         self.layer_norm2 = nn.LayerNorm(tc.hidden_size, eps=eps)
@@ -164,17 +164,6 @@ class _TextTransformer(nn.Module):
         self.final_layer_norm = nn.LayerNorm(cfg.text.hidden_size, eps=cfg.layer_norm_eps)
 
 
-def _tower_param_list(tower_prefix: str, n_layers: int) -> List[str]:
-    names = []
-    for i in range(n_layers):
-        p = f"{tower_prefix}.encoder.layers.{i}."
-        for lin in ("self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.out_proj", "mlp.fc1", "mlp.fc2"):
-            names += [p + lin + ".weight", p + lin + ".bias"]
-        for ln in ("layer_norm1", "layer_norm2"):
-            names += [p + ln + ".weight", p + ln + ".bias"]
-    return names
-
-
 class CLIPModel(nn.Module):
     """Same constructor argument style, attribute names and output keys as the reference CLIPModel."""
 
@@ -189,9 +178,7 @@ class CLIPModel(nn.Module):
         self.text_projection = nn.Linear(config.text.hidden_size, config.projection_dim, bias=False)
         self.logit_scale = nn.Parameter(torch.ones([]) * config.logit_scale_init_value)
         self._init_weights()
-        self._packs: Dict[str, "_WeightPack"] = {}
-        # fixed parameter order handed to the autograd.Function (position_ids buffers excluded)
-        self._pnames = [n for n, _ in self.named_parameters() if n != "logit_scale"]
+        self._packs: Dict[str, object] = {}        # the overlap streams and the p = 14 padded patch weight, per device
 
     @torch.no_grad()
     def _init_weights(self):
@@ -220,6 +207,20 @@ class CLIPModel(nn.Module):
                 m.weight.fill_(1.0)
             if isinstance(m, nn.Linear) and m.bias is not None:
                 m.bias.zero_()
+
+    def _declare_layout(self) -> ParamLayout:
+        """q/k/v of each encoder layer stacked into one [3C, C] operand and one fp32 [3C] bias; bf16 copies of the encoder
+        GEMM weights, the patch embedding and the two projections.  One gradient group per encoder layer, and one per tower
+        for the rest and its projection.  logit_scale is left out: the loss differentiates it."""
+        fuse = {}
+        for tower, tc in (("vision_model", self.config.vision), ("text_model", self.config.text)):
+            for i in range(tc.num_hidden_layers):
+                a = f"{tower}.encoder.layers.{i}.self_attn."
+                for kind in ("weight", "bias"):
+                    fuse[a + "qkv." + kind] = [a + x + "_proj." + kind for x in "qkv"]
+        gemm = ("qkv.weight", "qkv.bias", "out_proj.weight", "fc1.weight", "fc2.weight", "patch_embedding.weight",
+                "projection.weight")
+        return ParamLayout(self, exclude=("logit_scale",), fuse=fuse, cast=lambda n, p: n.endswith(gemm), group=_grad_group)
 
     # ------------------------------------------------------------------------------ public API
     def forward(self, input_ids=None, pixel_values=None, attention_mask=None, return_loss=False, **_unused):
@@ -265,61 +266,11 @@ class CLIPModel(nn.Module):
         return any(getattr(m, "gradient_checkpointing", False) for m in self.modules())
 
 
-# -------------------------------------------------------------------- bf16 compute copies
-class _WeightPack:
-    """bf16 compute copies of one tower's GEMM weights with q/k/v fused to [3C, C] (+ the fused fp32 qkv bias)."""
-
-    def __init__(self, layers, device, heads):
-        L = len(layers)
-        C_ = layers[0].self_attn.q_proj.weight.shape[0]
-        I = layers[0].mlp.fc1.weight.shape[0]
-        self.C, self.I, self.L = C_, I, L
-        self.q_scale = float(C_ // heads) ** -0.5          # CLIPAttention.scale = head_dim ** -0.5 (CLIP_ViP.py:245)
-        self.wqkv = torch.empty(L, 3 * C_, C_, dtype=bf16, device=device)
-        self.wo = torch.empty(L, C_, C_, dtype=bf16, device=device)
-        self.w1 = torch.empty(L, I, C_, dtype=bf16, device=device)
-        self.w2 = torch.empty(L, C_, I, dtype=bf16, device=device)
-        self.bqkv = torch.empty(L, 3 * C_, dtype=f32, device=device)
-
-    def items(self, layers):
-        C_ = self.C
-        out = []
-        for i, layer in enumerate(layers):
-            a = layer.self_attn
-            for j, lin in enumerate((a.q_proj, a.k_proj, a.v_proj)):
-                out.append((lin.weight, self.wqkv[i, j * C_:(j + 1) * C_]))
-                out.append((lin.bias, self.bqkv[i, j * C_:(j + 1) * C_]))
-            out += [(a.out_proj.weight, self.wo[i]), (layer.mlp.fc1.weight, self.w1[i]), (layer.mlp.fc2.weight, self.w2[i])]
-        return out
-
-
-def _refresh_weights(model: CLIPModel) -> None:
-    """Re-cast EVERY bf16 compute copy from the fp32 masters with one launch (modeling/_weights.py explains why this is
-    unconditional: in-place `p.data` writes of the reference's own optimizer must reach the next forward)."""
-    dev = model.logit_scale.device
-    pk = model._packs
-    if pk.get("device") != dev:
-        pk.clear()
-        pk["device"] = dev
-        pk["vision"] = _WeightPack(model.vision_model.encoder.layers, dev, model.config.vision.num_attention_heads)
-        pk["text"] = _WeightPack(model.text_model.encoder.layers, dev, model.config.text.num_attention_heads)
-        for key, p in (("small:patch", model.vision_model.embeddings.patch_embedding.weight),
-                       ("small:vproj", model.visual_projection.weight), ("small:tproj", model.text_projection.weight)):
-            pk[key] = torch.empty(p.shape, dtype=bf16, device=dev)
-        pk["mirror"] = WeightMirror()
-        items = pk["vision"].items(model.vision_model.encoder.layers) + pk["text"].items(model.text_model.encoder.layers)
-        items += [(model.vision_model.embeddings.patch_embedding.weight, pk["small:patch"]),
-                  (model.visual_projection.weight, pk["small:vproj"]), (model.text_projection.weight, pk["small:tproj"])]
-        pk["items"] = items           # (Parameter, destination view) pairs: Parameter objects are stable, their .data may move
-    pk["mirror"].refresh(pk["items"])
-
-
-def _pack(model: CLIPModel, which: str) -> _WeightPack:
-    return model._packs[which]
-
-
-def _small_bf16(model: CLIPModel, name: str) -> torch.Tensor:
-    return model._packs["small:" + name]
+def _grad_group(op: str) -> str:
+    """Gradient group of an operand: its encoder layer ("<tower>.encoder.layers.<i>."), else its tower."""
+    if ".encoder.layers." in op:
+        return ".".join(op.split(".")[:4]) + "."
+    return "text_model" if op.startswith(("text_model.", "text_projection.")) else "vision_model"
 
 
 # --------------------------------------------------------------------------- encoder layers
@@ -340,7 +291,7 @@ def _stream_dtype(model) -> torch.dtype:
     return torch.float16 if str(name) in ("fp16", "float16", "half") else f32
 
 
-def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, rows: int, save: bool, stream_dt,
+def _layer_fwd(x, pend, layer, w: ParamLayout, p: str, eps: float, attn_fwd, rows: int, save: bool, stream_dt,
                keep_input: bool = False, upto_fc1: bool = False):
     """One pre-LN residual block (CLIP_ViP.py:445-460).  x: residual stream [rows, C] in `stream_dt` (fp32 / fp16), or bf16 when
     stream_dt is None (round-1 path); pend: the previous block's bf16 branch output that still has to be added to it.
@@ -349,7 +300,7 @@ def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, ro
     `upto_fc1` rebuilds that tuple bit for bit.  `upto_fc1` stops after fc1 + QuickGELU and returns (None, None, saved): the
     backward never reads fc2's output."""
     fp32res = stream_dt is not None
-    C_, I = pk.C, pk.I
+    C_, I = layer.mlp.fc1.weight.shape[1], layer.mlp.fc1.weight.shape[0]
     dev = x.device
     plain = ops.rowmap(C_)
     mean1 = torch.empty(rows, dtype=f32, device=dev); rstd1 = torch.empty_like(mean1)
@@ -364,33 +315,35 @@ def _layer_fwd(x, pend, layer, pk: _WeightPack, i: int, eps: float, attn_fwd, ro
         ops.layernorm_fwd(x, plain, h, plain, ln1.weight, ln1.bias, mean1, rstd1, rows, C_, eps)
     qkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
     # q = (h Wq^T + bq) * head_dim**-0.5 : the scale multiplies the bias too (CLIP_ViP.py:341 / :269)
-    ops.linear_fwd(h, pk.wqkv[i], pk.bqkv[i], qkv, scale_cols=C_, col_scale=pk.q_scale)
+    ops.linear_fwd(h, w[p + "self_attn.qkv.weight"], w[p + "self_attn.qkv.bias"], qkv, scale_cols=C_,
+                   col_scale=layer.self_attn.scale)
     a = torch.empty(rows, C_, dtype=bf16, device=dev)
     att_saved = attn_fwd(qkv, a)
     mean2 = torch.empty(rows, dtype=f32, device=dev); rstd2 = torch.empty_like(mean2)
     h2 = torch.empty(rows, C_, dtype=bf16, device=dev)
     if fp32res:
         y1 = torch.empty(rows, C_, dtype=bf16, device=dev)
-        ops.linear_fwd(a, pk.wo[i], layer.self_attn.out_proj.bias, y1)                  # branch only: the add is in layer_norm2
+        # branch only: the add is in layer_norm2
+        ops.linear_fwd(a, w[p + "self_attn.out_proj.weight"], layer.self_attn.out_proj.bias, y1)
         x1 = torch.empty(rows, C_, dtype=stream_dt, device=dev)
         ops.layernorm_fwd(x, plain, h2, plain, ln2.weight, ln2.bias, mean2, rstd2, rows, C_, eps, add=y1, addmap=plain,
                           sum_out=x1, summap=plain)
         del y1
     else:
         x1 = torch.empty(rows, C_, dtype=bf16, device=dev)
-        ops.linear_fwd(a, pk.wo[i], layer.self_attn.out_proj.bias, x1, residual=x, ldr=C_)
+        ops.linear_fwd(a, w[p + "self_attn.out_proj.weight"], layer.self_attn.out_proj.bias, x1, residual=x, ldr=C_)
         ops.layernorm_fwd(x1, plain, h2, plain, ln2.weight, ln2.bias, mean2, rstd2, rows, C_, eps)
     pre = torch.empty(rows, I, dtype=bf16, device=dev) if save else None
     f1 = torch.empty(rows, I, dtype=bf16, device=dev)
-    ops.linear_fwd(h2, pk.w1[i], layer.mlp.fc1.bias, f1, act=_lib.ACT_QUICK_GELU, aux=pre, ld_aux=I)
+    ops.linear_fwd(h2, w[p + "mlp.fc1.weight"], layer.mlp.fc1.bias, f1, act=_lib.ACT_QUICK_GELU, aux=pre, ld_aux=I)
     saved = (x, mean1, rstd1, h, qkv, att_saved, a, x1, mean2, rstd2, h2, pre, f1) if save else (x if keep_input else None)
     if upto_fc1:
         return None, None, saved
     out = torch.empty(rows, C_, dtype=bf16, device=dev)
     if fp32res:
-        ops.linear_fwd(f1, pk.w2[i], layer.mlp.fc2.bias, out)                           # branch; added by the next LayerNorm
+        ops.linear_fwd(f1, w[p + "mlp.fc2.weight"], layer.mlp.fc2.bias, out)       # branch; added by the next LayerNorm
         return x1, out, saved
-    ops.linear_fwd(f1, pk.w2[i], layer.mlp.fc2.bias, out, residual=x1, ldr=C_)
+    ops.linear_fwd(f1, w[p + "mlp.fc2.weight"], layer.mlp.fc2.bias, out, residual=x1, ldr=C_)
     return out, None, saved
 
 
@@ -432,22 +385,22 @@ def _join_aux(aux) -> None:
         torch.cuda.current_stream().wait_stream(aux)
 
 
-def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch.Tensor], prefix: str, attn_bwd,
-               rows: int, aux=None):
+def _layer_bwd(dx, saved, layer, w: ParamLayout, grads: Dict[str, torch.Tensor], prefix: str, attn_bwd, rows: int,
+               aux=None):
     """Backward of one block; dx [rows, C] bf16 is d(loss)/d(block output).  Returns d(block input)."""
     (x, mean1, rstd1, h, qkv, att_saved, a, x1, mean2, rstd2, h2, pre, f1) = saved
-    C_, I = pk.C, pk.I
+    C_, I = layer.mlp.fc1.weight.shape[1], layer.mlp.fc1.weight.shape[0]
     dev = dx.device
     plain = ops.rowmap(C_)
     g = lambda n: grads[prefix + n]  # noqa: E731
     # ---- x_out = x1 + fc2(quick_gelu(fc1(LN2(x1))))
     ops.linear_wgrad(dx, f1, g("mlp.fc2.weight"))
     dpre = torch.empty(rows, I, dtype=bf16, device=dev)
-    ops.linear_dgrad(dx, pk.w2[i], dpre, act=_lib.ACT_DQUICK_GELU, aux=pre, ld_aux=I)
+    ops.linear_dgrad(dx, w[prefix + "mlp.fc2.weight"], dpre, act=_lib.ACT_DQUICK_GELU, aux=pre, ld_aux=I)
     _colsum(dpre, g("mlp.fc1.bias"), aux)
     ops.linear_wgrad(dpre, h2, g("mlp.fc1.weight"))
     dh2 = torch.empty(rows, C_, dtype=bf16, device=dev)
-    ops.linear_dgrad(dpre, pk.w1[i], dh2)
+    ops.linear_dgrad(dpre, w[prefix + "mlp.fc1.weight"], dh2)
     _join_aux(aux)          # dpre's column sum is complete: its memory may return to this stream's pool (see _colsum)
     del dpre
     dx1 = torch.empty(rows, C_, dtype=bf16, device=dev)
@@ -457,15 +410,13 @@ def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch
     # ---- x1 = x + out_proj(attn(qkv(LN1(x))))
     ops.linear_wgrad(dx1, a, g("self_attn.out_proj.weight"))
     da = dh2  # reuse
-    ops.linear_dgrad(dx1, pk.wo[i], da)
+    ops.linear_dgrad(dx1, w[prefix + "self_attn.out_proj.weight"], da)
     dqkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
     attn_bwd(qkv, a, da, att_saved, dqkv)
-    dwqkv = grads[prefix + "self_attn.qkv.weight"]
-    dbqkv = grads[prefix + "self_attn.qkv.bias"]
-    _colsum(dqkv, dbqkv, aux)
-    ops.linear_wgrad(dqkv, h, dwqkv)
+    _colsum(dqkv, g("self_attn.qkv.bias"), aux)
+    ops.linear_wgrad(dqkv, h, g("self_attn.qkv.weight"))
     dh = da
-    ops.linear_dgrad(dqkv, pk.wqkv[i], dh)
+    ops.linear_dgrad(dqkv, w[prefix + "self_attn.qkv.weight"], dh)
     _join_aux(aux)          # the qkv bias gradient is complete, and dqkv may be released
     del dqkv
     dxin = torch.empty(rows, C_, dtype=bf16, device=dev)
@@ -474,32 +425,13 @@ def _layer_bwd(dx, saved, layer, pk: _WeightPack, i: int, grads: Dict[str, torch
     return dxin
 
 
-def _alloc_layer_grads(layer, prefix: str, grads: Dict[str, torch.Tensor], dev) -> torch.Tensor:
-    C_ = layer.self_attn.q_proj.weight.shape[0]
-    shapes = {prefix + "self_attn.qkv.weight": (3 * C_, C_), prefix + "self_attn.qkv.bias": (3 * C_,)}
-    for n, p in layer.named_parameters():
-        if ".q_proj." in n or ".k_proj." in n or ".v_proj." in n:
-            continue
-        shapes[prefix + n] = tuple(p.shape)
-    return alloc_flat(shapes, grads, dev)
-
-
-def _grads_ready(model, grads: Dict[str, torch.Tensor], key: str) -> None:
+def _grads_ready(model, flat: torch.Tensor) -> None:
     """A gradient group (one encoder layer, or a tower's remaining parameters) is final: hand its flat buffer to
     `model.grad_ready_hook` (e.g. utils.distributed.OverlappedGradAverager, which starts an async NCCL all-reduce
     that overlaps with the rest of the backward pass — the hvd.DistributedOptimizer hooks of run_pretrain.py:226-228)."""
     hook = getattr(model, "grad_ready_hook", None)
-    flat = grads.get("__flat__" + key)
-    if hook is not None and flat is not None:
+    if hook is not None:
         hook(flat)
-
-
-def _finish_layer_grads(prefix: str, grads: Dict[str, torch.Tensor], C_: int):
-    w = grads.pop(prefix + "self_attn.qkv.weight")
-    b = grads.pop(prefix + "self_attn.qkv.bias")
-    for j, n in enumerate(("q_proj", "k_proj", "v_proj")):
-        grads[prefix + f"self_attn.{n}.weight"] = w[j * C_:(j + 1) * C_]
-        grads[prefix + f"self_attn.{n}.bias"] = b[j * C_:(j + 1) * C_]
 
 
 # ------------------------------------------------------------------------------ encoder stack
@@ -510,7 +442,7 @@ def _block_saved(sv, i: int):
     return s if sv.recompute is None else sv.recompute(i, s)
 
 
-def _encoder_fwd(model: CLIPModel, tower: str, pool_ln: str, pk: _WeightPack, x_in: list, rows: int, B: int, attn_fwd,
+def _encoder_fwd(model: CLIPModel, tower: str, pool_ln: str, w: ParamLayout, x_in: list, rows: int, B: int, attn_fwd,
                  pool_rows, wproj, save: bool, ckpt: bool, stream_dt, timer=None):
     """A tower's encoder layers, then its pooled LayerNorm (`pool_ln`) of the B rows picked by the row map `pool_rows()`
     returns after the layers, and the projection `wproj`.  x_in: a list holding the only reference to the embedded rows, so
@@ -527,13 +459,14 @@ def _encoder_fwd(model: CLIPModel, tower: str, pool_ln: str, pk: _WeightPack, x_
         if timer is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        x, pend, sv = _layer_fwd(x, pend, layer, pk, i, eps, attn_fwd, rows, save and not ckpt, stream_dt, keep_input=ckpt)
+        x, pend, sv = _layer_fwd(x, pend, layer, w, f"{tower}.encoder.layers.{i}.", eps, attn_fwd, rows, save and not ckpt,
+                                 stream_dt, keep_input=ckpt)
         if timer is not None:
             e1.record()
             timer.append(("fwd", e0, e1))
         layer_saved.append(sv)
     rmap = pool_rows()
-    pooled, meanp, rstdp, post_in = _pooled_ln(x, pend, rmap, getattr(tw, pool_ln), B, pk.C, eps)
+    pooled, meanp, rstdp, post_in = _pooled_ln(x, pend, rmap, getattr(tw, pool_ln), B, x.shape[1], eps)
     proj = torch.empty(B, model.config.projection_dim, dtype=f32, device=x.device)
     ops.linear_fwd(pooled, wproj, None, proj, out_mode=_lib.OUT_F32)
     if not save:
@@ -541,23 +474,25 @@ def _encoder_fwd(model: CLIPModel, tower: str, pool_ln: str, pk: _WeightPack, x_
     recompute = None
     if ckpt:
         def recompute(i, xin):
-            return _layer_fwd(xin, None, layers[i], pk, i, eps, attn_fwd, rows, True, stream_dt, upto_fc1=True)[2]
+            return _layer_fwd(xin, None, layers[i], w, f"{tower}.encoder.layers.{i}.", eps, attn_fwd, rows, True, stream_dt,
+                              upto_fc1=True)[2]
     return proj, SimpleNamespace(B=B, rows=rows, layers=layer_saved, x_last=(x, pend), pool_map=rmap, post_in=post_in,
                                  pooled=pooled, meanp=meanp, rstdp=rstdp, recompute=recompute)
 
 
-def _encoder_bwd(model: CLIPModel, tower: str, pool_ln: str, proj: str, pk: _WeightPack, sv, dproj_bf16, grads, wproj,
+def _encoder_bwd(model: CLIPModel, tower: str, pool_ln: str, proj: str, w: ParamLayout, sv, dproj_bf16, grads, flats,
                  attn_bwd, aux=None, timer=None):
     """Backward of _encoder_fwd from dproj_bf16 [B, proj] (the gradient of the un-normalised projection output): the
-    projection, the pooled LayerNorm, then the layers in reverse, each handing its finished gradient group to
-    `_grads_ready`.  aux: the stream of the layers' bias column sums (_colsum); timer: ("bwd", start, end) events per block.
+    projection, the pooled LayerNorm, then the layers in reverse, each handing its finished gradient group (its buffer in
+    `flats`) to `_grads_ready`.  aux: the stream of the layers' bias column sums (_colsum); timer: ("bwd", start, end) events
+    per block.
     Returns the gradient of the embedded rows [rows, C] bf16."""
     tw = getattr(model, tower)
-    C_, B, rows = pk.C, sv.B, sv.rows
+    C_, B, rows = getattr(tw, pool_ln).weight.shape[0], sv.B, sv.rows
     dev = dproj_bf16.device
     ops.linear_wgrad(dproj_bf16, sv.pooled, grads[proj + ".weight"])
     dpooled = torch.empty(B, C_, dtype=bf16, device=dev)
-    ops.linear_dgrad(dproj_bf16, wproj, dpooled)
+    ops.linear_dgrad(dproj_bf16, w[proj + ".weight"], dpooled)
     dx = torch.zeros(rows, C_, dtype=bf16, device=dev)  # only the pooled rows receive gradient from the head
     ln = f"{tower}.{pool_ln}."
     ops.layernorm_bwd(dpooled, ops.rowmap(C_), sv.post_in[0], sv.post_in[1], getattr(tw, pool_ln).weight, sv.meanp, sv.rstdp,
@@ -567,11 +502,11 @@ def _encoder_bwd(model: CLIPModel, tower: str, pool_ln: str, proj: str, pk: _Wei
         if timer is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        dx = _layer_bwd(dx, _block_saved(sv, i), tw.encoder.layers[i], pk, i, grads, prefix, attn_bwd, rows, aux)
+        dx = _layer_bwd(dx, _block_saved(sv, i), tw.encoder.layers[i], w, grads, prefix, attn_bwd, rows, aux)
         if timer is not None:
             e1.record()
             timer.append(("bwd", e0, e1))
-        _grads_ready(model, grads, prefix)
+        _grads_ready(model, flats[prefix])
     return dx
 
 
@@ -616,7 +551,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     S = M + T * L
     rows = B * S
     dev = video.device
-    pk = _pack(model, "vision")
+    w = param_layout(model)
     eps = cfg.layer_norm_eps
     Kp = 3 * cfg.patch_size * cfg.patch_size
     ldp = ops.patch_pitch(cfg.patch_size)    # patch-matrix row pitch: Kp rounded up to 8 columns, pad columns zero
@@ -635,7 +570,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     added = None if cfg.per_frame else emb.added_cls       # M = 1: the kernel reads no added_cls row
     ops.vip_embed_tables(emb.position_embedding.weight, temporal, emb.class_embedding, added, table, x0, B, T, L,
                          M, C_, cfg.temporal_size)
-    wp = _small_bf16(model, "patch").view(C_, Kp)
+    wp = w["vision_model.embeddings.patch_embedding.weight"].view(C_, Kp)
     if ldp != Kp:   # e.g. p = 14: the GEMM's B operand needs the same 16-byte row pitch as the patch matrix
         wpad = model._packs.get("pad:patch")
         if wpad is None or wpad.shape != (C_, ldp) or wpad.device != dev:
@@ -668,8 +603,8 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
         return lse
 
     # pooled = post_layernorm(last_hidden[:, 0])  (CLIP_ViP.py:891-893): CLS rows picked by the row map
-    proj, saved = _encoder_fwd(model, "vision_model", "post_layernorm", pk, x_in, rows, B, attn_fwd,
-                               lambda: ops.rowmap(C_, group=1, group_stride=S * C_), _small_bf16(model, "vproj"), save,
+    proj, saved = _encoder_fwd(model, "vision_model", "post_layernorm", w, x_in, rows, B, attn_fwd,
+                               lambda: ops.rowmap(C_, group=1, group_stride=S * C_), w["visual_projection.weight"], save,
                                ckpt, stream_dt, timer=getattr(model, "block_timer", None))  # bench.py: metric 2 of BASELINE.json
     if saved is not None:
         saved.T, saved.S, saved.patches, saved.x0, saved.ws = T, S, patches, x0, ws
@@ -677,7 +612,7 @@ def _vision_fwd(model: CLIPModel, video: torch.Tensor, save: bool, ckpt: bool = 
     return proj, saved
 
 
-def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, torch.Tensor]):
+def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, torch.Tensor], flats):
     """dproj_bf16 [B, proj] = gradient w.r.t. the un-normalised projection output."""
     cfg = model.config
     vm = model.vision_model
@@ -685,14 +620,13 @@ def _vision_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str,
     H = cfg.vision.num_attention_heads
     B, T, S = sv.B, sv.T, sv.S
     dev = dproj_bf16.device
-    pk = _pack(model, "vision")
     plain = ops.rowmap(C_)
 
     def attn_bwd(qkv, a, da, lse, dqkv):
-        ops.vip_attention_bwd(qkv, a, da, lse, dqkv, sv.ws, B, H, T, L, M, C_, pk.q_scale)
+        ops.vip_attention_bwd(qkv, a, da, lse, dqkv, sv.ws, B, H, T, L, M, C_, float(C_ // H) ** -0.5)
 
-    dx = _encoder_bwd(model, "vision_model", "post_layernorm", "visual_projection", pk, sv, dproj_bf16, grads,
-                      _small_bf16(model, "vproj"), attn_bwd, aux=_overlap_stream(model, dev, "overlap_colsum"),
+    dx = _encoder_bwd(model, "vision_model", "post_layernorm", "visual_projection", param_layout(model), sv, dproj_bf16,
+                      grads, flats, attn_bwd, aux=_overlap_stream(model, dev, "overlap_colsum"),
                       timer=getattr(model, "block_timer", None))
     # pre_layrnorm backward, written as two compact halves: patch rows [B, T*L, C] and global rows [B, M, C]
     d_patch = torch.empty(B * T * L, C_, dtype=bf16, device=dev)
@@ -755,24 +689,24 @@ def _text_fwd(model: CLIPModel, input_ids: torch.Tensor, attention_mask: Optiona
         ops.eos_offsets(ids, eos, None, C_)
         return ops.rowmap(C_, offsets=eos)
 
-    proj, saved = _encoder_fwd(model, "text_model", "final_layer_norm", _pack(model, "text"), x_in, rows, B, attn_fwd,
-                               eos_rows, _small_bf16(model, "tproj"), save, ckpt, stream_dt)
+    w = param_layout(model)
+    proj, saved = _encoder_fwd(model, "text_model", "final_layer_norm", w, x_in, rows, B, attn_fwd, eos_rows,
+                               w["text_projection.weight"], save, ckpt, stream_dt)
     if saved is not None:
         saved.Lt, saved.ids, saved.eos, saved.err = Lt, ids, eos, err
     return proj, saved
 
 
-def _text_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, torch.Tensor]):
+def _text_bwd(model: CLIPModel, dproj_bf16: torch.Tensor, sv, grads: Dict[str, torch.Tensor], flats):
     cfg = model.config
     C_, H = cfg.text.hidden_size, cfg.text.num_attention_heads
     B, Lt = sv.B, sv.Lt
-    pk = _pack(model, "text")
 
     def attn_bwd(qkv, a, da, probs, dqkv):
-        ops.text_attention_bwd(qkv, da, probs, dqkv, B, H, Lt, C_, pk.q_scale)
+        ops.text_attention_bwd(qkv, da, probs, dqkv, B, H, Lt, C_, float(C_ // H) ** -0.5)
 
-    dx = _encoder_bwd(model, "text_model", "final_layer_norm", "text_projection", pk, sv, dproj_bf16, grads,
-                      _small_bf16(model, "tproj"), attn_bwd)
+    dx = _encoder_bwd(model, "text_model", "final_layer_norm", "text_projection", param_layout(model), sv, dproj_bf16,
+                      grads, flats, attn_bwd)
     ops.text_embed_bwd(sv.ids, dx, grads["text_model.embeddings.token_embedding.weight"],
                        grads["text_model.embeddings.position_embedding.weight"], Lt, C_, cfg.vocab_size)
 
@@ -783,11 +717,11 @@ class _ClipVipFunction(torch.autograd.Function):
     def forward(ctx, model: CLIPModel, video, input_ids, attention_mask, normalize, grad_mode, *params):
         # grad_mode = torch.is_grad_enabled() of the caller (Function.forward itself always runs under no_grad, and
         # needs_input_grad reflects requires_grad even then): evaluation must not keep the activations alive
-        names = model._pnames
-        need = {n: r for n, r in zip(names, ctx.needs_input_grad[6:])}
+        w = param_layout(model)
+        need = {n: r for n, r in zip(w.names, ctx.needs_input_grad[6:])}
         save = grad_mode and any(need.values())
         ctx.model = model
-        _refresh_weights(model)
+        w.refresh()
         ctx.normalize = normalize
         ctx.vis = ctx.txt = None
         dev = params[0].device
@@ -848,12 +782,10 @@ class _ClipVipFunction(torch.autograd.Function):
     def backward(ctx, d_vis, d_txt):
         model: CLIPModel = ctx.model
         dev = model.logit_scale.device
-        names = model._pnames
-        named = dict(model.named_parameters())
-        grads: Dict[str, torch.Tensor] = {}
-        C_v, C_t = model.config.vision.hidden_size, model.config.text.hidden_size
-        jobs = (("vision_model", ctx.vis, d_vis, "visual_projection.weight", _vision_bwd, C_v),
-                ("text_model", ctx.txt, d_txt, "text_projection.weight", _text_bwd, C_t))
+        w = param_layout(model)
+        grads: Dict[str, torch.Tensor] = {}        # operand name -> gradient view
+        flats: Dict[str, torch.Tensor] = {}        # gradient group -> its flat buffer
+        jobs = (("vision_model", ctx.vis, d_vis, _vision_bwd), ("text_model", ctx.txt, d_txt, _text_bwd))
         main = torch.cuda.current_stream()
         side = ctx.side if (ctx.vis is not None and ctx.txt is not None and d_vis is not None and d_txt is not None) else None
         # data-parallel runs: leave `model.nccl_sm_reserve` SMs to the NCCL kernels of the overlapped gradient all-reduce for
@@ -863,20 +795,20 @@ class _ClipVipFunction(torch.autograd.Function):
             ops.set_sm_limit(torch.cuda.get_device_properties(dev).multi_processor_count - reserve)
         if side is not None:
             side.wait_stream(main)            # before any vision-backward launch: the text backward only needs d_txt
-        for tower, sv, dfeat, proj_name, bwd, C_ in jobs:
+        for tower, sv, dfeat, bwd in jobs:
             if sv is None or dfeat is None:
                 continue
             on_side = side is not None and tower == "text_model"
             if on_side:        # text backward on the side stream, under the vision backward (issued after it, see forward)
                 dfeat.record_stream(side)
                 with torch.cuda.stream(side):
-                    _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, names, named, dev)
+                    _tower_backward(model, ctx, w, tower, sv, dfeat, bwd, grads, flats, dev)
                 continue
-            _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, names, named, dev)
+            _tower_backward(model, ctx, w, tower, sv, dfeat, bwd, grads, flats, dev)
         if side is not None:
             main.wait_stream(side)
-            for k, t in grads.items():      # allocated in the side stream's pool, consumed by autograd on the main stream
-                if k.startswith("__flat__text_model"):
+            for k, t in flats.items():      # allocated in the side stream's pool, consumed by autograd on the main stream
+                if k.startswith("text_model"):
                     t.record_stream(main)
         hook = getattr(model, "grad_ready_hook", None)
         if hook is not None and hasattr(hook, "finish"):
@@ -884,18 +816,13 @@ class _ClipVipFunction(torch.autograd.Function):
         if reserve > 0:
             ops.set_sm_limit(0)
         ctx.vis = ctx.txt = None
-        return (None, None, None, None, None, None) + tuple(grads.get(n) if r else None
-                                                             for n, r in zip(names, ctx.needs_input_grad[6:]))
+        return (None, None, None, None, None, None) + w.grads_out(grads, ctx.needs_input_grad[6:])
 
 
-def _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, names, named, dev):
-    tw = getattr(model, tower)
-    for i, layer in enumerate(tw.encoder.layers):
-        pre = f"{tower}.encoder.layers.{i}."
-        grads["__flat__" + pre] = _alloc_layer_grads(layer, pre, grads, dev)
-    rest = {n: tuple(named[n].shape) for n in names if n.startswith(tower + ".") and ".encoder.layers." not in n}
-    rest[proj_name] = tuple(named[proj_name].shape)
-    grads["__flat__" + tower] = alloc_flat(rest, grads, dev)
+def _tower_backward(model, ctx, w: ParamLayout, tower, sv, dfeat, bwd, grads, flats, dev):
+    for key in w.groups:
+        if key.startswith(tower):
+            flats[key] = w.alloc_grads(key, grads)
     pool = getattr(sv, "pool", None)
     if pool is not None:        # frame-mean head: d(video feature) [B, P] -> d(frame projections) [B*T, P]
         proj, pool_t = pool
@@ -908,10 +835,8 @@ def _tower_backward(model, ctx, tower, sv, dfeat, proj_name, bwd, C_, grads, nam
             ops.l2norm_bwd(dfeat, sv.feat, sv.inv, dproj)
         else:
             dproj.copy_(dfeat)
-    bwd(model, dproj, sv, grads)
-    _grads_ready(model, grads, tower)
-    for i in range(len(tw.encoder.layers)):
-        _finish_layer_grads(f"{tower}.encoder.layers.{i}.", grads, C_)
+    bwd(model, dproj, sv, grads, flats)
+    _grads_ready(model, flats[tower])
 
 
 def _overlap_stream(model: CLIPModel, dev, option: str):
@@ -932,6 +857,6 @@ def _run(model: CLIPModel, video, input_ids, attention_mask, normalize: bool = T
         raise _lib.XpError("xpretrain_b200.CLIPModel must live on a CUDA (H100) device: there is no CPU path")
     if video is not None:
         _frame_path(model.config, video)
-    params = [p for n, p in model.named_parameters() if n != "logit_scale"]
-    vis, txt = _ClipVipFunction.apply(model, video, input_ids, attention_mask, normalize, torch.is_grad_enabled(), *params)
+    vis, txt = _ClipVipFunction.apply(model, video, input_ids, attention_mask, normalize, torch.is_grad_enabled(),
+                                      *param_layout(model).params)
     return (vis if video is not None else None), (txt if input_ids is not None else None)

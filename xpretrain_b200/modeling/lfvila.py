@@ -27,13 +27,10 @@ import torch
 import torch.nn as nn
 
 from .. import _lib, ops
-from ._blocks import alloc_flat
-from ._weights import WeightMirror
+from ._weights import ParamLayout, param_layout
 from .swin3d import SwinTransformer3D
 
 bf16, f32 = torch.bfloat16, torch.float32
-_HEAD = ("video_global_proj.weight", "video_global_proj.bias", "video_frame_proj.weight", "video_frame_proj.bias",
-         "classifier.weight", "classifier.bias")
 
 
 def _get(obj, key, default=None):
@@ -58,7 +55,12 @@ class LFVILA_Video_Classification(nn.Module):
         self.video_frame_proj = nn.Linear(hidden, hidden)
         self.n_labels = int(_get(_get(config, "DATA"), "classification_labels"))
         self.classifier = nn.Linear(hidden, self.n_labels)
-        self._head: Dict[str, object] = {}
+
+    def _declare_layout(self) -> ParamLayout:
+        """The head's parameters (the encoder has its own layout): bf16 copies of the three weights, the classifier's and
+        its fp32 bias padded with zero rows to a multiple of 8 labels (the GEMM's N alignment); one gradient group."""
+        return ParamLayout(self, exclude=("video_encoder.",), cast=lambda n, p: n.endswith(".weight") or n == "classifier.bias",
+                           pad8=("classifier.weight", "classifier.bias"))
 
     def forward(self, video_frames: torch.Tensor, labels=None):
         if not isinstance(labels, torch.Tensor):
@@ -72,28 +74,9 @@ class LFVILA_Video_Classification(nn.Module):
             raise ValueError(f"labels must be int64 class indices of shape [{video_frames.shape[0]}] (got {labels.dtype} "
                              f"{list(labels.shape)})")
         video_embd, _ = self.video_encoder(video_frames)                  # [B, N, H, W, C]
-        params = [dict(self.named_parameters())[n] for n in _HEAD]
         g, fr, pred, loss, acc = _HeadFunction.apply(self, torch.is_grad_enabled(), video_embd,
-                                                     labels.to(video_embd.device), *params)
+                                                     labels.to(video_embd.device), *param_layout(self).params)
         return dict(video_global_feat=g, video_frame_feat=fr, prediction=pred, loss=loss, acc=acc)
-
-
-def _head_weights(model: LFVILA_Video_Classification):
-    """bf16 compute copies of the three head weights (the classifier's padded with zero rows to a multiple of 8) and the
-    classifier bias padded with zeros, re-cast on every forward by one launch (modeling/_weights.py)."""
-    dev = model.classifier.weight.device
-    h = model._head
-    if h.get("device") != dev:
-        C, n = model.classifier.weight.shape[1], model.n_labels
-        n_pad = (n + 7) // 8 * 8
-        h.clear()
-        h.update(device=dev, mirror=WeightMirror(), n_pad=n_pad,
-                 wg=torch.empty(C, C, dtype=bf16, device=dev), wf=torch.empty(C, C, dtype=bf16, device=dev),
-                 wc=torch.zeros(n_pad, C, dtype=bf16, device=dev), bc=torch.zeros(n_pad, dtype=f32, device=dev))
-    n = model.n_labels
-    h["mirror"].refresh([(model.video_global_proj.weight, h["wg"]), (model.video_frame_proj.weight, h["wf"]),
-                         (model.classifier.weight, h["wc"][:n]), (model.classifier.bias, h["bc"][:n])])
-    return h
 
 
 class _HeadFunction(torch.autograd.Function):
@@ -104,8 +87,9 @@ class _HeadFunction(torch.autograd.Function):
         B, N, Hp, Wp, C = x.shape
         dev = x.device
         X = max(Hp - 1, 0) * max(Wp - 2, 0)
-        h = _head_weights(model)
-        n, n_pad = model.n_labels, h["n_pad"]
+        w = param_layout(model)
+        w.refresh()
+        n, n_pad = model.n_labels, w["classifier.weight"].shape[0]
         frame_raw = torch.empty(B * N, C, dtype=f32, device=dev)
         frame_bf = torch.empty(B * N, C, dtype=bf16, device=dev)
         global_raw = torch.empty(B, C, dtype=f32, device=dev)
@@ -113,16 +97,16 @@ class _HeadFunction(torch.autograd.Function):
         argmax = torch.empty(B, N, X, C, dtype=torch.uint8, device=dev)
         ops.lfvila_pool_fwd(x, frame_raw, frame_bf, global_raw, global_bf, argmax)
         gproj = torch.empty(B, C, dtype=f32, device=dev)
-        ops.linear_fwd(global_bf, h["wg"], model.video_global_proj.bias, gproj, out_mode=_lib.OUT_F32)
+        ops.linear_fwd(global_bf, w["video_global_proj.weight"], model.video_global_proj.bias, gproj, out_mode=_lib.OUT_F32)
         fproj = torch.empty(B * N, C, dtype=f32, device=dev)
-        ops.linear_fwd(frame_bf, h["wf"], model.video_frame_proj.bias, fproj, out_mode=_lib.OUT_F32)
+        ops.linear_fwd(frame_bf, w["video_frame_proj.weight"], model.video_frame_proj.bias, fproj, out_mode=_lib.OUT_F32)
         gfeat, gfeat_bf, gnorm = torch.empty_like(gproj), torch.empty(B, C, dtype=bf16, device=dev), gproj.new_empty(B)
         ops.lfvila_normalize_fwd(gproj, gfeat, gfeat_bf, gnorm)
         ffeat, fnorm = torch.empty_like(fproj), fproj.new_empty(B * N)
         ops.lfvila_normalize_fwd(fproj, ffeat, None, fnorm)
         del gproj, fproj
         logits = torch.empty(B, n_pad, dtype=f32, device=dev)
-        ops.linear_fwd(gfeat_bf, h["wc"], h["bc"], logits, out_mode=_lib.OUT_F32)
+        ops.linear_fwd(gfeat_bf, w["classifier.weight"], w["classifier.bias"], logits, out_mode=_lib.OUT_F32)
         pred = torch.empty(B, n, dtype=f32, device=dev)
         lse, loss, acc = logits.new_empty(B), logits.new_empty(()), logits.new_empty(1)
         ops.lfvila_ce_fwd(logits, n, labels, pred, lse, loss, acc)
@@ -140,13 +124,10 @@ class _HeadFunction(torch.autograd.Function):
         ctx.saved = None
         (B, N, Hp, Wp, C), xdt = ctx.x_meta
         dev = logits.device
-        h = model._head
-        n, n_pad = model.n_labels, h["n_pad"]
-        named = dict(model.named_parameters())
+        w = param_layout(model)
+        n, n_pad = model.n_labels, w["classifier.weight"].shape[0]
         grads: Dict[str, torch.Tensor] = {}
-        shapes = {k: tuple(named[k].shape) for k in _HEAD if not k.startswith("classifier.")}
-        shapes.update({"classifier.weight": (n_pad, C), "classifier.bias": (n_pad,)})   # padded: the GEMMs write n_pad rows
-        alloc_flat(shapes, grads, dev)
+        w.alloc_grads("", grads)                  # the classifier's padded: the GEMMs write n_pad rows
         d_global = d_frame = None
         # classifier, from the loss and / or a gradient of `prediction`
         d_class = None
@@ -156,7 +137,7 @@ class _HeadFunction(torch.autograd.Function):
             ops.linear_wgrad(dlog, gfeat_bf, grads["classifier.weight"])
             ops.colsum(dlog, grads["classifier.bias"])
             d_class = torch.empty(B, C, dtype=f32, device=dev)
-            ops.linear_dgrad(dlog, h["wc"], d_class, out_mode=_lib.OUT_F32)
+            ops.linear_dgrad(dlog, w["classifier.weight"], d_class, out_mode=_lib.OUT_F32)
         # video_global_proj + normalize, from the classifier and / or a gradient of `video_global_feat`
         if d_class is not None or d_gfeat is not None:
             dg = torch.empty(B, C, dtype=bf16, device=dev)
@@ -164,7 +145,7 @@ class _HeadFunction(torch.autograd.Function):
             ops.linear_wgrad(dg, global_bf, grads["video_global_proj.weight"])
             ops.colsum(dg, grads["video_global_proj.bias"])
             d_global = torch.empty(B, C, dtype=f32, device=dev)
-            ops.linear_dgrad(dg, h["wg"], d_global, out_mode=_lib.OUT_F32)
+            ops.linear_dgrad(dg, w["video_global_proj.weight"], d_global, out_mode=_lib.OUT_F32)
         # video_frame_proj + normalize, from a gradient of `video_frame_feat` (no loss uses it)
         if d_ffeat is not None:
             df = torch.empty(B * N, C, dtype=bf16, device=dev)
@@ -172,11 +153,9 @@ class _HeadFunction(torch.autograd.Function):
             ops.linear_wgrad(df, frame_bf, grads["video_frame_proj.weight"])
             ops.colsum(df, grads["video_frame_proj.bias"])
             d_frame = torch.empty(B * N, C, dtype=f32, device=dev)
-            ops.linear_dgrad(df, h["wf"], d_frame, out_mode=_lib.OUT_F32)
+            ops.linear_dgrad(df, w["video_frame_proj.weight"], d_frame, out_mode=_lib.OUT_F32)
         dx = None
         if ctx.needs_input_grad[2]:
             dx = torch.empty(B, N, Hp, Wp, C, dtype=xdt, device=dev)
             ops.lfvila_pool_bwd(d_frame, d_global, argmax, dx)
-        grads["classifier.weight"] = grads["classifier.weight"][:n]
-        grads["classifier.bias"] = grads["classifier.bias"][:n]
-        return (None, None, dx, None) + tuple(grads[k] if ctx.needs_input_grad[4 + j] else None for j, k in enumerate(_HEAD))
+        return (None, None, dx, None) + w.grads_out(grads, ctx.needs_input_grad[4:])

@@ -26,15 +26,15 @@ from __future__ import annotations
 
 from functools import reduce
 from operator import mul
-from typing import Dict, List, NamedTuple
+from typing import Dict, NamedTuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib, ops
-from ._blocks import alloc_flat, drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd, residual_linear
-from ._weights import refresh_weights, weight
+from ._blocks import drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd, residual_linear
+from ._weights import ParamLayout, matrix_weight, param_layout
 
 bf16, f32 = torch.bfloat16, torch.float32
 HEAD_DIM = 32
@@ -129,7 +129,6 @@ class SwinTransformer3D(nn.Module):
         self.norm = nn.LayerNorm(self.num_features)
         self.norm_local = nn.LayerNorm(self.num_features)                 # never reaches the output (:600)
         self.local_feat_proj = _PatchMerging(embed_dim * 2 ** 2)         # idem (:545)
-        self._cache: Dict[str, list] = {}
         self._tables: Dict[tuple, tuple] = {}
         self.forced_drop_masks = None
         self.init_weights()
@@ -146,6 +145,10 @@ class SwinTransformer3D(nn.Module):
                 nn.init.zeros_(m.bias)
             elif isinstance(m, _WindowAttention3D):
                 nn.init.trunc_normal_(m.relative_position_bias_table, std=.02)
+
+    def _declare_layout(self) -> ParamLayout:
+        """bf16 copies of the GEMM weights, one gradient group; `norm_local` / `local_feat_proj` are left out."""
+        return ParamLayout(self, exclude=("norm_local.", "local_feat_proj."), cast=matrix_weight)
 
     def draw_drop_masks(self, B: int, device, dtype):
         """Per block: the attention-branch factor then the MLP-branch factor, each floor(keep + U[0,1)) / keep of shape [B]
@@ -169,11 +172,9 @@ class SwinTransformer3D(nn.Module):
         if self.training and self.drop_path_rate > 0:
             masks = self.forced_drop_masks if self.forced_drop_masks is not None else \
                 self.draw_drop_masks(x.shape[0], x.device, x.dtype)
-        names, params = zip(*[(n, p) for n, p in self.named_parameters()
-                              if not n.startswith(("norm_local.", "local_feat_proj."))])
         # torch.is_grad_enabled() of the caller: Function.forward always runs under no_grad, and needs_input_grad reflects
         # requires_grad even then, so without it evaluation under torch.no_grad() would keep every activation to the end
-        out = _Swin3DFunction.apply(self, list(names), masks, torch.is_grad_enabled(), x, *params)
+        out = _Swin3DFunction.apply(self, masks, torch.is_grad_enabled(), x, *param_layout(self).params)
         return out, out
 
 
@@ -264,7 +265,7 @@ class _WindowSaved(NamedTuple):
     bias: torch.Tensor       # relative-position bias (+ shift mask) slab [nW, heads, L, L]
 
 
-def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, save: bool, scales, B: int):
+def _block_fwd(w, p: str, blk: _Block, x, geo, shifted: bool, heads: int, save: bool, scales, B: int):
     """SwinTransformerBlock3D.forward :248-268 on tokens x [n_real, C]."""
     C_ = x.shape[1]
     dev = x.device
@@ -277,7 +278,7 @@ def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, sa
         h[n_real:].zero_()
     _, mean1, rstd1 = layernorm(x, blk.norm1, wide=True, out=h)
     qkv = torch.empty(n_ext, 3 * C_, dtype=bf16, device=dev)
-    ops.linear_fwd(h, weight(model, p + "attn.qkv.weight"), blk.attn.qkv.bias, qkv, scale_cols=C_,
+    ops.linear_fwd(h, w[p + "attn.qkv.weight"], blk.attn.qkv.bias, qkv, scale_cols=C_,
                    col_scale=HEAD_DIM ** -0.5)                            # q * scale (:145), bias included
     # relative-position bias (+ shift mask) slab [nW, heads, L, L]
     tab = blk.attn.relative_position_bias_table.detach()
@@ -291,24 +292,24 @@ def _block_fwd(model, p: str, blk: _Block, x, geo, shifted: bool, heads: int, sa
     desc = ops.window_desc(n_ext, heads, HEAD_DIM, 3 * C_, C_, idx, bias)
     ops.seg_attention_fwd(qkv, a, lse, desc)
     # proj on the real rows (the crop of :242-243), residual + drop_path (:260)
-    x1 = residual_linear(model, p + "attn.proj", blk.attn.proj, a[:n_real], x, s_a)
-    out, mlp = mlp_fwd(model, p, blk, x1, save, s_m, wide=True)
+    x1 = residual_linear(w, p + "attn.proj", blk.attn.proj, a[:n_real], x, s_a)
+    out, mlp = mlp_fwd(w, p, blk, x1, save, s_m, wide=True)
     return out, ((_WindowSaved(x, mean1, rstd1, h, qkv, a, lse, bias), mlp) if save else None)
 
 
-def _block_bwd(model, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads: int, grads, scales):
+def _block_bwd(w, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads: int, grads, scales):
     win, mlp = saved
     C_ = dx.shape[1]
     dev = dx.device
     n_real, n_pad, L = geo["n_real"], geo["n_pad"], geo["L"]
     n_ext = n_real + n_pad
     s_a, s_m = scales if scales is not None else (None, None)
-    dx1 = mlp_bwd(model, p, blk, dx, mlp, grads, s_m, wide=True)
+    dx1 = mlp_bwd(w, p, blk, dx, mlp, grads, s_m, wide=True)
     # ---- x1 = x + drop_path(proj(window_attention(LN(x))))
     da = torch.empty(n_ext, C_, dtype=bf16, device=dev)
     if n_pad:
         da[n_real:].zero_()                                               # outputs at padded positions are cropped away
-    linear_bwd(model, p + "attn.proj", drop_scale(dx1, s_a), win.a[:n_real], grads, out=da[:n_real])
+    linear_bwd(w, p + "attn.proj", drop_scale(dx1, s_a), win.a[:n_real], grads, out=da[:n_real])
     idx = geo["idx"][1 if shifted else 0]
     ds = torch.empty(idx.shape[0], heads, L, L, dtype=bf16, device=dev)
     dqkv = torch.empty(n_ext, 3 * C_, dtype=bf16, device=dev)
@@ -325,20 +326,21 @@ def _block_bwd(model, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads:
     grads[p + "attn.relative_position_bias_table"].index_add_(0, ridx, dbias.view(heads, L * L).t())
     del ds
     # qkv Linear over real + padded rows (padded inputs are zero: they only reach the bias)
-    dh = linear_bwd(model, p + "attn.qkv", dqkv, win.h, grads)
+    dh = linear_bwd(w, p + "attn.qkv", dqkv, win.h, grads)
     return layernorm_bwd(dh[:n_real], win.x, blk.norm1, win.mean, win.rstd, dx1, grads, p + "norm1", wide=True)
 
 
 # ------------------------------------------------------------------------------------------- function
 class _Swin3DFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, model: SwinTransformer3D, names: List[str], masks, grad_mode: bool, video: torch.Tensor, *params):
+    def forward(ctx, model: SwinTransformer3D, masks, grad_mode: bool, video: torch.Tensor, *params):
         B, Cin, D, Hin, Win = video.shape
         ph, pw = model.patch_size[1], model.patch_size[2]
         if Cin != 3 or Hin % ph or Win % pw:
             raise ValueError("video must be [B, 3, D, H, W] with H, W divisible by the patch size")
-        save = grad_mode and any(ctx.needs_input_grad[5:])
-        refresh_weights(model)
+        save = grad_mode and any(ctx.needs_input_grad[4:])
+        w = param_layout(model)
+        w.refresh()
         dev = video.device
         C0 = model.embed_dim
         # ---- PatchEmbed3D (:431-448): frames x (h, w) patches, rows already in (b, d, h, w) order
@@ -350,7 +352,7 @@ class _Swin3DFunction(torch.autograd.Function):
         if ph != pw:
             raise NotImplementedError("square spatial patches only")
         ops.vip_patchify(frames, patches, ph)
-        w0 = weight(model, "patch_embed.proj.weight").view(C0, K0)
+        w0 = w["patch_embed.proj.weight"].view(C0, K0)
         tok = torch.empty(rows, C0, dtype=bf16, device=dev)
         ops.linear_fwd(patches, w0, model.patch_embed.proj.bias, tok)
         pe_saved = None
@@ -371,7 +373,7 @@ class _Swin3DFunction(torch.autograd.Function):
                     per_sample = D * H * W
                     scales = tuple(m.repeat_interleave(per_sample).contiguous() for m in masks[k])
                 shifted = (j % 2 == 1) and any(s > 0 for s in geo["ss"])
-                tok, sv = _block_fwd(model, f"layers.{i}.blocks.{j}.", blk, tok, geo, shifted, heads, save, scales, B)
+                tok, sv = _block_fwd(w, f"layers.{i}.blocks.{j}.", blk, tok, geo, shifted, heads, save, scales, B)
                 blocks_saved.append((sv, shifted, scales))
                 k += 1
             merge_saved = None
@@ -383,7 +385,7 @@ class _Swin3DFunction(torch.autograd.Function):
                 ops.gather_rows(tok, midx, cat, C_)
                 catn, mm, mr = layernorm(cat, layer.downsample.norm, wide=True)
                 red = torch.empty(n_out, 2 * C_, dtype=bf16, device=dev)
-                ops.linear_fwd(catn, weight(model, f"layers.{i}.downsample.reduction.weight"), None, red)
+                ops.linear_fwd(catn, w[f"layers.{i}.downsample.reduction.weight"], None, red)
                 merge_saved = (cat, mm, mr, catn, midx, rows, C_)
                 tok, H, W, rows = red, H2, W2, n_out
             layer_saved.append((blocks_saved, merge_saved))
@@ -392,20 +394,20 @@ class _Swin3DFunction(torch.autograd.Function):
         outn, fm, fr = layernorm(tok, model.norm, wide=True)
         out = outn.view(B, D, H, W, Cl).to(video.dtype)
         if save:
-            ctx.model, ctx.names, ctx.geos = model, names, geos
+            ctx.model, ctx.geos = model, geos
             ctx.saved = (patches, pe_saved, layer_saved, (tok, fm, fr))
             ctx.dims = (B, D, H, W, Cl)
         return out
 
     @staticmethod
     def backward(ctx, d_out):
-        model, names, geos = ctx.model, ctx.names, ctx.geos
+        model, geos = ctx.model, ctx.geos
+        w = param_layout(model)
         patches, pe_saved, layer_saved, (tok_last, fm, fr) = ctx.saved
         B, D, H, W, Cl = ctx.dims
         dev = d_out.device
-        named = dict(model.named_parameters())
         grads: Dict[str, torch.Tensor] = {}
-        alloc_flat({n: tuple(named[n].shape) for n in names}, grads, dev)
+        w.alloc_grads("", grads)
         dy = d_out.reshape(B * D * H * W, Cl).to(bf16).contiguous()
         dtok = layernorm_bwd(dy, tok_last, model.norm, fm, fr, None, grads, "norm", wide=True)
         for i in reversed(range(model.num_layers)):
@@ -417,14 +419,14 @@ class _Swin3DFunction(torch.autograd.Function):
                 name = f"layers.{i}.downsample."
                 ops.linear_wgrad(dtok, catn, grads[name + "reduction.weight"])
                 dcatn = torch.empty(n_out, 4 * C_, dtype=bf16, device=dev)
-                ops.linear_dgrad(dtok, weight(model, name + "reduction.weight"), dcatn)
+                ops.linear_dgrad(dtok, w[name + "reduction.weight"], dcatn)
                 dcat = layernorm_bwd(dcatn, cat, layer.downsample.norm, mm, mr, None, grads, name + "norm", wide=True)
                 dtok = torch.empty(rows_in, C_, dtype=bf16, device=dev)
                 ops.scatter_rows(dcat, midx, dtok, C_)                    # every input row occurs exactly once
             heads = model.num_heads[i]
             for j in reversed(range(len(layer.blocks))):
                 sv, shifted, scales = blocks_saved[j]
-                dtok = _block_bwd(model, f"layers.{i}.blocks.{j}.", layer.blocks[j], dtok, sv, geos[i], shifted, heads, grads,
+                dtok = _block_bwd(w, f"layers.{i}.blocks.{j}.", layer.blocks[j], dtok, sv, geos[i], shifted, heads, grads,
                                   scales)
                 blocks_saved[j] = None
         # ---- PatchEmbed3D
@@ -435,5 +437,4 @@ class _Swin3DFunction(torch.autograd.Function):
         ops.linear_wgrad(dtok, patches, grads["patch_embed.proj.weight"].view(C0, -1))
         ops.colsum(dtok, grads["patch_embed.proj.bias"])
         ctx.saved = None
-        return (None, None, None, None, None) + tuple(grads[n] if ctx.needs_input_grad[5 + j] else None
-                                                      for j, n in enumerate(names))
+        return (None, None, None, None) + w.grads_out(grads, ctx.needs_input_grad[4:])

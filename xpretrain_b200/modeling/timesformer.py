@@ -30,16 +30,15 @@ There is no CPU path.
 from __future__ import annotations
 
 import math
-from typing import Dict, List, NamedTuple, Optional
+from typing import Dict, NamedTuple, Optional
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib, ops
-from ._blocks import (MlpSaved, alloc_flat, drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd,
-                      residual_linear)
-from ._weights import refresh_weights, weight
+from ._blocks import MlpSaved, drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd, residual_linear
+from ._weights import ParamLayout, matrix_weight, param_layout
 
 bf16, f32 = torch.bfloat16, torch.float32
 ATTENTION_TYPES = ('divided_space_time', 'space_only', 'joint_space_time')
@@ -97,7 +96,6 @@ class TimeSformer(nn.Module):
         divided = attention_type == 'divided_space_time'
         self.blocks = nn.ModuleList([_TsfBlock(embed_dim, hidden, qkv_bias, self.eps, divided) for _ in range(depth)])
         self.norm = nn.LayerNorm(embed_dim, eps=self.eps)   # constructed, never applied (timesformer.py:451)
-        self._cache: Dict[str, list] = {}
         self.forced_drop_masks = None     # tests: per-block (m_t, m_s, m_m) factors instead of fresh random draws
         self._init_weights()
 
@@ -117,6 +115,12 @@ class TimeSformer(nn.Module):
             if i > 0 and self.attention_type == 'divided_space_time':
                 nn.init.zeros_(blk.temporal_fc.weight)
                 nn.init.zeros_(blk.temporal_fc.bias)
+
+    def _declare_layout(self) -> ParamLayout:
+        """bf16 copies of the GEMM weights, one gradient group per block; the never-applied `norm` is left out, and the
+        pos_embed / time_embed gradients come from the table interpolation's own backward."""
+        return ParamLayout(self, exclude=("norm.",), cast=matrix_weight,
+                           group=lambda op: ".".join(op.split(".")[:2]) if op.startswith("blocks.") else None)
 
     @torch.jit.ignore
     def no_weight_decay(self):
@@ -151,8 +155,9 @@ class TimeSformer(nn.Module):
             B, T, _, H, W = x.shape
             masks = self.forced_drop_masks if self.forced_drop_masks is not None else \
                 self.draw_drop_masks(B, T, H, W, x.device, x.dtype)
-        names, params = zip(*[(n, p) for n, p in self.named_parameters() if not n.startswith("norm.")])
-        return _TimeSformerFunction.apply(self, list(names), masks, x, *params)
+        # torch.is_grad_enabled() of the caller: Function.forward always runs under no_grad, and needs_input_grad reflects
+        # requires_grad even then, so without it evaluation under torch.no_grad() would keep every activation to the end
+        return _TimeSformerFunction.apply(self, masks, torch.is_grad_enabled(), x, *param_layout(self).params)
 
 
 # ----------------------------------------------------------------------------------- helpers
@@ -201,7 +206,7 @@ class _BlockSaved(NamedTuple):
     mlp: MlpSaved
 
 
-def _attn_fwd(model: TimeSformer, i: int, half: str, x, desc) -> _AttnSaved:
+def _attn_fwd(model: TimeSformer, w, i: int, half: str, x, desc) -> _AttnSaved:
     """LayerNorm -> fused qkv GEMM -> attention of block i's temporal (half 'temporal_') or spatial / dense (half '') part.
     The kernel follows the descriptor: seg attention (temporal, spatial) or dense attention (joint, space-only)."""
     blk, p = model.blocks[i], f"blocks.{i}.{half}attn."
@@ -211,7 +216,7 @@ def _attn_fwd(model: TimeSformer, i: int, half: str, x, desc) -> _AttnSaved:
     h, mean, rstd = layernorm(x, getattr(blk, half + "norm1"))
     qkv = torch.empty(rows, 3 * C_, dtype=bf16, device=dev)
     # (q k^T) * head_dim**-0.5 (timesformer.py:165): 0.125 is a power of two, folding it into q (bias included) is exact
-    ops.linear_fwd(h, weight(model, p + "qkv.weight"), att.qkv.bias, qkv, scale_cols=C_, col_scale=0.125)
+    ops.linear_fwd(h, w[p + "qkv.weight"], att.qkv.bias, qkv, scale_cols=C_, col_scale=0.125)
     a = torch.empty(rows, C_, dtype=bf16, device=dev)
     lse = torch.empty(model.num_heads, rows, dtype=f32, device=dev)
     if isinstance(desc, _lib.XpDenseAttn):
@@ -221,7 +226,7 @@ def _attn_fwd(model: TimeSformer, i: int, half: str, x, desc) -> _AttnSaved:
     return _AttnSaved(x, mean, rstd, h, qkv, a, lse)
 
 
-def _attn_bwd(model: TimeSformer, i: int, half: str, da, sv: _AttnSaved, desc, grads, dres):
+def _attn_bwd(model: TimeSformer, w, i: int, half: str, da, sv: _AttnSaved, desc, grads, dres):
     """Backward of _attn_fwd from the gradient of the attention output; dres is the gradient carried by the residual path
     around this part.  Returns the gradient of the part's input."""
     blk, p = model.blocks[i], f"blocks.{i}.{half}"
@@ -232,11 +237,11 @@ def _attn_bwd(model: TimeSformer, i: int, half: str, da, sv: _AttnSaved, desc, g
         ops.dense_attention_bwd(sv.qkv, sv.a, da, sv.lse, delta, dqkv, desc, 0.125)
     else:
         ops.seg_attention_bwd(sv.qkv, sv.a, da, sv.lse, delta, dqkv, desc, 0.125)
-    dh = linear_bwd(model, p + "attn.qkv", dqkv, sv.h, grads)
+    dh = linear_bwd(w, p + "attn.qkv", dqkv, sv.h, grads)
     return layernorm_bwd(dh, sv.x, getattr(blk, half + "norm1"), sv.mean, sv.rstd, dres, grads, p + "norm1")
 
 
-def _block_fwd(model: TimeSformer, i: int, x, descs, save: bool, scales=None):
+def _block_fwd(model: TimeSformer, w, i: int, x, descs, save: bool, scales=None):
     """timesformer.py:207-226.  x: [rows, C] bf16 tokens, (h w t) order.  descs: (temporal, spatial) attention descriptors
     of 'divided_space_time', or (None, dense) for 'joint_space_time' / 'space_only' (:202-205), whose blocks have no temporal
     part.  scales: per-row DropPath factors (temporal, attention, mlp) of this block or None."""
@@ -247,48 +252,49 @@ def _block_fwd(model: TimeSformer, i: int, x, descs, save: bool, scales=None):
     temporal = p_t = None
     if d_t is not None:
         # ---- temporal attention -> proj -> drop_path -> temporal_fc -> residual (:209-214)
-        temporal = _attn_fwd(model, i, "temporal_", x, d_t)
+        temporal = _attn_fwd(model, w, i, "temporal_", x, d_t)
         p_t = torch.empty(x.shape[0], C_, dtype=bf16, device=x.device)
-        ops.linear_fwd(temporal.a, weight(model, p + "temporal_attn.proj.weight"), blk.temporal_attn.proj.bias, p_t)
+        ops.linear_fwd(temporal.a, w[p + "temporal_attn.proj.weight"], blk.temporal_attn.proj.bias, p_t)
         if s_t is not None:
             ops.rowscale(p_t, s_t, p_t)          # in place: the saved p_t is the dropped one, as temporal_fc consumed it
         xt = torch.empty(x.shape[0], C_, dtype=bf16, device=x.device)
-        ops.linear_fwd(p_t, weight(model, p + "temporal_fc.weight"), blk.temporal_fc.bias, xt, residual=x, ldr=C_)
+        ops.linear_fwd(p_t, w[p + "temporal_fc.weight"], blk.temporal_fc.bias, xt, residual=x, ldr=C_)
         x = xt
     # ---- spatial / dense attention -> proj -> drop_path -> residual (:216-224, :202-204)
-    attn = _attn_fwd(model, i, "", x, d_a)
-    x2 = residual_linear(model, p + "attn.proj", blk.attn.proj, attn.a, x, s_a)
+    attn = _attn_fwd(model, w, i, "", x, d_a)
+    x2 = residual_linear(w, p + "attn.proj", blk.attn.proj, attn.a, x, s_a)
     # ---- MLP with exact-erf GELU (:225, :132-138)
-    out, mlp = mlp_fwd(model, p, blk, x2, save, s_m)
+    out, mlp = mlp_fwd(w, p, blk, x2, save, s_m)
     return out, (_BlockSaved(temporal, p_t, attn, mlp) if save else None)
 
 
-def _block_bwd(model: TimeSformer, i: int, dx, saved: _BlockSaved, descs, grads, scales=None):
+def _block_bwd(model: TimeSformer, w, i: int, dx, saved: _BlockSaved, descs, grads, scales=None):
     blk, p = model.blocks[i], f"blocks.{i}."
     s_t, s_a, s_m = scales if scales is not None else (None, None, None)
-    dx2 = mlp_bwd(model, p, blk, dx, saved.mlp, grads, s_m)
+    dx2 = mlp_bwd(w, p, blk, dx, saved.mlp, grads, s_m)
     # ---- x2 = xt + drop_path(proj(attn(LN(xt))))
-    da = linear_bwd(model, p + "attn.proj", drop_scale(dx2, s_a), saved.attn.a, grads)
-    dxt = _attn_bwd(model, i, "", da, saved.attn, descs[1], grads, dx2)
+    da = linear_bwd(w, p + "attn.proj", drop_scale(dx2, s_a), saved.attn.a, grads)
+    dxt = _attn_bwd(model, w, i, "", da, saved.attn, descs[1], grads, dx2)
     if saved.temporal is None:
         return dxt
     # ---- xt = x + temporal_fc(drop_path(proj_t(attn_t(LN(x)))))   (the saved p_t is already the dropped one)
-    dp_t = linear_bwd(model, p + "temporal_fc", dxt, saved.p_t, grads)
+    dp_t = linear_bwd(w, p + "temporal_fc", dxt, saved.p_t, grads)
     if s_t is not None:
         ops.rowscale(dp_t, s_t, dp_t)
-    da_t = linear_bwd(model, p + "temporal_attn.proj", dp_t, saved.temporal.a, grads)
-    return _attn_bwd(model, i, "temporal_", da_t, saved.temporal, descs[0], grads, dxt)
+    da_t = linear_bwd(w, p + "temporal_attn.proj", dp_t, saved.temporal.a, grads)
+    return _attn_bwd(model, w, i, "temporal_", da_t, saved.temporal, descs[0], grads, dxt)
 
 
 class _TimeSformerFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, model: TimeSformer, names: List[str], masks, x: torch.Tensor, *params):
+    def forward(ctx, model: TimeSformer, masks, grad_mode: bool, x: torch.Tensor, *params):
         B, T, C_, H, W = x.shape
         if C_ != model.embed_dim:
             raise ValueError(f"expected {model.embed_dim} channels, got {C_}")
         HW, rows = H * W, B * H * W * T
-        save = any(ctx.needs_input_grad[3:])
-        refresh_weights(model)
+        save = grad_mode and any(ctx.needs_input_grad[3:])
+        w = param_layout(model)
+        w.refresh()
         x = x.contiguous()
         pos_tab, time_tab = _tables(model, T, H, W)
         tok = torch.empty(rows, C_, dtype=bf16, device=x.device)
@@ -305,19 +311,20 @@ class _TimeSformerFunction(torch.autograd.Function):
                       (None,) + tuple(m.repeat_interleave(seq_len).contiguous() for m in masks[i]) for i in range(model.depth)]
         saved = []
         for i in range(model.depth):
-            tok, sv = _block_fwd(model, i, tok, descs, save, scales[i])
+            tok, sv = _block_fwd(model, w, i, tok, descs, save, scales[i])
             saved.append(sv)
         out = torch.empty(B, T, C_, H, W, dtype=x.dtype, device=x.device)   # timesformer.py:523 (values; contiguous)
         ops.tsf_untokenize(tok, out, B, T, C_, HW)
         if save:
-            ctx.model, ctx.names, ctx.saved, ctx.descs, ctx.scales = model, names, saved, descs, scales
+            ctx.model, ctx.saved, ctx.descs, ctx.scales = model, saved, descs, scales
             ctx.dims = (B, T, C_, H, W)
             ctx.x_dtype = x.dtype
         return out
 
     @staticmethod
     def backward(ctx, d_out):
-        model, names, saved, descs = ctx.model, ctx.names, ctx.saved, ctx.descs
+        model, saved, descs = ctx.model, ctx.saved, ctx.descs
+        w = param_layout(model)
         B, T, C_, H, W = ctx.dims
         HW, rows = H * W, B * H * W * T
         dev = d_out.device
@@ -325,9 +332,8 @@ class _TimeSformerFunction(torch.autograd.Function):
         ops.tsf_embed_fwd(d_out.contiguous(), None, None, dtok, B, T, C_, HW)
         grads: Dict[str, torch.Tensor] = {}
         for i in reversed(range(model.depth)):
-            shapes = {n: tuple(p.shape) for n, p in model.blocks[i].named_parameters(prefix=f"blocks.{i}")}
-            alloc_flat(shapes, grads, dev)
-            dtok = _block_bwd(model, i, dtok, saved[i], descs, grads, ctx.scales[i])
+            w.alloc_grads(f"blocks.{i}", grads)
+            dtok = _block_bwd(model, w, i, dtok, saved[i], descs, grads, ctx.scales[i])
             saved[i] = None
         dx = None
         if ctx.needs_input_grad[3]:
@@ -352,4 +358,4 @@ class _TimeSformerFunction(torch.autograd.Function):
                 pos_tab, _ = _tables(model, T, H, W, pp)
                 grads["pos_embed"], = torch.autograd.grad([pos_tab], [pp], [d_pos_tab])
         ctx.saved = None
-        return (None, None, None, dx) + tuple(grads[n] if ctx.needs_input_grad[4 + j] else None for j, n in enumerate(names))
+        return (None, None, None, dx) + w.grads_out(grads, ctx.needs_input_grad[4:])
