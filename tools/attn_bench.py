@@ -11,42 +11,17 @@ bitwise equal results.  FLOPs: 1.474 GFLOP forward per (sample, layer) at the BE
 4·N·N_keys·64 per head as counted by the kernels' live pairs; backward x2.5."""
 import argparse
 import hashlib
-import json
+import os
 import sys
 
 import torch
 
-sys.path.insert(0, __file__.rsplit("/", 2)[0])
-from xpretrain_b200 import _lib  # noqa: E402
-
-ap = argparse.ArgumentParser()
-ap.add_argument("B", nargs="?", type=int, default=64, help="batch of the staged shape")
-ap.add_argument("--shapes", default="staged", help="comma-separated subset of staged, long, dense, or all")
-ap.add_argument("--lib", default=None, help="path of the library to load instead of the in-tree build")
-ap.add_argument("--digest", action="store_true", help="print a SHA-256 of out, lse and dqkv per shape")
-ap.add_argument("--iters", type=int, default=10)
-args = ap.parse_args()
-if args.lib:
-    _lib.LIB_PATH = args.lib
-from xpretrain_b200 import ops  # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from tools import harness  # noqa: E402
+from xpretrain_b200 import _lib, ops  # noqa: E402
 
 dev = torch.device("cuda", 0)
 bf16 = torch.bfloat16
-flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-
-
-def timeit(fn):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(args.iters):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); fn(); e1.record()
-        torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1))
-    ts.sort()
-    return ts[len(ts) // 2]
 
 
 def inputs(rows, C):
@@ -64,7 +39,7 @@ def digest(*ts):
     return h.hexdigest()
 
 
-def vip(name, B, H, T, L, M):
+def vip(B, H, T, L, M):
     C, S = 64 * H, M + T * L
     qkv, dout = inputs(B * S, C)
     out = torch.empty(B * S, C, dtype=bf16, device=dev)
@@ -75,10 +50,10 @@ def vip(name, B, H, T, L, M):
     bwd = lambda: ops.vip_attention_bwd(qkv, out, dout, lse, dqkv, ws, B, H, T, L, M, C, 0.125)
     # frame queries see M + L keys; global queries see M + T*L keys
     flop = 1.474e9 * B if (B, H, T, L, M) == (B, 12, 12, 196, 4) else 4.0 * 64 * H * B * (T * L * (M + L) + M * S)
-    return run(name, dict(B=B, H=H, T=T, L=L, M=M), fwd, bwd, flop, lambda: (out, lse, dqkv))
+    return dict(B=B, H=H, T=T, L=L, M=M), fwd, bwd, flop, (out, lse, dqkv)
 
 
-def dense(name, n_seq, H, N):
+def dense(n_seq, H, N):
     C, n = 64 * H, n_seq * N
     qkv, dout = inputs(n, C)
     out = torch.empty(n, C, dtype=bf16, device=dev)
@@ -88,29 +63,45 @@ def dense(name, n_seq, H, N):
     desc = ops.dense_desc(n, H, 3 * C, C, n_seq=n_seq, seq_len=N)
     fwd = lambda: ops.dense_attention_fwd(qkv, out, lse, desc)
     bwd = lambda: ops.dense_attention_bwd(qkv, out, dout, lse, delta, dqkv, desc, 0.125)
-    return run(name, dict(n_seq=n_seq, H=H, N=N), fwd, bwd, 4.0 * 64 * H * n_seq * N * N, lambda: (out, lse, dqkv))
+    return dict(n_seq=n_seq, H=H, N=N), fwd, bwd, 4.0 * 64 * H * n_seq * N * N, (out, lse, dqkv)
 
 
-def run(name, shape, fwd, bwd, flop, outputs):
+def run(args, flush, name, shape, fwd, bwd, flop, outputs):
     res = {"name": name}
     if args.digest:   # from freshly seeded inputs, before any timing
         fwd(); bwd()
         torch.cuda.synchronize()
-        res["digest"] = digest(*outputs())
-    res["fwd_ms"] = timeit(fwd)
-    res["bwd_ms"] = timeit(bwd)
+        res["digest"] = digest(*outputs)
+    res["fwd_ms"] = harness.median_ms(fwd, args.iters, 3, flush)
+    res["bwd_ms"] = harness.median_ms(bwd, args.iters, 3, flush)
     res["fwd_tflops"] = flop / res["fwd_ms"] / 1e9
     res["bwd_tflops"] = 2.5 * flop / res["bwd_ms"] / 1e9
     res["shape"] = shape
-    print(json.dumps(res), flush=True)
+    harness.emit(res)
 
 
-SHAPES = {
-    "staged": [lambda: vip("vip_staged_b16", args.B, 12, 12, 196, 4)],
-    "long": [lambda: vip("vip_long_l256", 96, 16, 12, 256, 4), lambda: vip("vip_long_l576", 40, 16, 12, 576, 4)],
-    "dense": [lambda N=N: dense(f"dense_n{N}", 16, 16, N) for N in (392, 1120, 6272)],
-}
-for key in (SHAPES if args.shapes == "all" else args.shapes.split(",")):
-    for shape in SHAPES[key]:
-        shape()
-        torch.cuda.empty_cache()
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("B", nargs="?", type=int, default=64, help="batch of the staged shape")
+    ap.add_argument("--shapes", default="staged", help="comma-separated subset of staged, long, dense, or all")
+    ap.add_argument("--lib", default=None, help="path of the library to load instead of the in-tree build")
+    ap.add_argument("--digest", action="store_true", help="print a SHA-256 of out, lse and dqkv per shape")
+    ap.add_argument("--iters", type=int, default=10)
+    args = ap.parse_args()
+    harness.require_gpu()
+    if args.lib:
+        _lib.LIB_PATH = args.lib
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    shapes = {
+        "staged": [("vip_staged_b16", lambda: vip(args.B, 12, 12, 196, 4))],
+        "long": [("vip_long_l256", lambda: vip(96, 16, 12, 256, 4)), ("vip_long_l576", lambda: vip(40, 16, 12, 576, 4))],
+        "dense": [(f"dense_n{N}", lambda N=N: dense(16, 16, N)) for N in (392, 1120, 6272)],
+    }
+    for key in (shapes if args.shapes == "all" else args.shapes.split(",")):
+        for name, make in shapes[key]:
+            run(args, flush, name, *make())
+            torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()

@@ -12,29 +12,15 @@ cases 2 and 3 are not run without checkpointing (they do not fit in 80 GB).
     python tools/checkpoint_bench.py [--steps 5] [--warmup 2]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
-from types import SimpleNamespace
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-from xpretrain_b200.modeling import VidCLIP  # noqa: E402
-from xpretrain_b200.optimization.loss import gather_nce_loss  # noqa: E402
+from tools import harness  # noqa: E402
 
 LT = 32
-
-
-def gpu_identity():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = "unknown"
-    return {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": q}
 
 
 def saved_bytes(cfg, B, T, Lt, ckpt):
@@ -51,58 +37,24 @@ def saved_bytes(cfg, B, T, Lt, ckpt):
     return vis + nt * tblock + rt * 6 * Ct
 
 
-def build_model(dev):
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.60, add_cls_num=3)
-    torch.manual_seed(0)
-    model = VidCLIP(SimpleNamespace(clip_config="openai/clip-vit-base-patch16", clip_weights="",
-                                    clip_vision_additional_config=add))
-    with torch.no_grad():
-        model.clipmodel.vision_model.embeddings.temporal_embedding.normal_(0, 0.02)
-    return model.to(dev)
-
-
-def inputs(dev, B, T):
-    g = torch.Generator().manual_seed(1234)
-    video = torch.randn(B, T, 3, 224, 224, generator=g)
-    ids = torch.randint(1, 49406, (B, LT), generator=g)
-    ids[:, -1] = 49407
-    return video.to(dev), ids.to(dev), torch.ones(B, LT, dtype=torch.long, device=dev)
-
-
 def run(model, batch, ckpt, steps, warmup):
-    """(ms per step, peak bytes above the allocation before the first step, outputs of the last step)."""
+    """(ms per step, peak GiB above the allocation before the first step, outputs of the last step)."""
     cm = model.clipmodel
     (cm.gradient_checkpointing_enable if ckpt else cm.gradient_checkpointing_disable)()
-    params = list(model.parameters())
     last = {}
 
     def step():
-        for p in params:
-            p.grad = None
-        out = model(video=batch[0], text_input_ids=batch[1], text_input_mask=batch[2])
-        loss = gather_nce_loss(out["vis_features"], out["text_features"], cm.logit_scale)
-        loss.backward()
+        loss, out = harness.clip_train_step(model, batch)
         last.update(loss=loss.detach(), vis=out["vis_features"].detach(), txt=out["text_features"].detach())
 
-    for p in params:
+    for p in model.parameters():
         p.grad = None
-    torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats()
     base = torch.cuda.memory_allocated()
-    for _ in range(warmup):
-        step()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    peak = torch.cuda.max_memory_allocated() - base
+    ms, peak = harness.peak_gib(lambda: harness.window_ms(step, steps, warmup))
     last["grads"] = {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
     cm.gradient_checkpointing_disable()
-    return e0.elapsed_time(e1) / steps, peak, last
+    return ms, peak - base / harness.GIB, last
 
 
 def compare(a, b):
@@ -124,38 +76,38 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
+    harness.require_gpu()
     dev = torch.device("cuda", 0)
-    ident = gpu_identity()
-    model = build_model(dev)
+    model = harness.clip_model(dev, "openai/clip-vit-base-patch16", seed_temporal=True)
     cfg = model.clipmodel.config
-    gib = 2 ** 30
+    gib = harness.GIB
 
     B, T = 64, 12
-    batch = inputs(dev, B, T)
+    batch = harness.clip_batch(dev, B, T, 224, LT)
     res = {"off": [], "on": []}
     outs = {}
     for mode in ("off", "on", "off", "on"):
         ms, peak, last = run(model, batch, mode == "on", args.steps, args.warmup)
-        res[mode].append({"ms_per_step": round(ms, 2), "pairs_per_s": round(B / ms * 1e3, 1), "peak_gib": round(peak / gib, 2)})
+        res[mode].append({"ms_per_step": round(ms, 2), "pairs_per_s": round(B / ms * 1e3, 1), "peak_gib": round(peak, 2)})
         outs.setdefault(mode, []).append(last)
     cmp_modes = compare(outs["off"][-1], outs["on"][-1])
     cmp_runs = compare(outs["off"][0], outs["off"][-1])      # the same mode twice: the run-to-run spread of the atomics
     del outs
-    print(json.dumps({"case": "B64_T12_off_vs_on", "B": B, "T": T, **ident, "runs": res,
-                      "predicted_saved_gib": {"off": round(saved_bytes(cfg, B, T, LT, False) / gib, 2),
-                                              "on": round(saved_bytes(cfg, B, T, LT, True) / gib, 2)},
-                      "off_vs_on": cmp_modes, "off_vs_off": cmp_runs}), flush=True)
+    harness.emit({"case": "B64_T12_off_vs_on", "B": B, "T": T, "runs": res,
+                  "predicted_saved_gib": {"off": round(saved_bytes(cfg, B, T, LT, False) / gib, 2),
+                                          "on": round(saved_bytes(cfg, B, T, LT, True) / gib, 2)},
+                  "off_vs_on": cmp_modes, "off_vs_off": cmp_runs})
     del batch
 
     for B, T in ((128, 12), (64, 32)):
-        batch = inputs(dev, B, T)
+        batch = harness.clip_batch(dev, B, T, 224, LT)
         ms, peak, last = run(model, batch, True, args.steps, args.warmup)
         finite = bool(torch.isfinite(last["loss"]).item()) and all(bool(torch.isfinite(g).all()) for g in last["grads"].values())
         del last, batch
-        print(json.dumps({"case": f"B{B}_T{T}_on", "B": B, "T": T, **ident, "ms_per_step": round(ms, 2),
-                          "pairs_per_s": round(B / ms * 1e3, 1), "peak_gib": round(peak / gib, 2), "finite": finite,
-                          "predicted_saved_gib": {"off": round(saved_bytes(cfg, B, T, LT, False) / gib, 2),
-                                                  "on": round(saved_bytes(cfg, B, T, LT, True) / gib, 2)}}), flush=True)
+        harness.emit({"case": f"B{B}_T{T}_on", "B": B, "T": T, "ms_per_step": round(ms, 2),
+                      "pairs_per_s": round(B / ms * 1e3, 1), "peak_gib": round(peak, 2), "finite": finite,
+                      "predicted_saved_gib": {"off": round(saved_bytes(cfg, B, T, LT, False) / gib, 2),
+                                              "on": round(saved_bytes(cfg, B, T, LT, True) / gib, 2)}})
 
 
 if __name__ == "__main__":

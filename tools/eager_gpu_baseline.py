@@ -6,7 +6,6 @@ torch.autocast(bfloat16) — the reference cannot run `.to(bfloat16)` (SURVEY.md
 bf16 mode.  fwd + InfoNCE + bwd, CUDA-event timed, B = 64 (falls back to 32 / 16 if eager runs out of memory).
 This is a measurement tool (it executes oracle/ on purpose); nothing in the product imports it.
 """
-import json
 import os
 import sys
 
@@ -14,6 +13,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import clipvip_oracle as O  # noqa: E402
+from tools import harness  # noqa: E402
 
 
 def run(B, steps=5, warmup=2):
@@ -34,25 +34,21 @@ def run(B, steps=5, warmup=2):
         loss.backward()
         return loss
 
-    for _ in range(warmup):
-        step()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    ms, peak = harness.peak_gib(lambda: harness.window_ms(step, steps, warmup))
     return {"impl": "pytorch-eager (oracle port of the reference) under bf16 autocast", "batch": B, "ms_per_step": round(ms, 2),
-            "pairs_per_s": round(B / ms * 1e3, 2), "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 1)}
+            "pairs_per_s": round(B / ms * 1e3, 2), "max_mem_gb": round(peak, 1)}
+
+
+def main():
+    harness.require_gpu()
+    for B in (64, 32, 16):
+        try:
+            harness.emit(run(B))
+            break
+        except torch.OutOfMemoryError:
+            harness.emit({"batch": B, "error": "out of memory in eager"})
+            torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
-    for B in (64, 32, 16):
-        try:
-            print(json.dumps(run(B)), flush=True)
-            break
-        except torch.OutOfMemoryError:
-            print(json.dumps({"batch": B, "error": "out of memory in eager"}), flush=True)
-            torch.cuda.empty_cache()
+    main()

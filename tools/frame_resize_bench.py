@@ -11,39 +11,23 @@
 Prints one JSON line; the card's name and power limit are read in the same run.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from tools import harness  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else torch.cuda.get_device_name(0)
 
 
 def kernel_time(dev, H, W, frames=64 * 12, S=224, p=16, iters=50):
     from xpretrain_b200 import ops
     video = torch.randint(0, 256, (frames, H, W, 3), dtype=torch.uint8, device=dev)
     out = torch.empty(frames * (S // p) ** 2, ops.patch_pitch(p), dtype=torch.bfloat16, device=dev)
-    for _ in range(5):
-        ops.vip_resize_patchify_u8(video, out, S, p)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        ops.vip_resize_patchify_u8(video, out, S, p)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / iters
+    ms = harness.window_ms(lambda: ops.vip_resize_patchify_u8(video, out, S, p), iters, 5)
     nbytes = video.numel() + out.numel() * 2
     return {"frames": frames, "src": f"{H}x{W}", "ms": round(ms, 4), "bytes_read_MB": round(video.numel() / 1e6, 1),
             "bytes_written_MB": round(out.numel() * 2 / 1e6, 1), "bound_ms": round(nbytes / HBM_BYTES_PER_S * 1e3, 4),
@@ -113,15 +97,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "frame_resize_bench.py measures on an H100"
+    harness.require_gpu()
     dev = torch.device("cuda", 0)
-    res = {"card": card(),
-           "kernel": [kernel_time(dev, 240, 320), kernel_time(dev, 720, 1280)],
+    res = {"kernel": [kernel_time(dev, 240, 320), kernel_time(dev, 720, 1280)],
            "step_b64_t12": step_times(dev),
            "cpu_transform_ms_per_12_frame_sample_1_thread": {"240x320": cpu_transform_ms(240, 320),
                                                              "360x640": cpu_transform_ms(360, 640)}}
-    line = json.dumps(res)
-    print(line)
+    line = harness.emit(res)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:

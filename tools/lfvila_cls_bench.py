@@ -12,7 +12,6 @@ tool: it executes oracle/ on purpose; nothing in the product imports it.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 from types import SimpleNamespace
@@ -22,58 +21,16 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import lfvila_cls_oracle as L  # noqa: E402
 from oracle import swin3d_oracle as SO  # noqa: E402
+from tools import harness  # noqa: E402
 
 # the head's own kernels (pool, normalise, loss) by name; its GEMMs and column sums share kernels with the encoder, so the
 # head's whole share is the step's kernel time minus the encoder's (head_ms)
 HEAD_KERNELS = ("lfvila_",)
 
 
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
-
-
-def peak_of(fn):
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() / 2 ** 30
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return torch.cuda.get_device_name(0) + ", power limit not readable"
-
-
 def head_ms(model, video, labels):
     """Device time of the head in one training step: the encoder alone (forward + backward of a weighted sum of its output)
     is subtracted from the whole step, both as sums of kernel times from torch.profiler."""
-    from torch.profiler import ProfilerActivity, profile
-
-    def kernel_ms(fn):
-        fn()
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        evs = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        total = sum(e.device_time for e in evs) / 1e3
-        named = sum(e.device_time for e in evs if any(k in e.name for k in HEAD_KERNELS)) / 1e3
-        return total, named
-
     enc_out = model.video_encoder(video)[0]
     w = torch.randn(enc_out.shape, device=video.device, dtype=enc_out.dtype)
     del enc_out
@@ -86,8 +43,8 @@ def head_ms(model, video, labels):
         model.zero_grad(set_to_none=True)
         (model.video_encoder(video)[0] * w).sum().backward()
 
-    total, named = kernel_ms(step)
-    enc, _ = kernel_ms(encoder)
+    total, named = harness.profiled_kernel_ms(step, HEAD_KERNELS)
+    enc, _ = harness.profiled_kernel_ms(encoder)
     return total, enc, named
 
 
@@ -98,6 +55,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--labels", type=int, default=180)
     a = ap.parse_args()
+    harness.require_gpu()
     from xpretrain_b200.modeling import LFVILA_Video_Classification
 
     dev = torch.device("cuda", 0)
@@ -128,21 +86,21 @@ def main():
             model(video, labels)
 
     model.train()
-    ms_train = timed(train_step, a.steps, a.warmup)
-    peak_train = peak_of(train_step)
+    ms_train = harness.window_ms(train_step, a.steps, a.warmup)
+    _, peak_train = harness.peak_gib(train_step)
     model.eval()
-    ms_eval = timed(evaluate, a.steps, a.warmup)
-    peak_eval = peak_of(evaluate)
+    ms_eval = harness.window_ms(evaluate, a.steps, a.warmup)
+    _, peak_eval = harness.peak_gib(evaluate)
     model.train()
     total, enc_ms, named = head_ms(model, video, labels)
     res = {"what": f"LFVILA_Video_Classification, coin_cls.yaml, {B} x 3 x {D} x {H} x {W}, {n} labels",
-           "card": card(), "train_ms_per_step": round(ms_train, 2), "train_clips_per_s": round(B / ms_train * 1e3, 2),
+           "train_ms_per_step": round(ms_train, 2), "train_clips_per_s": round(B / ms_train * 1e3, 2),
            "train_peak_gib": round(peak_train, 2), "eval_ms": round(ms_eval, 2),
            "eval_clips_per_s": round(B / ms_eval * 1e3, 2), "eval_peak_gib": round(peak_eval, 2),
            "profiled_step_kernel_ms": round(total, 2), "profiled_encoder_kernel_ms": round(enc_ms, 2),
            "head_kernel_ms": round(total - enc_ms, 3), "head_share_of_step": round((total - enc_ms) / total, 4),
            "head_named_kernels_ms": round(named, 3)}
-    print(json.dumps(res), flush=True)
+    harness.emit(res)
     del model
     torch.cuda.empty_cache()
 
@@ -161,11 +119,11 @@ def main():
                 with torch.autocast("cuda", dtype=torch.bfloat16):
                     out = L.lfvila_cls_forward(sdo, v, lab, cfg)
                 out["loss"].float().backward()
-            ms_e = timed(eager, max(2, a.steps // 2), 1)
-            print(json.dumps({"what": "reference algorithm, eager PyTorch + bf16 autocast (oracle/lfvila_cls_oracle.py)",
-                              "batch": eb, "train_ms_per_step": round(ms_e, 2),
-                              "train_clips_per_s": round(eb / ms_e * 1e3, 2),
-                              "speedup_clips_per_s": round((B / ms_train) / (eb / ms_e), 2)}), flush=True)
+            ms_e = harness.window_ms(eager, max(2, a.steps // 2), 1)
+            harness.emit({"what": "reference algorithm, eager PyTorch + bf16 autocast (oracle/lfvila_cls_oracle.py)",
+                          "batch": eb, "train_ms_per_step": round(ms_e, 2),
+                          "train_clips_per_s": round(eb / ms_e * 1e3, 2),
+                          "speedup_clips_per_s": round((B / ms_train) / (eb / ms_e), 2)})
             break
         except torch.OutOfMemoryError:
             for t in sdo.values():

@@ -4,9 +4,7 @@ same loss in eager PyTorch fp32 on the same GPU, plus kernel launches per call. 
     python tools/loss_bench.py [--sizes 128,512,1024] [--dim 512] [--iters 200] [--warmup 20]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -15,20 +13,11 @@ import torch.nn.functional as F
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import loss_family_oracle as LF  # noqa: E402
+from tools import harness  # noqa: E402
 from xpretrain_b200 import ops  # noqa: E402
 from xpretrain_b200.optimization.loss import _LOSSES, build_loss_func  # noqa: E402
 
 TEMP = 0.05
-
-
-def gpu_identity():
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = "unknown"
-    return name, q
 
 
 def features(name, N, d, dev):
@@ -38,19 +27,6 @@ def features(name, N, d, dev):
     return [F.normalize(torch.randn(N, d, generator=g) + 0.5 * base, dim=-1).to(dev) for _ in range(n_args)]
 
 
-def timed(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="128,512,1024")
@@ -58,10 +34,8 @@ def main():
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("loss_bench needs a GPU")
+    harness.require_gpu()
     dev = torch.device("cuda", 0)
-    gpu, power = gpu_identity()
     rows = []
     for N in (int(x) for x in args.sizes.split(",")):
         for name in sorted(_LOSSES):
@@ -82,12 +56,11 @@ def main():
             ours()
             torch.cuda.synchronize()
             launches = ops.launch_count()
-            t_ours = timed(ours, args.iters, args.warmup)
-            t_eager = timed(eager, args.iters, args.warmup)
+            t_ours = harness.window_ms(ours, args.iters, args.warmup)
+            t_eager = harness.window_ms(eager, args.iters, args.warmup)
             rows.append({"loss": name, "N": N, "d": args.dim, "ours_ms": round(t_ours, 4), "eager_fp32_ms": round(t_eager, 4),
                          "speedup": round(t_eager / t_ours, 2), "launches_per_call": launches})
-    print(json.dumps({"metric": "contrastive_loss_fwd_bwd_ms", "gpu": gpu, "power_limit_and_max_sm_clock": power,
-                      "iters": args.iters, "warmup": args.warmup, "results": rows}))
+    harness.emit({"metric": "contrastive_loss_fwd_bwd_ms", "iters": args.iters, "warmup": args.warmup, "results": rows})
 
 
 if __name__ == "__main__":

@@ -3,7 +3,10 @@
 fwd + bwd of the module (synthetic video, a weighted-sum loss, DropPath off), CUDA-event timed, at BASELINE.json's
 [8,3,32,224,224] and the reference-native 192x320; beside it the reference algorithm in PyTorch eager (the pinned oracle, bf16
 autocast) on the same GPU.  A measurement tool: it executes oracle/ on purpose; nothing in the product imports it.
+
+    python tools/swin3d_bench.py [--graph]
 """
+import argparse
 import json
 import os
 import sys
@@ -12,22 +15,14 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import swin3d_oracle as SO  # noqa: E402
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
+from tools import harness  # noqa: E402
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--graph", action="store_true", help="also time the step replayed from CUDA graphs")
+    args = ap.parse_args()
+    harness.require_gpu()
     from xpretrain_b200.modeling.swin3d import SwinTransformer3D
 
     dev = torch.device("cuda", 0)
@@ -64,9 +59,9 @@ def main():
                 out = SO.swin3d_forward(sdo, video, cfg)
             (out.float() * w_out).sum().backward()
 
-        ms = timed(ours, 5, 2)
+        ms = harness.window_ms(ours, 5, 2)
         ms_graph, graph_note = None, None
-        if "--graph" in sys.argv:
+        if args.graph:
             # the 24 blocks issue ~1300 small launches per step: replay them from CUDA graphs (torch.cuda.make_graphed_callables
             # captures this module's forward and backward, all launched on the capture stream through the C ABI)
             class First(torch.nn.Module):
@@ -86,21 +81,21 @@ def main():
                 ref_out = model(video)[0].detach()
                 got = gm(video).detach()
                 graph_note = f"graphed output rel diff {float((got - ref_out).norm() / ref_out.norm()):.1e}"
-                ms_graph = timed(graphed, 5, 2)
+                ms_graph = harness.window_ms(graphed, 5, 2)
             except Exception as exc:  # noqa: BLE001 - report, do not hide
                 graph_note = f"capture failed: {type(exc).__name__}: {str(exc)[:200]}"
         try:
-            ms_e = timed(eager, 3, 1)
+            ms_e = harness.window_ms(eager, 3, 1)
         except torch.OutOfMemoryError:
             ms_e = None
             torch.cuda.empty_cache()
         fl = 3.0 * SO.flops_per_sample(cfg, D, H, W) * B
-        print(json.dumps({"shape": [B, 3, D, H, W], "what": what, "ms_fwd_bwd": round(ms, 3),
-                          "samples_per_s": round(B / ms * 1e3, 1), "tflops": round(fl / ms / 1e9, 1),
-                          "frac_of_sustained_peak": round(fl / ms / 1e9 / peak, 3),
-                          "cuda_graph_ms": None if ms_graph is None else round(ms_graph, 3), "cuda_graph_note": graph_note,
-                          "eager_bf16_ms": None if ms_e is None else round(ms_e, 3),
-                          "speedup_vs_eager": None if ms_e is None else round(ms_e / ms, 2)}), flush=True)
+        harness.emit({"shape": [B, 3, D, H, W], "what": what, "ms_fwd_bwd": round(ms, 3),
+                      "samples_per_s": round(B / ms * 1e3, 1), "tflops": round(fl / ms / 1e9, 1),
+                      "frac_of_sustained_peak": round(fl / ms / 1e9 / peak, 3),
+                      "cuda_graph_ms": None if ms_graph is None else round(ms_graph, 3), "cuda_graph_note": graph_note,
+                      "eager_bf16_ms": None if ms_e is None else round(ms_e, 3),
+                      "speedup_vs_eager": None if ms_e is None else round(ms_e / ms, 2)})
 
 
 if __name__ == "__main__":

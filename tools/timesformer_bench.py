@@ -12,22 +12,11 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import timesformer_oracle as TO  # noqa: E402
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
+from tools import harness  # noqa: E402
 
 
 def main():
+    harness.require_gpu()
     from xpretrain_b200.modeling.timesformer import TimeSformer
 
     dev = torch.device("cuda", 0)
@@ -65,13 +54,13 @@ def main():
                 out = TO.timesformer_forward(sdo, xo, cfg)
             (out.float() * w_out).sum().backward()
 
-        ms = timed(ours, 10, 3)
-        ms_e = timed(eager, 5, 2)
+        ms = harness.window_ms(ours, 10, 3)
+        ms_e = harness.window_ms(eager, 5, 2)
         fl = 3.0 * TO.flops_per_sample(cfg, T, H, W) * B
-        print(json.dumps({"shape": [B, T, cfg.embed_dim, H, W], "what": what, "ms_fwd_bwd": round(ms, 3),
-                          "samples_per_s": round(B / ms * 1e3, 1), "tflops": round(fl / ms / 1e9, 1),
-                          "frac_of_sustained_peak": round(fl / ms / 1e9 / peak, 3),
-                          "eager_bf16_ms": round(ms_e, 3), "speedup_vs_eager": round(ms_e / ms, 2)}), flush=True)
+        harness.emit({"shape": [B, T, cfg.embed_dim, H, W], "what": what, "ms_fwd_bwd": round(ms, 3),
+                      "samples_per_s": round(B / ms * 1e3, 1), "tflops": round(fl / ms / 1e9, 1),
+                      "frac_of_sustained_peak": round(fl / ms / 1e9 / peak, 3),
+                      "eager_bf16_ms": round(ms_e, 3), "speedup_vs_eager": round(ms_e / ms, 2)})
 
 
 if __name__ == "__main__":

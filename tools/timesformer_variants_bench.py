@@ -10,9 +10,7 @@ the dense attention kernel alone.
 Prints one JSON line per measurement, starting with the card's name, power limit and clocks.
 A measurement tool: it executes oracle/ on purpose; nothing in the product imports it.
 """
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -20,27 +18,9 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import timesformer_oracle as TO  # noqa: E402
 from oracle import timesformer_variants_oracle as V  # noqa: E402
+from tools import harness  # noqa: E402
 
 GRIDS = ((8, 7, 7), (7, 10, 16), (8, 28, 28))
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm",
-                        "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip()
 
 
 def model_bench(dev, B=16):
@@ -64,7 +44,7 @@ def model_bench(dev, B=16):
                 p.grad = None
             (model(x) * w_out).sum().backward()
 
-        ms = timed(ours, 5, 2)
+        ms = harness.window_ms(ours, 5, 2)
         fl = 3.0 * V.flops_per_sample(cfg, T, H, W, kind) * B
         rec = {"what": "joint model fwd+bwd", "grid_THW": [T, H, W], "batch": B, "ms": round(ms, 2),
                "clips_per_s": round(B / ms * 1e3, 1), "model_tflops": round(fl / ms / 1e9, 1)}
@@ -81,7 +61,7 @@ def model_bench(dev, B=16):
                     out = V.timesformer_forward(sdo, xo, cfg, kind)
                 (out.float() * we).sum().backward()
             try:
-                ms_e = timed(eager, 3, 1)
+                ms_e = harness.window_ms(eager, 3, 1)
                 rec.update(eager_batch=be, eager_ms=round(ms_e, 2), eager_clips_per_s=round(be / ms_e * 1e3, 1))
                 break
             except torch.OutOfMemoryError:
@@ -89,7 +69,7 @@ def model_bench(dev, B=16):
                 be //= 2
         if "eager_clips_per_s" in rec:
             rec["speedup_vs_eager"] = round(rec["clips_per_s"] / rec["eager_clips_per_s"], 2)
-        print(json.dumps(rec), flush=True)
+        harness.emit(rec)
         del x
         torch.cuda.empty_cache()
 
@@ -122,24 +102,24 @@ def attention_bench(dev, B=16, heads=16, rounds=3):
         for _ in range(rounds):                 # alternate the two kernels, call by call
             for name, (f, b) in kernels.items():
                 f()
-                res[name]["fwd"].append(timed(f, steps, 1))
-                res[name]["bwd"].append(timed(b, steps, 1))
+                res[name]["fwd"].append(harness.window_ms(f, steps, 1))
+                res[name]["bwd"].append(harness.window_ms(b, steps, 1))
         fl = 4.0 * N * N * 64 * heads * B
         for name in kernels:
             fwd, bwd = min(res[name]["fwd"]), min(res[name]["bwd"])
-            print(json.dumps({"what": "attention", "kernel": name, "grid_THW": [T, H, W], "N": N, "batch": B,
-                              "heads": heads, "fwd_ms": round(fwd, 3), "fwd_tflops": round(fl / fwd / 1e9, 1),
-                              "bwd_ms": round(bwd, 3), "bwd_tflops": round(2.5 * fl / bwd / 1e9, 1),
-                              "fwd_ms_all": [round(v, 3) for v in res[name]["fwd"]],
-                              "bwd_ms_all": [round(v, 3) for v in res[name]["bwd"]]}), flush=True)
+            harness.emit({"what": "attention", "kernel": name, "grid_THW": [T, H, W], "N": N, "batch": B,
+                          "heads": heads, "fwd_ms": round(fwd, 3), "fwd_tflops": round(fl / fwd / 1e9, 1),
+                          "bwd_ms": round(bwd, 3), "bwd_tflops": round(2.5 * fl / bwd / 1e9, 1),
+                          "fwd_ms_all": [round(v, 3) for v in res[name]["fwd"]],
+                          "bwd_ms_all": [round(v, 3) for v in res[name]["bwd"]]})
         del qkv, dout, out, dqkv
         torch.cuda.empty_cache()
 
 
 def main():
-    assert torch.cuda.is_available(), "timesformer_variants_bench.py measures on an H100"
+    harness.require_gpu()
     dev = torch.device("cuda", 0)
-    print(json.dumps({"card": card()}), flush=True)
+    harness.emit({})
     attention_bench(dev)
     model_bench(dev)
 
