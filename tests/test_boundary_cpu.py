@@ -214,13 +214,9 @@ def test_every_launch_goes_through_ops_call():
 
 def test_no_cpu_fallback():
     """The product path must fail loudly off-GPU instead of computing on the host."""
-    from types import SimpleNamespace
+    from clipvip_cases import b16, vidclip
     from xpretrain_b200 import _lib
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
+    model = vidclip(b16(1, 1))
     with pytest.raises(_lib.XpError):
         model(video=torch.zeros(1, 1, 3, 224, 224), text_input_ids=torch.zeros(1, 4, dtype=torch.long),
               text_input_mask=torch.ones(1, 4, dtype=torch.long))
@@ -235,14 +231,10 @@ def test_product_path_never_imports_the_oracle():
 
 
 def test_state_dict_names_match_reference_layout():
-    from types import SimpleNamespace
+    from clipvip_cases import b16, vidclip
     from oracle import clipvip_oracle as O
-    from xpretrain_b200.modeling import VidCLIP
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 2, 3072), text=TowerConfig(512, 8, 2, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    cfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, 2, 3072), text=O.TowerCfg(512, 8, 2, 2048))
+    cfg = b16(2, 2)
+    model = vidclip(cfg)
     sd = O.init_state_dict(cfg)      # keyed like the reference CLIPModel.state_dict() (pinned by make_golden.py)
     own = model.clipmodel.state_dict()
     assert set(own) == set(sd)
@@ -335,9 +327,7 @@ def test_training_restorer_shaped_checkpoint_round_trips(tmp_path):
     (`_to_cuda`, :159-174).  Our module tree and our AdamW must accept that file unchanged: same keys, same optimizer-state
     layout (`step`, `exp_avg`, `exp_avg_sq`; param_groups with lr / betas / eps / weight_decay / correct_bias)."""
     import torch
-    from types import SimpleNamespace
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
+    from clipvip_cases import b16, vidclip
     from xpretrain_b200.optimization.adamw import AdamW, build_e2e_optimizer_w_lr_mul
 
     def to_cpu(state):     # restatement of load_save.py:177-192
@@ -360,10 +350,7 @@ def test_training_restorer_shaped_checkpoint_round_trips(tmp_path):
         return state
 
     def build(seed):
-        torch.manual_seed(seed)
-        add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-        mc = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-        model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
+        model = vidclip(b16(1, 1), seed=seed)
         opt = AdamW(build_e2e_optimizer_w_lr_mul(list(model.named_parameters()), 1e-4, 0.2), lr=1e-4, betas=(0.9, 0.98))
         return model, opt
 

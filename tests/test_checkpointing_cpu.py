@@ -1,17 +1,13 @@
 """CPU: the gradient-checkpointing switches of CLIPModel carry the reference's names (CLIP_ViP.py:478,524-526,626) and change
 neither the parameters nor the absence of a CPU path."""
-from types import SimpleNamespace
-
 import pytest
 import torch
 
+from clipvip_cases import b16, vidclip
+
 
 def _vidclip():
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-    return VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
+    return vidclip(b16(1, 1))
 
 
 def test_switches_have_the_reference_names_and_default_off():

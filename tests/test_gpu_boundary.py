@@ -3,10 +3,10 @@
 `freeze_text_encoder` (VidCLIP.py:92-103), and the contract that a weight written IN PLACE through `p.data` — the idiom
 of the reference's own AdamW (CLIP-ViP/src/optimization/adamw.py:89,101), which autograd's version counter does not see —
 is what the next forward computes with."""
-from types import SimpleNamespace
-
 import pytest
 import torch
+
+from clipvip_cases import b16, rel, vidclip
 
 pytestmark = pytest.mark.gpu
 
@@ -18,21 +18,11 @@ def dev():
     return torch.device("cuda", 0)
 
 
-def _rel(a, b):
-    return float((a.float() - b.float()).norm() / b.float().norm().clamp_min(1e-30))
-
-
 def _small(dev, seed=3, layers=2):
     from oracle import clipvip_oracle as O
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    cfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, layers, 3072), text=O.TowerCfg(512, 8, layers, 2048))
+    cfg = b16(layers, layers)
     sd = O.init_state_dict(cfg, seed=seed)
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, layers, 3072), text=TowerConfig(512, 8, layers, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    model.clipmodel.load_state_dict(sd, strict=False)
-    return O, cfg, sd, model.to(dev)
+    return O, cfg, sd, vidclip(cfg, sd=sd, dev=dev)
 
 
 def test_single_tower_entry_points_against_oracle(dev):
@@ -47,13 +37,13 @@ def test_single_tower_entry_points_against_oracle(dev):
         gt_raw = model.clipmodel.get_text_features(input_ids=ids.to(dev), attention_mask=mask.to(dev), if_norm=False)
         both = model(video=video.to(dev), text_input_ids=ids.to(dev), text_input_mask=mask.to(dev))
     assert torch.equal(fv, both["vis_features"]) and torch.equal(ft, both["text_features"]) and torch.equal(gi_n, fv)
-    assert _rel(fv.cpu(), want["vis_features"]) < 1e-2 and _rel(ft.cpu(), want["text_features"]) < 1e-2
+    assert rel(fv.cpu(), want["vis_features"]) < 1e-2 and rel(ft.cpu(), want["text_features"]) < 1e-2
     # un-normalised projections (CLIP_ViP.py:1039-1041, 1083-1085): the oracle towers return them before l2_normalize
     vis_raw = O.vision_tower(sd, video, cfg) @ sd["visual_projection.weight"].t()
     txt_raw = O.text_tower(sd, ids, mask, cfg) @ sd["text_projection.weight"].t()
-    assert _rel(gi_raw.cpu(), vis_raw) < 1e-2 and _rel(gt_raw.cpu(), txt_raw) < 1e-2
+    assert rel(gi_raw.cpu(), vis_raw) < 1e-2 and rel(gt_raw.cpu(), txt_raw) < 1e-2
     assert float((gi_raw.norm(dim=-1) - 1).abs().min()) > 1e-3          # really not normalised
-    assert _rel(torch.nn.functional.normalize(gi_raw, dim=-1).cpu(), fv.cpu()) < 1e-5
+    assert rel(torch.nn.functional.normalize(gi_raw, dim=-1).cpu(), fv.cpu()) < 1e-5
 
 
 def test_freeze_text_encoder(dev):
@@ -81,7 +71,7 @@ def test_freeze_text_encoder(dev):
     model.freeze_text_encoder(freeze_text_proj=True)
     _, g2 = run()
     assert g2["text_projection.weight"] is None and all(g is None for n, g in g2.items() if n.startswith("text_model."))
-    assert _rel(g2["visual_projection.weight"], g0["visual_projection.weight"]) < 1e-4
+    assert rel(g2["visual_projection.weight"], g0["visual_projection.weight"]) < 1e-4
 
 
 def test_inplace_data_updates_of_the_reference_adamw_reach_the_next_forward(dev):
@@ -101,13 +91,13 @@ def test_inplace_data_updates_of_the_reference_adamw_reach_the_next_forward(dev)
     assert all(p._version == versions[n] for n, p in model.clipmodel.named_parameters())   # autograd did not notice
     with torch.no_grad():
         out1 = model(video=dvideo, text_input_ids=dids, text_input_mask=dmask)
-    assert _rel(out1["vis_features"], out0["vis_features"].detach()) > 5e-2                 # the forward moved ...
+    assert rel(out1["vis_features"], out0["vis_features"].detach()) > 5e-2                 # the forward moved ...
     new_sd = {k: v.detach().cpu() for k, v in model.clipmodel.state_dict().items()}
     want = O.clip_vip_forward(new_sd, video, ids, mask, cfg)                                 # ... to where the fp32 oracle goes
     # (an lr = 2e-2 step moves every weight by about its own initial scale: activations grow and so does the bf16 error; the
     # stale-weights failure this test guards against is a 100 % error, the bar only has to separate the two)
-    assert _rel(out1["vis_features"].cpu(), want["vis_features"]) < 2e-2
-    assert _rel(out1["text_features"].cpu(), want["text_features"]) < 2e-2
+    assert rel(out1["vis_features"].cpu(), want["vis_features"]) < 2e-2
+    assert rel(out1["text_features"].cpu(), want["text_features"]) < 2e-2
     # same contract for load_state_dict and overload_logit_scale-style fills
     model.clipmodel.load_state_dict(sd, strict=False)
     with torch.no_grad():

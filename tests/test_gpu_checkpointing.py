@@ -1,4 +1,5 @@
-"""H100: gradient checkpointing of the CLIP-ViP encoders (`CLIPModel.gradient_checkpointing_enable()`).
+"""H100: gradient checkpointing of the CLIP-ViP encoders, ViT-B and ViT-L/14, and of the per-frame CLIP model
+(`CLIPModel.gradient_checkpointing_enable()`).
 
 A checkpointed tower keeps only each block's input and rebuilds the block's saved tensors in the backward by rerunning the
 same kernels.  The recompute must reproduce the forward bit for bit, so loss and features must be equal with the switch on and
@@ -6,21 +7,14 @@ off, and gradients may differ only by the reordering of the split-K fp32 atomics
 (contract_harness.reordering_violations).
 """
 import gc
-import os
-from types import SimpleNamespace
 
 import pytest
 import torch
 
+from clipvip_cases import b16, l14, ragged_batch, small_golden_case, train_step, vidclip
 from contract_harness import GRAD_REL, reordering_violations
 
 pytestmark = pytest.mark.gpu
-
-# the bars of test_gpu_parity.py's small-golden case (set there from the reference's own bf16 deviation)
-EMB_REL_L2 = 1.2e-2
-ROW_COSINE = 1.0 - 1e-3
-LOSS_REL = 1e-2
-GRAD_COSINE = 0.97
 
 
 @pytest.fixture(scope="module")
@@ -30,43 +24,8 @@ def dev():
     return torch.device("cuda", 0)
 
 
-def _model(dev, v_layers, t_layers, patch=16, stream="fp32", seed=0):
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, v_layers, 3072), text=TowerConfig(512, 8, t_layers, 2048),
-                       patch_size=patch, residual_fp32=(stream != "bf16"), residual_dtype=("fp16" if stream == "fp16" else "fp32"))
-    torch.manual_seed(seed)
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    with torch.no_grad():
-        model.clipmodel.vision_model.embeddings.temporal_embedding.normal_(0, 0.02)
-    return model.to(dev)
-
-
-def _inputs(dev, B, T, Lt, u8=False, seed=1):
-    g = torch.Generator().manual_seed(seed)
-    if u8:
-        video = torch.randint(0, 256, (B, T, 224, 224, 3), generator=g, dtype=torch.uint8)
-    else:
-        video = torch.randn(B, T, 3, 224, 224, generator=g)
-    ids = torch.randint(1, 49406, (B, Lt), generator=g)
-    mask = torch.ones(B, Lt, dtype=torch.long)
-    eos = torch.randint(2, Lt, (B,), generator=g)          # ragged: EOS, then padding with mask 0
-    for b in range(B):
-        ids[b, eos[b]:] = 49407
-        mask[b, eos[b] + 1:] = 0
-    return video.to(dev), ids.to(dev), mask.to(dev)
-
-
-def _step(model, video, ids, mask):
-    from xpretrain_b200.optimization.loss import NCELearnableTempLoss
-    model.zero_grad(set_to_none=True)
-    out = model(video=video, text_input_ids=ids, text_input_mask=mask)
-    loss = NCELearnableTempLoss()(out["vis_features"], out["text_features"], model.clipmodel.logit_scale)
-    loss.backward()
-    torch.cuda.synchronize()
-    grads = {n: (p.grad.detach().clone() if p.grad is not None else None) for n, p in model.named_parameters()}
-    return loss.detach(), out["vis_features"].detach(), out["text_features"].detach(), grads
+def _model(dev, cfg):
+    return vidclip(cfg, seed=0, temporal_init=True, dev=dev)
 
 
 def _assert_same(off, on):
@@ -79,14 +38,19 @@ def _assert_same(off, on):
 def _off_on(model, video, ids, mask):
     cm = model.clipmodel
     cm.gradient_checkpointing_disable()
-    off = _step(model, video, ids, mask)
+    off = train_step(model, video, ids, mask)
     cm.gradient_checkpointing_enable()
     assert cm.is_gradient_checkpointing
-    on = _step(model, video, ids, mask)
+    on = train_step(model, video, ids, mask)
     cm.gradient_checkpointing_disable()
     return off, on
 
 
+# The ViP model at B = 4, T = 12 with its temporal table redrawn; the per-frame model (its tower reruns per frame) and
+# ViT-L/14 (the streamed attention) at B = 3, T = 3 with their construction-time weights.
+VIP = {"cfg": b16(2, 2), "per_frame": False, "temporal_init": True, "B": 4, "T": 12}
+FRAME = {"cfg": b16(2, 2), "per_frame": True, "temporal_init": False, "B": 3, "T": 3}
+L14 = {"cfg": l14(224, 2, 2), "per_frame": False, "temporal_init": False, "B": 3, "T": 3}
 SWEEP = {
     "fp32": {},
     "fp16_stream": {"stream": "fp16"},
@@ -94,72 +58,44 @@ SWEEP = {
     "uint8_video": {"u8": True},
     "t4_interp": {"T": 4},
     "frozen_text": {"frozen": True},
-    "vit_b32": {"patch": 32},
+    "vit_b32": {"cfg": b16(2, 2, patch=32)},
     "sm_reserve8": {"reserve": 8},
+    "frame_clip_fp32": FRAME,
+    "frame_clip_fp16_stream": {**FRAME, "stream": "fp16"},
+    "frame_clip_bf16_stream": {**FRAME, "stream": "bf16"},
+    "frame_clip_uint8_video": {**FRAME, "u8": True},
+    "vit_l14_fp32": L14,
+    "vit_l14_fp16_stream": {**L14, "stream": "fp16"},
+    "vit_l14_bf16_stream": {**L14, "stream": "bf16"},
+    "vit_l14_uint8_video": {**L14, "u8": True},
 }
 
 
 @pytest.mark.parametrize("case", list(SWEEP))
 def test_checkpointing_reproduces_results_depth2(dev, case):
-    c = SWEEP[case]
-    model = _model(dev, 2, 2, patch=c.get("patch", 16), stream=c.get("stream", "fp32"))
+    c = {**VIP, **SWEEP[case]}
+    model = vidclip(c["cfg"], stream=c.get("stream", "fp32"), per_frame=c["per_frame"], seed=0,
+                    temporal_init=c["temporal_init"], dev=dev)
     if c.get("frozen"):
         model.freeze_text_encoder(freeze_text_proj=True)
     model.clipmodel.nccl_sm_reserve = c.get("reserve", 0)
-    video, ids, mask = _inputs(dev, 4, c.get("T", 12), 24, u8=c.get("u8", False))
+    video, ids, mask = ragged_batch(c["B"], c["T"], 24, u8=c.get("u8", False), dev=dev)
     off, on = _off_on(model, video, ids, mask)
+    assert off[1].shape == (c["B"], c["cfg"].proj_dim)
     if c.get("frozen"):
         assert all(g is None for n, g in on[3].items() if n.startswith("clipmodel.text_model."))
     _assert_same(off, on)
 
 
 def test_checkpointing_reproduces_results_full_depth(dev):
-    model = _model(dev, 12, 12)
-    video, ids, mask = _inputs(dev, 4, 12, 32)
+    model = _model(dev, b16(12, 12))
+    video, ids, mask = ragged_batch(4, 12, 32, dev=dev)
     off, on = _off_on(model, video, ids, mask)
     _assert_same(off, on)
 
 
 def test_checkpointing_depth2_ragged_against_reference_golden(dev, golden_dir):
-    from oracle import clipvip_oracle as O
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    from xpretrain_b200.optimization.loss import build_loss_func
-    gold = torch.load(os.path.join(golden_dir, "depth2_b3_t12_ragged.pt"), weights_only=False)
-    meta = gold["meta"]
-    cfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, meta["vision_layers"], 3072), text=O.TowerCfg(512, 8, meta["text_layers"], 2048))
-    sd = O.init_state_dict(cfg, seed=meta["weight_seed"])
-    video, ids, mask = O.synthetic_batch(meta["B"], meta["T"], meta["Lt"], cfg, seed=meta["data_seed"], ragged_text=meta["ragged"])
-    assert torch.equal(ids, gold["input_ids"])
-    add = SimpleNamespace(type="ViP", temporal_size=cfg.temporal_size, if_use_temporal_embed=1,
-                          logit_scale_init_value=cfg.logit_scale_init, add_cls_num=cfg.add_cls_num)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, cfg.vision.layers, 3072), text=TowerConfig(512, 8, cfg.text.layers, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    missing, unexpected = model.clipmodel.load_state_dict(sd, strict=False)
-    assert not missing and not unexpected
-    model = model.to(dev)
-    model.clipmodel.gradient_checkpointing_enable()
-    out = model(video=video.to(dev), text_input_ids=ids.to(dev), text_input_mask=mask.to(dev))
-    loss = build_loss_func({"loss_name": "NCELearnableTempLoss"})(out["vis_features"], out["text_features"],
-                                                                    model.clipmodel.logit_scale)
-    vis, txt = out["vis_features"].detach().cpu(), out["text_features"].detach().cpu()
-    rel = lambda a, b: float((a.float() - b.float()).norm() / b.float().norm())  # noqa: E731
-    assert rel(vis, gold["vis_features"]) < EMB_REL_L2 and rel(txt, gold["text_features"]) < EMB_REL_L2
-    assert torch.nn.functional.cosine_similarity(vis, gold["vis_features"]).min() > ROW_COSINE
-    assert torch.nn.functional.cosine_similarity(txt, gold["text_features"]).min() > ROW_COSINE
-    assert abs(float(loss) - float(gold["loss"])) < LOSS_REL * abs(float(gold["loss"]))
-    loss.backward()
-    torch.cuda.synchronize()
-    named = dict(model.clipmodel.named_parameters())
-    for k, gn in gold["grad_norms"].items():
-        assert named[k].grad is not None, k
-        if gn >= 1e-4:
-            assert 0.85 < float(named[k].grad.norm()) / gn < 1.15, k
-    for k, sample in gold["grad_samples"].items():
-        if sample.norm() < 1e-6:
-            continue
-        got = named[k].grad.detach().flatten()[:256].cpu()
-        assert float(torch.nn.functional.cosine_similarity(got, sample, dim=0)) > GRAD_COSINE, k
+    small_golden_case(dev, golden_dir, "depth2_b3_t12_ragged", checkpointing=True)
 
 
 def _kept_by_forward(model, video, ids, mask):
@@ -198,11 +134,11 @@ def _predicted_kept_bytes(cfg, B, T, Lt):
 
 
 def test_checkpointing_forward_keeps_only_boundaries(dev):
-    model = _model(dev, 12, 12)
+    model = _model(dev, b16(12, 12))
     B, T, Lt = 4, 12, 32
-    video, ids, mask = _inputs(dev, B, T, Lt)
+    video, ids, mask = ragged_batch(B, T, Lt, dev=dev)
     model.clipmodel.gradient_checkpointing_enable()
-    _step(model, video, ids, mask)                      # weight copies and streams exist before the measurement
+    train_step(model, video, ids, mask)                      # weight copies and streams exist before the measurement
     kept = _kept_by_forward(model, video, ids, mask)
     want = _predicted_kept_bytes(model.clipmodel.config, B, T, Lt)
     print(f"  checkpointed forward keeps {kept / 2**20:.1f} MiB, predicted {want / 2**20:.1f} MiB")
@@ -214,14 +150,14 @@ def _step_peak(model, video, ids, mask):
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
     base = torch.cuda.memory_allocated()
-    _step(model, video, ids, mask)
+    train_step(model, video, ids, mask)
     return torch.cuda.max_memory_allocated() - base
 
 
 def test_checkpointing_halves_peak_memory(dev):
-    model = _model(dev, 12, 12)
-    video, ids, mask = _inputs(dev, 4, 12, 32)
-    _step(model, video, ids, mask)
+    model = _model(dev, b16(12, 12))
+    video, ids, mask = ragged_batch(4, 12, 32, dev=dev)
+    train_step(model, video, ids, mask)
     peak_off = _step_peak(model, video, ids, mask)
     model.clipmodel.gradient_checkpointing_enable()
     peak_on = _step_peak(model, video, ids, mask)
@@ -231,12 +167,12 @@ def test_checkpointing_halves_peak_memory(dev):
 
 
 def test_checkpointing_is_ignored_in_eval_mode(dev):
-    model = _model(dev, 2, 2)
-    video, ids, mask = _inputs(dev, 4, 12, 24)
+    model = _model(dev, b16(2, 2))
+    video, ids, mask = ragged_batch(4, 12, 24, dev=dev)
     model.eval()
-    _step(model, video, ids, mask)
+    train_step(model, video, ids, mask)
     kept_off = _kept_by_forward(model, video, ids, mask)
-    off = _step(model, video, ids, mask)
+    off = train_step(model, video, ids, mask)
     model.clipmodel.gradient_checkpointing_enable()
     kept_on = _kept_by_forward(model, video, ids, mask)
     out = model(video=video, text_input_ids=ids, text_input_mask=mask)
@@ -244,7 +180,7 @@ def test_checkpointing_is_ignored_in_eval_mode(dev):
     for sv in (ctx.vis, ctx.txt):
         assert sv.recompute is None and all(isinstance(s, tuple) for s in sv.layers)
     del out, ctx, sv
-    on = _step(model, video, ids, mask)
+    on = train_step(model, video, ids, mask)
     # the same tensors are saved (checked above); two readings of the same code path are not exact to the byte (they have
     # differed by 0.2 MiB), which is far below one block's saved state (about 260 MiB here)
     assert abs(kept_on - kept_off) <= 2**20, (kept_on, kept_off)
@@ -254,15 +190,15 @@ def test_checkpointing_is_ignored_in_eval_mode(dev):
 
 
 def test_checkpointing_hands_over_the_same_gradient_buffers(dev):
-    model = _model(dev, 2, 2)
-    video, ids, mask = _inputs(dev, 4, 12, 24)
+    model = _model(dev, b16(2, 2))
+    video, ids, mask = ragged_batch(4, 12, 24, dev=dev)
     cm = model.clipmodel
     seen = {}
     for mode in ("off", "on"):
         (cm.gradient_checkpointing_enable if mode == "on" else cm.gradient_checkpointing_disable)()
         rec = seen[mode] = []
         cm.grad_ready_hook = lambda flat: rec.append(flat.detach().clone())
-        _step(model, video, ids, mask)
+        train_step(model, video, ids, mask)
     cm.grad_ready_hook = None
     assert [t.numel() for t in seen["on"]] == [t.numel() for t in seen["off"]]
     assert len(seen["off"]) == 2 * 2 + 2                  # one per layer, then the rest of each tower

@@ -25,15 +25,13 @@ These cases are separate tests from the reference-golden comparisons of test_gpu
 test_gpu_frame_clip.py: those compare with the real reference's numbers and its own bf16 runs, these with the fp32 oracle
 and the module's rounding; one failing does not hide the other.  The arm and the rule live in clipvip_arm.py.
 """
-import os
-
 import pytest
 import torch
 
 from clipvip_arm import features_objective, oracle_run, rule_violations
+from clipvip_cases import b16, load_golden, module_config
 from contract_harness import Report
 from oracle import clipvip_oracle as O
-from oracle import frame_clip_oracle as FC
 
 pytestmark = pytest.mark.gpu
 
@@ -53,17 +51,6 @@ def dev():
 def _report():
     yield
     REPORT.print()
-
-
-def module_config(cfg, stream="fp32", per_frame=False, temporal=True):
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    return ClipVipConfig(vision=TowerConfig(cfg.vision.width, cfg.vision.heads, cfg.vision.layers, cfg.vision.mlp),
-                         text=TowerConfig(cfg.text.width, cfg.text.heads, cfg.text.layers, cfg.text.mlp),
-                         image_size=cfg.image_size, patch_size=cfg.patch, projection_dim=cfg.proj_dim,
-                         vocab_size=cfg.vocab, max_position_embeddings=cfg.max_text_pos, layer_norm_eps=cfg.ln_eps,
-                         residual_fp32=stream != "bf16", residual_dtype="fp16" if stream == "fp16" else "fp32",
-                         temporal_size=cfg.temporal_size, if_use_temporal_embed=int(temporal), add_cls_num=cfg.add_cls_num,
-                         logit_scale_init_value=cfg.logit_scale_init, vision_type="meanP" if per_frame else "ViP")
 
 
 def normalised_frames(u8):
@@ -117,41 +104,6 @@ def clipvip_case(dev, tag, cfg, sd, video, ids, mask, streams=("fp32",), per_fra
 
 
 # ========================================================================================================== cases
-def b16(v_layers, t_layers, **kw):
-    return O.ClipVipCfg(vision=O.TowerCfg(768, 12, v_layers, 3072), text=O.TowerCfg(512, 8, t_layers, 2048), **kw)
-
-
-def l14(image_size, v_layers, t_layers):
-    return O.ClipVipCfg(vision=O.TowerCfg(1024, 16, v_layers, 4096), text=O.TowerCfg(768, 12, t_layers, 3072),
-                        image_size=image_size, patch=14, proj_dim=768)
-
-
-def golden_inputs(golden_dir, name, frame_clip=False):
-    """(cfg, state dict, video, ids, mask) of a golden's seeds, its ids and (where it stores one) video checksum checked
-    against the golden."""
-    gold = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
-    meta = gold["meta"]
-    if frame_clip:
-        if meta["vision_width"] == 1024:
-            cfg = l14(meta["image_size"], meta["vision_layers"], meta["text_layers"])
-            cfg.patch = meta["patch"]
-        else:
-            cfg = b16(meta["vision_layers"], meta["text_layers"], image_size=meta["image_size"], patch=meta["patch"])
-        sd = FC.init_state_dict(cfg, seed=meta["weight_seed"])
-    else:
-        if "image_size" in meta and meta.get("patch", 16) == 14:
-            cfg = l14(meta["image_size"], meta["vision_layers"], meta["text_layers"])
-        else:
-            cfg = b16(meta["vision_layers"], meta["text_layers"])
-        sd = O.init_state_dict(cfg, seed=meta["weight_seed"])
-    video, ids, mask = O.synthetic_batch(meta["B"], meta["T"], meta["Lt"], cfg, seed=meta["data_seed"],
-                                         ragged_text=meta.get("ragged", True))
-    assert torch.equal(ids, gold["input_ids"])
-    if "video_checksum" in gold:
-        assert abs(float(video.double().sum()) - gold["video_checksum"]) < 1e-6
-    return cfg, sd, video, ids, mask
-
-
 GOLDEN_CASES = {  # name: (golden, streams, per frame)
     "b16_depth2_ragged": ("depth2_b3_t12_ragged", ("fp32", "fp16", "bf16"), False),
     "b16_cfg1_t4": ("cfg1_b2_t4", ("fp32",), False),
@@ -166,7 +118,7 @@ GOLDEN_CASES = {  # name: (golden, streams, per frame)
 
 def golden_case(dev, golden_dir, name, pad_to=None):
     golden, streams, per_frame = GOLDEN_CASES[name]
-    cfg, sd, video, ids, mask = golden_inputs(golden_dir, golden, frame_clip=per_frame)
+    _, cfg, sd, video, ids, mask = load_golden(golden_dir, golden)
     pad = None
     if pad_to is not None:
         pad = O.synthetic_batch(pad_to - ids.shape[0], video.shape[1], ids.shape[1], cfg, seed=777, ragged_text=True)

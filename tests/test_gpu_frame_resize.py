@@ -15,12 +15,11 @@ resize, pinned on the CPU by test_frame_resize_cpu.py, and through every model e
                fp32 oracle on those frames; gradient checkpointing leaves loss and features bit-identical; float frames of
                another size raise ValueError before any launch
 """
-from types import SimpleNamespace
-
 import pytest
 import torch
 
 from clipvip_arm import features_objective, oracle_run, rule_violations
+from clipvip_cases import b16, l14, module_config, vidclip
 from contract_harness import Guarded, Report, same_bits
 from oracle import clipvip_oracle as O
 from oracle import embed_ref as EMB
@@ -181,21 +180,10 @@ def test_refusals_launch_nothing(dev, case):
 
 
 # ========================================================================================================= model
-def _module_config(cfg, per_frame):
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    return ClipVipConfig(vision=TowerConfig(cfg.vision.width, cfg.vision.heads, cfg.vision.layers, cfg.vision.mlp),
-                         text=TowerConfig(cfg.text.width, cfg.text.heads, cfg.text.layers, cfg.text.mlp),
-                         image_size=cfg.image_size, patch_size=cfg.patch, projection_dim=cfg.proj_dim,
-                         vocab_size=cfg.vocab, max_position_embeddings=cfg.max_text_pos, layer_norm_eps=cfg.ln_eps,
-                         temporal_size=cfg.temporal_size, add_cls_num=cfg.add_cls_num,
-                         logit_scale_init_value=cfg.logit_scale_init, vision_type="meanP" if per_frame else "ViP")
-
-
 MODELS = {  # name: (oracle config, per frame, B, T)
-    "vip_b16_t12": (O.ClipVipCfg(vision=O.TowerCfg(768, 12, 2, 3072), text=O.TowerCfg(512, 8, 1, 2048)), False, 2, 12),
-    "frame_b16": (O.ClipVipCfg(vision=O.TowerCfg(768, 12, 2, 3072), text=O.TowerCfg(512, 8, 1, 2048)), True, 2, 3),
-    "vip_l14_336": (O.ClipVipCfg(vision=O.TowerCfg(1024, 16, 1, 4096), text=O.TowerCfg(768, 12, 1, 3072), image_size=336,
-                                 patch=14, proj_dim=768), False, 2, 2),
+    "vip_b16_t12": (b16(2, 1), False, 2, 12),
+    "frame_b16": (b16(2, 1), True, 2, 3),
+    "vip_l14_336": (l14(336, 1, 1), False, 2, 2),
 }
 
 
@@ -203,7 +191,7 @@ def _setup(dev, name, seed=0):
     from xpretrain_b200.modeling.clip_vip import CLIPModel
     cfg, per_frame, B, T = MODELS[name]
     sd = (FC if per_frame else O).init_state_dict(cfg, seed=seed)
-    model = CLIPModel(_module_config(cfg, per_frame))
+    model = CLIPModel(module_config(cfg, per_frame=per_frame))
     missing, unexpected = model.load_state_dict(sd, strict=False)
     assert not missing and not unexpected, (missing, unexpected)
     _, ids, mask = O.synthetic_batch(B, T, 16, cfg, seed=seed + 1, ragged_text=True)
@@ -264,14 +252,8 @@ def test_per_frame_model_takes_4d_uint8_images(dev, monkeypatch):
 
 
 def test_image_branch_takes_uint8_frames(dev, monkeypatch):
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
     cfg, sd, _, frames, transformed, ref, ids, mask = _setup(dev, "vip_b16_t12")
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 2, 3072), text=TowerConfig(512, 8, 1, 2048))
-    vid = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    vid.clipmodel.load_state_dict(sd, strict=False)
-    vid = vid.to(dev)
+    vid = vidclip(cfg, sd=sd, dev=dev)
     image, image_f = frames[:, :1].contiguous(), transformed[:, :1].contiguous()    # [B, 1, H, W, 3] / [B, 1, 3, S, S]
     cap = _Captured(monkeypatch)
     with torch.no_grad():

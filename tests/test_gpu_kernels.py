@@ -184,13 +184,8 @@ def test_uint8_frames_preprocessing_bit_exact_vs_reference_transform(dev):
     ops.vip_patchify_u8(frames.to(dev), patches, 16)
     assert torch.equal(patches.cpu(), ref_p)
     # and the model accepts the raw frames: same features as feeding the reference-transformed float video
-    from types import SimpleNamespace
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-    torch.manual_seed(0)
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add)).to(dev)
+    from clipvip_cases import b16, vidclip
+    model = vidclip(b16(1, 1), seed=0, dev=dev)
     with torch.no_grad():
         a = model.forward_video(frames.to(dev))
         b = model.forward_video(img.reshape(B, T, 3, H, W).to(dev))

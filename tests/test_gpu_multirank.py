@@ -27,17 +27,10 @@ def _rel(a, b):
 
 
 def _build(dev, layers=1):
-    from types import SimpleNamespace
+    from clipvip_cases import b16, vidclip
     from oracle import clipvip_oracle as O
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    cfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, layers, 3072), text=O.TowerCfg(512, 8, layers, 2048))
-    sd = O.init_state_dict(cfg, seed=2)
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, layers, 3072), text=TowerConfig(512, 8, layers, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    model.clipmodel.load_state_dict(sd, strict=False)
-    return O, cfg, model.to(dev)
+    cfg = b16(layers, layers)
+    return O, cfg, vidclip(cfg, sd=O.init_state_dict(cfg, seed=2), dev=dev)
 
 
 def _worker(rank, world, port, b, q):

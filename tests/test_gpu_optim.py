@@ -99,19 +99,13 @@ def test_no_cpu_path():
 def test_training_step_on_the_dual_encoder_matches_the_oracle_update(dev):
     """fwd + InfoNCE + bwd + fused clip + AdamW on VidCLIP (depth 1): every parameter moves exactly as adamw.py says for
     the gradients the backward produced, and the next forward really uses the updated weights (bf16 copies refreshed)."""
-    from types import SimpleNamespace
-
+    from clipvip_cases import b16, vidclip
     from oracle import clipvip_oracle as O
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    from xpretrain_b200.modeling.vidclip import VidCLIP
     from xpretrain_b200.optimization import build_loss_func
     from xpretrain_b200.optimization.adamw import AdamW, build_e2e_optimizer_w_lr_mul
 
-    ocfg = O.ClipVipCfg(vision=O.TowerCfg(768, 12, 1, 3072), text=O.TowerCfg(512, 8, 1, 2048))
-    add = SimpleNamespace(type="ViP", temporal_size=ocfg.temporal_size, if_use_temporal_embed=1,
-                          logit_scale_init_value=ocfg.logit_scale_init, add_cls_num=ocfg.add_cls_num)
-    cfg = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-    model = VidCLIP(SimpleNamespace(clip_config=cfg, clip_weights="", clip_vision_additional_config=add)).to(dev)
+    ocfg = b16(1, 1)
+    model = vidclip(ocfg, dev=dev)
     video, ids, mask = O.synthetic_batch(8, 2, 16, ocfg, seed=3)
     video, ids, mask = video.to(dev), ids.to(dev), mask.to(dev)
     loss_fn = build_loss_func({"loss_name": "NCELearnableTempLoss"})

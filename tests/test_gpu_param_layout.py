@@ -8,6 +8,7 @@ from types import SimpleNamespace
 import pytest
 import torch
 
+from clipvip_cases import b16, vidclip
 from contract_harness import same_bits
 
 pytestmark = pytest.mark.gpu
@@ -25,11 +26,7 @@ SWIN = dict(embed_dim=64, depths=[2, 2], num_heads=[2, 4], stages=[0, 1], downsa
 
 
 def _clip_vip(tmp):
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type="ViP", temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6, add_cls_num=3)
-    mc = ClipVipConfig(vision=TowerConfig(768, 12, 1, 3072), text=TowerConfig(512, 8, 1, 2048))
-    return VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
+    return vidclip(b16(1, 1))
 
 
 def _clip_vip_inputs(dev, g):

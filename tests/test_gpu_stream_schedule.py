@@ -34,11 +34,11 @@ masks, offsets, pointer tables or workspace counters early.  No case loops waiti
 number of hook groups.
 """
 import collections
-from types import SimpleNamespace
 
 import pytest
 import torch
 
+from clipvip_cases import b16, l14, ragged_batch, vidclip
 from contract_harness import GRAD_REL, reordering_violations, same_bits
 
 pytestmark = pytest.mark.gpu
@@ -176,36 +176,14 @@ class _Hook:
 
 
 # ------------------------------------------------------------------------------------------------------ CLIP-ViP cases
-def _model(dev, v_layers=2, t_layers=2, stream="fp32", large=False, vision_type="ViP", seed=0):
-    from xpretrain_b200.modeling import VidCLIP
-    from xpretrain_b200.modeling.clip_vip import ClipVipConfig, TowerConfig
-    add = SimpleNamespace(type=vision_type, temporal_size=12, if_use_temporal_embed=1, logit_scale_init_value=4.6,
-                          add_cls_num=3)
-    if large:
-        mc = ClipVipConfig(vision=TowerConfig(1024, 16, v_layers, 4096), text=TowerConfig(768, 12, t_layers, 3072),
-                           patch_size=14, projection_dim=768)
-    else:
-        mc = ClipVipConfig(vision=TowerConfig(768, 12, v_layers, 3072), text=TowerConfig(512, 8, t_layers, 2048))
-    mc.residual_fp32, mc.residual_dtype = stream != "bf16", ("fp16" if stream == "fp16" else "fp32")
-    torch.manual_seed(seed)
-    model = VidCLIP(SimpleNamespace(clip_config=mc, clip_weights="", clip_vision_additional_config=add))
-    if vision_type == "ViP":
-        with torch.no_grad():
-            model.clipmodel.vision_model.embeddings.temporal_embedding.normal_(0, 0.02)
-    return model.to(dev)
+def _model(dev, cfg=None, stream="fp32", per_frame=False):
+    """B/16 at depth 2 unless `cfg` says otherwise; the ViP tower with its temporal table redrawn."""
+    return vidclip(cfg or b16(2, 2), stream=stream, per_frame=per_frame, seed=0, temporal_init=not per_frame, dev=dev)
 
 
 def _batch(dev, B=4, T=12, Lt=12, seed=1):
-    """Video [B, T, 3, 224, 224] and ragged text: EOS, then padding with mask 0."""
-    g = torch.Generator().manual_seed(seed)
-    video = torch.randn(B, T, 3, 224, 224, generator=g)
-    ids = torch.randint(1, 49406, (B, Lt), generator=g)
-    mask = torch.ones(B, Lt, dtype=torch.long)
-    eos = torch.randint(2, Lt, (B,), generator=g)
-    for b in range(B):
-        ids[b, eos[b]:] = 49407
-        mask[b, eos[b] + 1:] = 0
-    return {"video": video.to(dev), "text_input_ids": ids.to(dev), "text_input_mask": mask.to(dev)}
+    video, ids, mask = ragged_batch(B, T, Lt, seed=seed, dev=dev)
+    return {"video": video, "text_input_ids": ids, "text_input_mask": mask}
 
 
 def _image_batch(dev, B=4, Lt=12, seed=2):
@@ -305,8 +283,8 @@ CASES = {   # name: (model kwargs, batch kwargs, setup, modes, train)
     "bf16_stream": ({"stream": "bf16"}, {}, None, ALL, True),
     "frozen_text": ({}, {}, "frozen", ALL, True),
     "sm_reserve8": ({}, {}, "reserve", ALL, True),
-    "per_frame_clip": ({"vision_type": "meanP"}, {}, None, ALL, True),
-    "vit_l14_224_d1": ({"large": True, "v_layers": 1, "t_layers": 1}, {}, None, ALL, True),
+    "per_frame_clip": ({"per_frame": True}, {}, None, ALL, True),
+    "vit_l14_224_d1": ({"cfg": l14(224, 1, 1)}, {}, None, ALL, True),
     "image_caption": ({}, {}, "image", ALL, True),
 }
 
@@ -336,7 +314,7 @@ def test_bench_configuration_schedule(dev, delay, cycles_per_ms):
     each other, so that the bound has room above the run-to-run reordering (measured 9.0e-7 and 1.02e-6 of the scale in two
     runs on an H100 80GB HBM3 at 700 W, about 10x inside; the overlapped-against-serial comparisons of the small cases
     reach 1.3e-6)."""
-    model = _model(dev, 12, 12)
+    model = _model(dev, b16(12, 12))
     batch = _batch(dev, B=64, T=12, Lt=32)
     ref_out, ref_g = _clip_case(delay, cycles_per_ms, "bench_b64_12+12", model, batch, ["none", "side", "aux"])
     outs, grads, hook_bad, _, _ = _clip_run(delay, model, batch, "none", {}, False)
