@@ -194,6 +194,21 @@ int xp_vip_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t fr
  * patches_bf16 not 16-byte aligned.  frames_hwc may have any alignment. */
 int xp_vip_resize_patchify_u8(const uint8_t* frames_hwc, void* patches_bf16, int64_t frames, int32_t H, int32_t W, int32_t S,
                               int32_t patch, const float* mean3, const float* std3, void* stream);
+/* LF-VILA's input transform (init_transform_dict, LF-VILA/src/datasets/dataloader.py:94-121, as torchvision 0.11 runs it
+ * on float tensors) fused into Swin-3D's patch extraction.  frames_hwc uint8 [clips, N, H, W, 3]; params int32 [clips, 5]
+ * (device) = top, left, h, w, flip per clip.  Per frame: /255, resize to Ha x Wa (stage A), crop the box (top, left, h, w),
+ * resize the box to Ho x Wo (stage B, taps clamped to the box), mirror the columns if flip != 0, Normalize, one rounding to
+ * bf16.  Both resizes are F.interpolate(mode="bilinear", align_corners=False) without antialias, with torch's fp32 source
+ * coordinate (one rounding: a fused multiply-add); the composite weights are float64 rounded to fp32, accumulated in fp32
+ * in a fixed order (bitwise repeatable).  Writes exactly the clips*N*(Ho/8)*(Wo/8) x 192 patch matrix xp_vip_patchify
+ * writes for the transformed video: rows (clip, frame, h, w), columns (c, kh, kw).  mean3 / std3 are HOST arrays of 3
+ * floats.  Refused before any launch: H, W, Ha, Wa, Ho or Wo outside [1, 4096], patch != 8, Ho or Wo not a multiple of 8,
+ * a patches_bf16 not 16-byte aligned.  Boxes are the caller's to validate (0 <= top, 1 <= h, top + h <= Ha, likewise
+ * left / w / Wa); every tap is clamped to the frame, so an invalid box reads nothing outside it.  frames_hwc may have any
+ * alignment. */
+int xp_lfvila_frames_patchify_u8(const uint8_t* frames_hwc, const int32_t* params, void* patches_bf16, int32_t clips,
+                                 int32_t N, int32_t H, int32_t W, int32_t Ha, int32_t Wa, int32_t Ho, int32_t Wo,
+                                 int32_t patch, const float* mean3, const float* std3, void* stream);
 /* CLIP_ViP.py:170-176,183-195: table[t*L+l] = interp(temporal_embedding)[t] + position_embedding[1+l] (bf16,
  * [T*L, C]) and the M = 1 + add_cls_num global rows x[b, m] = (class_embedding | added_cls[m-1]) + position_embedding[0]
  * written into x_bf16 [B, M+T*L, C].  temporal may be NULL (if_use_temporal_embed = 0); added is read only when M > 1.

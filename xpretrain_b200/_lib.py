@@ -110,6 +110,8 @@ SIGNATURES = {
     "xp_vip_patchify_u8": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, P(c_float), P(c_float), c_void_p]),
     "xp_vip_resize_patchify_u8": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, P(c_float), P(c_float),
                                           c_void_p]),
+    "xp_lfvila_frames_patchify_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                             c_int, c_int, c_int, P(c_float), P(c_float), c_void_p]),
     "xp_vip_embed_tables": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                     c_int, c_int, c_int, c_void_p]),
     "xp_vip_embed_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,

@@ -4,7 +4,8 @@ Drop-in for `LFVILA_Video_Classification` of LF-VILA/src/models/lfvila_video_cla
 `(args, config)` (`config.VideoEncoder`, `config.bert_config` read for `hidden_size`, `config.DATA.classification_labels`),
 the same `state_dict()` (`video_encoder.*` of modeling/swin3d.py, `video_global_proj.*`, `video_frame_proj.*`,
 `classifier.*`; the max-pool holds nothing), and the same `forward(video_frames, labels) -> dict(video_global_feat,
-video_frame_feat, prediction, loss, acc)`.
+video_frame_feat, prediction, loss, acc)`.  `forward` also takes decord's uint8 frames `[B, N, H, W, 3]` and an optional
+`crops=` (modeling/lfvila_frames.py): the datasets' transform to `config.DATA.input_res` then runs on the GPU.
 
 The encoder call is modeling/swin3d.py's, unchanged.  The head after it runs as ONE autograd.Function:
   * xp_lfvila_pool_fwd: MaxPool2d((2, 3), stride 1) over each frame's Hp x Wp grid, the frame means `video_frame_feat`
@@ -21,13 +22,14 @@ pool on its fp16 output).  There is no CPU path.
 from __future__ import annotations
 
 import json
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
 from .. import _lib, ops
 from ._weights import ParamLayout, param_layout
+from .lfvila_frames import INPUT_RES, Crops
 from .swin3d import SwinTransformer3D
 
 bf16, f32 = torch.bfloat16, torch.float32
@@ -54,6 +56,7 @@ class LFVILA_Video_Classification(nn.Module):
         self.video_global_proj = nn.Linear(hidden, hidden)
         self.video_frame_proj = nn.Linear(hidden, hidden)
         self.n_labels = int(_get(_get(config, "DATA"), "classification_labels"))
+        self.input_res = tuple(int(v) for v in _get(_get(config, "DATA"), "input_res", INPUT_RES))   # uint8 input only
         self.classifier = nn.Linear(hidden, self.n_labels)
 
     def _declare_layout(self) -> ParamLayout:
@@ -62,7 +65,10 @@ class LFVILA_Video_Classification(nn.Module):
         return ParamLayout(self, exclude=("video_encoder.",), cast=lambda n, p: n.endswith(".weight") or n == "classifier.bias",
                            pad8=("classifier.weight", "classifier.bias"))
 
-    def forward(self, video_frames: torch.Tensor, labels=None):
+    def forward(self, video_frames: torch.Tensor, labels=None, crops: Optional[Crops] = None):
+        """video_frames: the transformed float video [B, 3, N, H, W], or decoder's uint8 frames [B, N, H, W, 3], transformed
+        to config.DATA.input_res as LF-VILA's datasets do: with `crops` (lfvila_frames.train_crops) while training, the
+        val / test transform when crops is None."""
         if not isinstance(labels, torch.Tensor):
             # nn.CrossEntropyLoss()(logits, labels) raises this for labels=None (:58-59)
             raise TypeError(f"cross_entropy_loss(): argument 'target' (position 2) must be Tensor, not "
@@ -73,7 +79,7 @@ class LFVILA_Video_Classification(nn.Module):
         if labels.dtype != torch.int64 or labels.dim() != 1 or labels.shape[0] != video_frames.shape[0]:
             raise ValueError(f"labels must be int64 class indices of shape [{video_frames.shape[0]}] (got {labels.dtype} "
                              f"{list(labels.shape)})")
-        video_embd, _ = self.video_encoder(video_frames)                  # [B, N, H, W, C]
+        video_embd, _ = self.video_encoder(video_frames, crops=crops, out_size=self.input_res)      # [B, N, H, W, C]
         g, fr, pred, loss, acc = _HeadFunction.apply(self, torch.is_grad_enabled(), video_embd,
                                                      labels.to(video_embd.device), *param_layout(self).params)
         return dict(video_global_feat=g, video_frame_feat=fr, prediction=pred, loss=loss, acc=acc)

@@ -6,7 +6,8 @@ Drop-in for `SwinTransformer3D` of LF-VILA/src/models/video_encoder.py:450-620 a
 
 The module tree only holds parameters; forward/backward run as ONE autograd.Function over token-major bf16 matrices
 `[B*D*H*W, C]` (rows in the reference's channels-last (b, d, h, w) order):
-  * PatchEmbed3D (:431-448): im2col (`xp_vip_patchify`) + wgmma GEMM + LayerNorm;
+  * PatchEmbed3D (:431-448): im2col (`xp_vip_patchify`; for uint8 frames `xp_lfvila_frames_patchify_u8`, which fuses the
+    LF-VILA datasets' resize / crop / flip / Normalize in) + wgmma GEMM + LayerNorm;
   * every block (:209-268): LayerNorm -> fused-qkv GEMM -> window attention -> proj GEMM (+residual) -> LayerNorm -> MLP GEMMs
     (erf-GELU epilogue, +residual).  The reference's F.pad / torch.roll / window_partition / window_reverse / crop copies (:214-243)
     do not exist: the attention kernel (`xp_seg_attention_*` in its indexed mode) reads and writes token rows through an index
@@ -26,7 +27,7 @@ from __future__ import annotations
 
 from functools import reduce
 from operator import mul
-from typing import Dict, NamedTuple
+from typing import Dict, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -35,6 +36,7 @@ import torch.nn.functional as F
 from .. import _lib, ops
 from ._blocks import drop_scale, layernorm, layernorm_bwd, linear_bwd, mlp_bwd, mlp_fwd, residual_linear
 from ._weights import ParamLayout, matrix_weight, param_layout
+from .lfvila_frames import INPUT_RES, Crops, eval_crops
 
 bf16, f32 = torch.bfloat16, torch.float32
 HEAD_DIM = 32
@@ -163,18 +165,32 @@ class SwinTransformer3D(nn.Module):
                              for _ in range(2)))
         return out
 
-    def forward(self, x: torch.Tensor, only_local: bool = False):
+    def forward(self, x: torch.Tensor, only_local: bool = False, crops: Optional[Crops] = None,
+                out_size: Tuple[int, int] = INPUT_RES):
+        """x: the transformed float video [B, 3, D, H, W], or decoder's uint8 frames [B, D, H, W, 3], which are transformed
+        as LF-VILA's datasets do (modeling/lfvila_frames.py) to out_size while their patches are extracted: with `crops`
+        (train_crops while training), or the val / test transform when crops is None."""
         if not x.is_cuda:
             raise _lib.XpError("xpretrain_b200 SwinTransformer3D needs CUDA tensors on an H100: there is no CPU path")
         if only_local:
             raise NotImplementedError("only_local=True (the early local_feat return, :604-605) is not built")
+        u8 = None
+        if x.dtype == torch.uint8:
+            if x.dim() != 5 or x.shape[-1] != 3:
+                raise ValueError(f"uint8 video must be decoded frames [B, D, H, W, 3] (got {list(x.shape)})")
+            if self.patch_size[1:] != [8, 8] or out_size[0] % 8 or out_size[1] % 8:
+                raise ValueError(f"uint8 video needs the 8 x 8 patch and an output size divisible by it (got patch "
+                                 f"{self.patch_size[1:]}, out_size {tuple(out_size)})")
+            u8 = (eval_crops(x.shape[0]) if crops is None else crops, tuple(out_size))
+        elif crops is not None:
+            raise ValueError("crops apply to uint8 frames [B, D, H, W, 3]; float video is already transformed")
         masks = None
         if self.training and self.drop_path_rate > 0:
             masks = self.forced_drop_masks if self.forced_drop_masks is not None else \
-                self.draw_drop_masks(x.shape[0], x.device, x.dtype)
+                self.draw_drop_masks(x.shape[0], x.device, f32 if u8 else x.dtype)
         # torch.is_grad_enabled() of the caller: Function.forward always runs under no_grad, and needs_input_grad reflects
         # requires_grad even then, so without it evaluation under torch.no_grad() would keep every activation to the end
-        out = _Swin3DFunction.apply(self, masks, torch.is_grad_enabled(), x, *param_layout(self).params)
+        out = _Swin3DFunction.apply(self, masks, torch.is_grad_enabled(), u8, x, *param_layout(self).params)
         return out, out
 
 
@@ -333,25 +349,32 @@ def _block_bwd(w, p: str, blk: _Block, dx, saved, geo, shifted: bool, heads: int
 # ------------------------------------------------------------------------------------------- function
 class _Swin3DFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, model: SwinTransformer3D, masks, grad_mode: bool, video: torch.Tensor, *params):
-        B, Cin, D, Hin, Win = video.shape
+    def forward(ctx, model: SwinTransformer3D, masks, grad_mode: bool, u8, video: torch.Tensor, *params):
+        # u8: None for float video [B, 3, D, H, W]; (crops, (Ho, Wo)) for uint8 frames [B, D, H, W, 3]
         ph, pw = model.patch_size[1], model.patch_size[2]
-        if Cin != 3 or Hin % ph or Win % pw:
-            raise ValueError("video must be [B, 3, D, H, W] with H, W divisible by the patch size")
-        save = grad_mode and any(ctx.needs_input_grad[4:])
+        if u8 is None:
+            B, Cin, D, Hin, Win = video.shape
+            if Cin != 3 or Hin % ph or Win % pw:
+                raise ValueError("video must be [B, 3, D, H, W] with H, W divisible by the patch size")
+        else:
+            (B, D), (Hin, Win) = video.shape[:2], u8[1]
+        save = grad_mode and any(ctx.needs_input_grad[5:])
         w = param_layout(model)
         w.refresh()
         dev = video.device
         C0 = model.embed_dim
         # ---- PatchEmbed3D (:431-448): frames x (h, w) patches, rows already in (b, d, h, w) order
-        frames = video.permute(0, 2, 1, 3, 4).contiguous()               # [B, D, 3, H, W]
         H, W = Hin // ph, Win // pw
         rows = B * D * H * W
         K0 = 3 * ph * pw
         patches = torch.empty(rows, K0, dtype=bf16, device=dev)
         if ph != pw:
             raise NotImplementedError("square spatial patches only")
-        ops.vip_patchify(frames, patches, ph)
+        if u8 is None:
+            frames = video.permute(0, 2, 1, 3, 4).contiguous()           # [B, D, 3, H, W]
+            ops.vip_patchify(frames, patches, ph)
+        else:
+            ops.lfvila_frames_patchify_u8(video, u8[0].params, u8[0].stage_a, u8[1], patches, ph)
         w0 = w["patch_embed.proj.weight"].view(C0, K0)
         tok = torch.empty(rows, C0, dtype=bf16, device=dev)
         ops.linear_fwd(patches, w0, model.patch_embed.proj.bias, tok)
@@ -392,7 +415,7 @@ class _Swin3DFunction(torch.autograd.Function):
             geos.append(geo)
         Cl = tok.shape[1]
         outn, fm, fr = layernorm(tok, model.norm, wide=True)
-        out = outn.view(B, D, H, W, Cl).to(video.dtype)
+        out = outn.view(B, D, H, W, Cl).to(f32 if u8 else video.dtype)
         if save:
             ctx.model, ctx.geos = model, geos
             ctx.saved = (patches, pe_saved, layer_saved, (tok, fm, fr))
@@ -437,4 +460,4 @@ class _Swin3DFunction(torch.autograd.Function):
         ops.linear_wgrad(dtok, patches, grads["patch_embed.proj.weight"].view(C0, -1))
         ops.colsum(dtok, grads["patch_embed.proj.bias"])
         ctx.saved = None
-        return (None, None, None, None) + w.grads_out(grads, ctx.needs_input_grad[4:])
+        return (None, None, None, None, None) + w.grads_out(grads, ctx.needs_input_grad[5:])

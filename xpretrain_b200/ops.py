@@ -333,6 +333,37 @@ def vip_resize_patchify_u8(frames_hwc: torch.Tensor, patches: torch.Tensor, size
     _call("xp_vip_resize_patchify_u8", _p(frames_hwc), _p(patches), n, H, W, size, patch, m3, s3)
 
 
+IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)   # LF-VILA dataloader.py:94-99
+
+
+def lfvila_frames_patchify_u8(frames_hwc: torch.Tensor, params: torch.Tensor, stage_a, out_size, patches: torch.Tensor,
+                              patch: int = 8, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """frames_hwc uint8 [B, N, H, W, 3] -> Swin-3D's bf16 patch matrix [B*N*(Ho/8)*(Wo/8), 192] of the transformed video:
+    resize to stage_a = (Ha, Wa), crop the box params[b] = (top, left, h, w, flip) (a CPU int32 [B, 5] tensor), resize the
+    box to out_size = (Ho, Wo), mirror if flip, /255 + Normalize.  The boxes are checked here and uploaded without a device
+    synchronise."""
+    if frames_hwc.dtype != torch.uint8 or frames_hwc.dim() != 5 or frames_hwc.shape[-1] != 3:
+        raise ValueError(f"lfvila_frames_patchify_u8: frames must be uint8 [B, N, H, W, 3] (got {frames_hwc.dtype} "
+                         f"{list(frames_hwc.shape)})")
+    B, N, H, W, _ = frames_hwc.shape
+    (Ha, Wa), (Ho, Wo) = (int(v) for v in stage_a), (int(v) for v in out_size)
+    if params.device.type != "cpu" or params.dtype != torch.int32 or tuple(params.shape) != (B, 5):
+        raise _lib.XpError(f"lfvila_frames_patchify_u8: params must be a CPU int32 [{B}, 5] tensor (got {params.device} "
+                           f"{params.dtype} {list(params.shape)})")
+    top, left, h, w = (params[:, k] for k in range(4))
+    bad = (top < 0) | (left < 0) | (h < 1) | (w < 1) | (top + h > Ha) | (left + w > Wa)
+    if bool(bad.any()):
+        b = int(bad.nonzero()[0])
+        raise _lib.XpError(f"lfvila_frames_patchify_u8: clip {b}'s box {params[b, :4].tolist()} is not inside the "
+                           f"{Ha} x {Wa} stage-A image")
+    _aligned_output(patches, 16, "lfvila_frames_patchify_u8")
+    frames_hwc = aligned_input(frames_hwc)
+    dev_params = params.pin_memory().to(frames_hwc.device, non_blocking=True) if B else params
+    m3, s3 = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+    _call("xp_lfvila_frames_patchify_u8", _p(frames_hwc), dev_params.data_ptr(), _p(patches), B, N, H, W, Ha, Wa, Ho, Wo,
+          patch, m3, s3)
+
+
 def vip_embed_tables(pos, temporal, cls, added, table, x, B, T, L, M, C_, temporal_size):
     _call("xp_vip_embed_tables", _p(pos), _p(temporal), _p(cls), _p(added), _p(table), _p(x), B, T, L, M, C_, temporal_size)
 
